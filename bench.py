@@ -5,12 +5,20 @@ One "step" = one pass of the hot path over one batch of synthetic input:
     sample B (u,i,j) triples -> gather 3 rows -> score -> log-sigmoid grad -> scatter-add
 fused in ONE kernel launch (elliot_b200/csrc/bpr_train.cu, eb_bpr_step_sampled_f32).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
+
+--dump-outputs DIR: after the K timed steps, the tables the timed path leaves behind (what a caller of
+eb_bpr_step_sampled_f32 receives: the updated item factors and biases, a fixed seeded sample of user rows,
+the accumulated loss) are written as DIR/<name>.npy (float32 / float64), before anything else touches them.
+Inputs are seeded, so two builds run with the same arguments can be compared output for output: with
+--dump-outputs the timed steps run in deterministic rounds (--schedule auto), where only the fp32 order of one
+round's atomic adds to a shared row varies between runs.  Free-running Hogwild, the default otherwise, reads rows
+while other triples update them, so its tables differ from run to run by more than rounding.
 
 N>1 (torchrun, one rank per GPU): every rank owns its own shard of 1M users (weak scaling;
 user rows never leave their GPU), the 100K-item table is replicated and kept consistent with
 one NCCL all-reduce of the per-step item deltas (the path's only exchange step).
-Rank 0 prints ONE JSON line (contract in the task statement).
+Rank 0 prints ONE JSON result line.
 """
 import argparse
 import json
@@ -26,7 +34,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-# ---- workload: BASELINE.json configs[1] "BPRMF d=64 synthetic 1M x 100K interactions, 1xB200"
+# ---- workload: BASELINE.json configs[1] "BPRMF d=64 synthetic 1M x 100K interactions", one GPU
 N_USERS, N_ITEMS, D = 1_000_000, 100_000, 64
 PER_USER = 100
 BATCH = 1 << 22                      # triples per step
@@ -36,11 +44,26 @@ ALG_BYTES_MATERIALISED = ALG_BYTES_SAMPLED + 12
 
 
 def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 6650.0, 1590.0, "fallback"
+    """H100 SXM data-sheet peaks (700 W part): HBM3 3.35 TB/s, dense bf16 989 TFLOP/s.  Not reached figures: the
+    roofline fractions below are shares of these."""
+    return 3350.0, 989.0, "datasheet H100 SXM"
+
+
+DUMP_USER_ROWS = 65536                      # seeded sample of the 1M user rows written by --dump-outputs
+
+
+def dump_outputs(out_dir, U, V, b, loss, seed=1234):
+    """The timed path's outputs after its last step, as float32 / float64 .npy files (26 MB of V + b, 16 MB of sampled U)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    g = torch.Generator(device="cpu"); g.manual_seed(seed)
+    rows = torch.randperm(U.shape[0], generator=g)[:DUMP_USER_ROWS].sort().values
+    np.save(os.path.join(out_dir, "item_factors.npy"), V.float().cpu().numpy())
+    np.save(os.path.join(out_dir, "item_bias.npy"), b.float().cpu().numpy())
+    np.save(os.path.join(out_dir, "user_factors_sample.npy"), U[rows.to(U.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "user_factors_sample_rows.npy"), rows.numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "loss_sum.npy"), loss.double().cpu().numpy())
 
 
 class ClockSampler:
@@ -149,7 +172,7 @@ def cpu_baseline(indptr_h, indices_h, budget_s=12.0):
 
 def run_reference(args):
     """--impl reference: the reference's own CPU implementation of the path.  The reference is
-    pure Python and /root/reference is not on the GPU box, so this is the oracle port
+    pure Python and is not installed next to this package, so this is the oracle port
     (kind "port"): the interpreter-bound NumPy restatement with the reference's per-triple cost
     profile is the headline value; the (much faster) C port is reported beside it."""
     rank = int(os.environ.get("RANK", "0"))
@@ -253,7 +276,12 @@ def main():
                          "NCCL all-reduce in line (simple) or one step late beside the next step (overlap); auto = fastest in a "
                          "short untimed trial")
     ap.add_argument("--reserve-sms", type=int, default=12, help="N>1, overlap: SMs left to the NCCL kernel")
-    ap.add_argument("--blocks", default="all", help="comma list of extra blocks (scoring,c5,exact,large,vae,neumf,mf2020,sharded) or all/none")
+    ap.add_argument("--schedule", default="auto", choices=["auto", "hogwild", "rounds"],
+                    help="BPR step schedule: free-running Hogwild, or deterministic rounds (reads, grid barrier, atomic adds, grid "
+                         "barrier); auto = rounds with --dump-outputs, Hogwild otherwise")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the path's outputs (updated tables, loss) as DIR/<name>.npy")
+    ap.add_argument("--blocks", default="all", help="comma list of extra blocks (scoring,c5,exact,large,vae,neumf,mf2020,schedules,sharded) or all/none")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -313,12 +341,13 @@ def main():
     V.copy_(torch.randn(N_ITEMS, D, device=dev, generator=gv) * 0.1)
     b = items_flat[N_ITEMS * D:]; b.zero_()
     indptr, indices = synth_csr(torch, dev, seed=100 + rank)
-    # per-user membership signatures pay off on large catalogues (profiles/r2_hogwild_ab.json: +4 % at 2 M items, -10 % at C2's
-    # L2-resident 100 K items), so the C2 step runs without them
+    # per-user membership signatures pay off on large catalogues, not on C2's L2-resident 100 K items, so the C2 step runs
+    # without them
     filt = None
     loss = torch.zeros(1, dtype=torch.float64, device=dev)
     seed = 42 + rank
     counter = [0]
+    rounds = args.schedule == "rounds" or (args.schedule == "auto" and args.dump_outputs is not None)
     sm_total = ops.device_info()[0]
 
     # ---- N>1: schedules for the one exchange step (reconciliation of the replicated item table; deltas averaged)
@@ -343,7 +372,7 @@ def main():
 
     def step(reserve):
         ops.bpr_step_sampled_f32(U, V, b, D, N_USERS, N_ITEMS, indptr, indices, BATCH, seed, counter[0] * BATCH, *HP,
-                                 loss=loss, reserve_sms=reserve, filter=filt)
+                                 loss=loss, reserve_sms=reserve, filter=filt, deterministic=rounds)
         counter[0] += 1
 
     def run_steps(m, n, per_step_events=None):
@@ -393,6 +422,8 @@ def main():
         dist.barrier()
     kern_ms = sum(s.elapsed_time(e) for s, e in zip(ks, ke)) / K
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, U, V, b, loss)
     ms_total = allmax(ms_total)
     value = BATCH * K * world / (ms_total * 1e-3)
 
@@ -463,7 +494,7 @@ def main():
             dist.barrier()
 
     # ---- second half of the path: full-catalogue scoring + mask + top-10 on the tensor cores (+ device metrics)
-    S_USERS = 148 * 128 * 2
+    S_USERS = 132 * 128 * 2                                             # two 128-user blocks per H100 SM
 
     def blk_scoring():
         _, _, sst = ops.score_topk_tc(U, V, b, D, 10, indptr, indices, user_begin=0, n_sel=S_USERS)
@@ -484,7 +515,7 @@ def main():
         ev = res["ev"].cpu().tolist()
         fl = 2.0 * D * N_ITEMS * S_USERS
         return {"metric": "scored_users_per_sec", "value": S_USERS * world / (ms * 1e-3), "unit": "users/s", "ms": ms,
-                "config": {"workload": f"{S_USERS} users/GPU x {N_ITEMS} items, d={D}, k=10, bias + train mask, tcgen05 bf16 + exact fp32 re-rank",
+                "config": {"workload": f"{S_USERS} users/GPU x {N_ITEMS} items, d={D}, k=10, bias + train mask, wgmma bf16 + exact fp32 re-rank",
                            "rechecked_users": sst["rechecked"], "padded_k": sst["kp"]},
                 "with_device_metrics": {"value": S_USERS * world / (ms_ev * 1e-3), "unit": "users/s", "ndcg_at_10_rank0": ev[1] / max(ev[0], 1.0)},
                 "roofline": {"bound": "tensor", "achieved": fl / (ms * 1e-3) / 1e12, "executed": fl * sst["kp"] / D / (ms * 1e-3) / 1e12,
@@ -551,7 +582,7 @@ def main():
         ach = ALG_BYTES_SAMPLED * BATCH / (ms * 1e-3) / 1e9
         tr = traffic_of("bpr_hogwild_large")
         return {"metric": "bpr_triples_per_sec", "value": BATCH / (ms * 1e-3), "unit": "triples/s", "ms": ms,
-                "config": {"workload": f"{N_USERS} users x {LI} items (V = {LI * D * 4 >> 20} MB >> 126 MB L2), d={D}, {BATCH} triples/step"},
+                "config": {"workload": f"{N_USERS} users x {LI} items (V = {LI * D * 4 >> 20} MB >> 50 MB L2), d={D}, {BATCH} triples/step"},
                 "roofline": {"bound": "hbm", "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": ach / hbm, "traffic": tr,
                              "frac_dram_measured": None if tr is None else tr / (ms * 1e-3) / 1e9 / hbm},
                 "finite": bool(torch.isfinite(VL).all().item())}
@@ -578,15 +609,14 @@ def main():
             m.apply_grads()
         ms = timed(step3, 20, warm=3)
         fl = 3 * 2 * B3 * ni3 * 600 + 3 * 2 * B3 * 600 * 400 + 3 * 2 * B3 * 200 * 600     # fwd+bwd dense layers (input layer is a CSR gather)
-        sus = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("bf16_tflops_sustained", tflops) \
-            if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else tflops
+        sus = tflops
         adam_bytes = 28 * sum(v.numel() for v in m.P.values())
         return {"metric": "multivae_users_per_sec", "value": B3 * world / (ms * 1e-3), "unit": "users/s", "ms_per_step": ms,
                 "config": {"workload": f"configs[2]: MultiVAE 600/200, {nu3} x {ni3} (ML-20M shape, ~144 items/user), batch {B3}/GPU, dropout 0.5, "
-                                       "one native call per step phase (8 tcgen05 GEMMs + fused elementwise + dense Adam)",
+                                       "one native call per step phase (8 wgmma GEMMs + fused elementwise + dense Adam)",
                            "parallelism": "single GPU" if world == 1 else f"data parallel x{world}: ONE all-reduce of the flat gradient buffer"},
                 "roofline": {"bound": "tensor", "achieved": fl / (ms * 1e-3) / 1e12, "peak": sus, "unit": "TFLOP/s",
-                             "frac": fl / (ms * 1e-3) / 1e12 / sus, "peak_source": "bf16_tflops_sustained",
+                             "frac": fl / (ms * 1e-3) / 1e12 / sus, "peak_source": which,
                              "adam_hbm_floor_ms": adam_bytes / (hbm * 1e9) * 1e3},
                 "finite": bool(all(torch.isfinite(v).all().item() for v in m.P.values()))}
     block("vae", blk_vae)
@@ -677,6 +707,21 @@ def main():
     if world == 1:
         block("mf2020", blk_mf2020)
 
+    # ---- the C2 step under both schedules (on copies of the tables): what determinism costs
+    def blk_schedules():
+        Uc, Vc, bc = U.clone(), V.clone(), b.clone(); c = [0]
+        res = {}
+        for name, det in (("hogwild", False), ("rounds", True)):
+            def st():
+                ops.bpr_step_sampled_f32(Uc, Vc, bc, D, N_USERS, N_ITEMS, indptr, indices, BATCH, seed + 7, c[0] * BATCH, *HP,
+                                         deterministic=det)
+                c[0] += 1
+            ms = timed(st, 10, warm=3)
+            res[name] = {"ms_per_step": ms, "value": BATCH / (ms * 1e-3), "unit": "triples/s"}
+        return {"config": {"workload": "C2 step as in the headline, free-running Hogwild vs deterministic rounds"}, **res}
+    if world == 1:
+        block("schedules", blk_schedules)
+
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -695,15 +740,16 @@ def main():
         "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": f"C2: BPRMF d=64, 1M users x 100K items per GPU, ~100 train items/user, {BATCH} triples/step, "
-                               "fused sample+gather+score+grad+scatter kernel (Hogwild atomics)",
+                               "fused sample+gather+score+grad+scatter kernel, vector atomics, "
+                               + ("deterministic rounds" if rounds else "free-running Hogwild"),
                    "global_batch": BATCH * world, "parallelism": par,
                    "sync_schedule": {"chosen": chosen, "trial_ms": tune, "peer": peer_note, "partition": partition_note},
-                   "l2": "inputs larger than L2 (256 MB user table + 400 MB CSR per GPU vs 126 MB), fresh random rows every step"},
+                   "l2": "inputs larger than L2 (256 MB user table + 400 MB CSR per GPU vs 50 MB), fresh random rows every step"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm,
                      "traffic": traffic, "frac_dram_measured": None if traffic is None else traffic / (kern_ms * 1e-3) / 1e9 / hbm,
                      "peak_source": which, "kernel": "bpr_hogwild_kernel<64,SAMPLE,ATOMIC>", "kernel_ms": kern_ms,
                      "alg_bytes_per_triple": ALG_BYTES_SAMPLED,
-                     "note": "the 25.6 MB item table is L2-resident at C2, so DRAM moves fewer bytes than the algorithmic count; "
+                     "note": "the 25.6 MB item table fits the 50 MB L2 at C2, so DRAM moves fewer bytes than the algorithmic count; "
                              "the `large` block is the regime where the two agree"},
         "e2e": {"value": e2e_value, "unit": "triples/s", "h2d_bytes_per_step": 8 * BATCH, "d2h_bytes_per_step": 8,
                 "h2d_GBps_per_gpu": 8 * BATCH * K / (e2e_ms * 1e-3) / 1e9, "numa": numa,
@@ -712,7 +758,8 @@ def main():
         "seconds_total": round(time.time() - t_start, 1),
     }
     ren = {"scoring": "scoring", "c5": "scoring_c5_slice", "exact": "exact_c1", "large": "c2_large_catalog", "vae": "multivae_c3",
-           "neumf": "neumf_c4", "sharded": "sharded_bpr", "mf2020": "mf2020"}
+           "neumf": "neumf_c4", "sharded": "sharded_bpr", "mf2020": "mf2020",
+           "schedules": "c2_schedules"}
     for k, v in extra.items():
         out[ren[k]] = v
     if world == 1 and not args.no_cpu_baseline:
@@ -723,7 +770,7 @@ def main():
 
 
 def traffic_of(name):
-    """dram bytes per launch of a kernel from the committed ncu capture (profiles/traffic_<name>.json), or None."""
+    """dram bytes per launch of a kernel from a stored capture (profiles/traffic_<name>.json) if one exists, else None."""
     tp = os.path.join(ROOT, "profiles", f"traffic_{name}.json")
     if os.path.exists(tp):
         return json.load(open(tp)).get("dram_bytes_per_launch")

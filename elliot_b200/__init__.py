@@ -1,4 +1,4 @@
-"""elliot_b200 — B200-native core for Elliot's embedding-training hot path.
+"""elliot_b200 — H100 (sm_90a) core for Elliot's embedding-training hot path.
 
     from elliot_b200 import run_experiment            # mirrors elliot.run.run_experiment
     from elliot_b200.recommender import BPRMF         # mirrors elliot.recommender.BPRMF

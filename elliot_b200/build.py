@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library (elliot_b200/csrc/libelliot_b200.so) with nvcc for sm_100a.
+"""Build the C-ABI shared library (elliot_b200/csrc/libelliot_b200.so) with nvcc for sm_90a.
 
 In-tree, no torch dependency: the library exposes plain `extern "C"` entry points
 (include/elliot_b200.h) and is loaded with ctypes.  `python -m elliot_b200.build` rebuilds.
@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libelliot_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
          "-Xptxas", "-v", "-Wno-deprecated-gpu-targets"]
 

@@ -1,4 +1,4 @@
-// bpr_train.cu — fused BPR-MF training step kernels (sm_100a).
+// bpr_train.cu — fused BPR-MF training step kernels (sm_90a).
 //
 // Replaces MFModel.train_step/update_factors
 // (elliot/recommender/latent_factor_models/BPRMF/BPRMF_model.py:87-117) and, in the
@@ -14,6 +14,7 @@
 //    consistent with the array order of the triples: every row carries a turn counter,
 //    a triple waits until each of its three rows has seen exactly the touches that
 //    precede it in the sequence (ranks come from a radix sort of (row, position)).
+#include <cooperative_groups.h>
 #include <cub/cub.cuh>
 #include <stdlib.h>
 
@@ -107,8 +108,17 @@ struct Rows {
     float bi, bj;
 };
 
-template <int DP, bool SAMPLE, bool ATOMIC, bool PEER>
+// ROUNDS (opt-in, flags bit 6 / deterministic=True in ops) makes the step deterministic.  The launch is cooperative and runs in
+// rounds: every warp loads the rows of UNR triples per lane group, computes their updates from those values, the whole grid
+// waits, every warp adds its updates, the grid waits again.  A triple therefore reads exactly the values left by the
+// previous rounds — which round a triple falls into is fixed by its index and the grid size, not by timing — so the same
+// inputs give the same tables on every run (up to the order in which one round's atomic adds to a shared row land, i.e.
+// fp32 rounding).  Staleness stays bounded by one round (the grid's lane groups x UNR triples).  The barriers cost
+// throughput (the row loads of one round no longer overlap the previous round's atomics), so the default is free-running
+// Hogwild; rounds exist for local tables with atomic updates only.
+template <int DP, bool SAMPLE, bool ATOMIC, bool PEER, bool ROUNDS = false>
 __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p) {
+    static_assert(!ROUNDS || (ATOMIC && !PEER), "deterministic rounds: local tables, atomic updates");
     constexpr int NV = DP / 4;                 // float4 per row
     constexpr int G = NV >= 32 ? 32 : NV;      // lanes per triple
     constexpr int VPL = NV / G;                // float4 per lane
@@ -148,7 +158,10 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
         }
     };
 
-    for (int64_t tile = warp_id; tile * 32 < p.n; tile += nwarps) {
+    // ROUNDS: every warp runs the same number of iterations (idle ones with u = -1), so all of them reach every grid barrier
+    const int64_t n_tiles = (p.n + 31) / 32;
+    const int64_t tile_end = ROUNDS ? (n_tiles + nwarps - 1) / nwarps * nwarps : n_tiles;
+    for (int64_t tile = warp_id; tile < tile_end; tile += nwarps) {
         const int64_t t = tile * 32 + lane;
         int u = -1, i = 0, j = 0;
         if (t < p.n) {
@@ -178,6 +191,65 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
                 ti_[q] = __shfl_sync(0xffffffffu, i, gbase + s0 + q);
                 tj_[q] = __shfl_sync(0xffffffffu, j, gbase + s0 + q);
                 load_rows(rw[q], tu_[q], ti_[q], tj_[q]);
+            }
+            if constexpr (ROUNDS) {
+                // ---- read phase: scores and updates of this round's triples from the values the previous rounds left; each
+                // triple's updates overwrite its rows in rw (registers: the rows are dead once the updates are formed)
+#pragma unroll
+                for (int q = 0; q < UNR; q++) {
+                    Rows<VPL> &cur = rw[q];
+                    float part = 0.f;
+                    if (tu_[q] >= 0) {
+#pragma unroll
+                        for (int v = 0; v < VPL; v++) {
+                            part += cur.u[v].x * (cur.vi[v].x - cur.vj[v].x) + cur.u[v].y * (cur.vi[v].y - cur.vj[v].y) +
+                                    cur.u[v].z * (cur.vi[v].z - cur.vj[v].z) + cur.u[v].w * (cur.vi[v].w - cur.vj[v].w);
+                        }
+                    }
+#pragma unroll
+                    for (int off = G / 2; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
+                    if (tu_[q] >= 0) {
+                        const float x = part + (cur.bi - cur.bj);
+                        const float z = __fdividef(1.f, 1.f + __expf(x));  // BPRMF_model.py:98
+                        if (gl == 0) loss_acc += fmaxf(-x, 0.f) + __logf(1.f + __expf(-fabsf(x)));
+#pragma unroll
+                        for (int v = 0; v < VPL; v++) {
+                            const float4 a = cur.u[v], bi4 = cur.vi[v], bj4 = cur.vj[v];
+                            float4 du, un;
+                            du.x = p.lr * ((bi4.x - bj4.x) * z - p.reg_u * a.x);
+                            du.y = p.lr * ((bi4.y - bj4.y) * z - p.reg_u * a.y);
+                            du.z = p.lr * ((bi4.z - bj4.z) * z - p.reg_u * a.z);
+                            du.w = p.lr * ((bi4.w - bj4.w) * z - p.reg_u * a.w);
+                            un.x = a.x + du.x; un.y = a.y + du.y; un.z = a.z + du.z; un.w = a.w + du.w;
+                            // item rows see the UPDATED user row (view aliasing, BPRMF_model.py:92,109-116)
+                            cur.vi[v] = make_float4(p.lr * (un.x * z - p.reg_pos * bi4.x), p.lr * (un.y * z - p.reg_pos * bi4.y),
+                                                    p.lr * (un.z * z - p.reg_pos * bi4.z), p.lr * (un.w * z - p.reg_pos * bi4.w));
+                            cur.vj[v] = make_float4(p.lr * (-un.x * z - p.reg_neg * bj4.x), p.lr * (-un.y * z - p.reg_neg * bj4.y),
+                                                    p.lr * (-un.z * z - p.reg_neg * bj4.z), p.lr * (-un.w * z - p.reg_neg * bj4.w));
+                            cur.u[v] = du;
+                        }
+                        const float dbi = p.lr * (z - p.reg_b * cur.bi), dbj = p.lr * (-z - p.reg_b * cur.bj);
+                        cur.bi = dbi; cur.bj = dbj;
+                    }
+                }
+                cooperative_groups::this_grid().sync();      // every read of this round is done
+                // ---- write phase
+#pragma unroll
+                for (int q = 0; q < UNR; q++) {
+                    if (tu_[q] < 0) continue;
+                    float *pu = p.U + (int64_t)tu_[q] * ld, *pi, *pj, *pbi, *pbj;
+                    item_row(ti_[q], pi, pbi); item_row(tj_[q], pj, pbj);
+#pragma unroll
+                    for (int v = 0; v < VPL; v++) {
+                        const int e = (v * G + gl) * 4;
+                        red_add_v4(pu + e, rw[q].u[v]);
+                        red_add_v4(pi + e, rw[q].vi[v]);
+                        red_add_v4(pj + e, rw[q].vj[v]);
+                    }
+                    if (gl == 0) { red_add_f32(pbi, rw[q].bi); red_add_f32(pbj, rw[q].bj); }
+                }
+                cooperative_groups::this_grid().sync();      // every write of this round has landed before the next reads
+                continue;
             }
 #pragma unroll
             for (int q = 0; q < UNR; q++) {
@@ -440,8 +512,7 @@ static int launch_stage_t(const HogwildParams &p, int reserve_sms, cudaStream_t 
 }
 
 // Which kernel: flags bit 4 (16) forces the register-staged kernel, bit 5 (32) the shared-memory-staged one; otherwise the
-// measured default — on ONE local table the two are within 2 % of each other (profiles/r2_hogwild_ab.json: 0.99 vs 1.01 ms at C2,
-// 1.34 vs 1.37 ms at 2 M items) and the register kernel stays; with the item table spread over peer GPUs the staged kernel is the
+// default — on ONE local table the register kernel; with the item table spread over peer GPUs the staged kernel is the
 // default (`peer_default`): its row copies are in flight without holding registers while the rows cross NVLink.
 static bool use_stage(int dp, int flags, bool peer_default) {
     static const int env = [] { const char *e = getenv("EB_HOGWILD_STAGE"); return e ? atoi(e) : -1; }();
@@ -500,10 +571,10 @@ __global__ void __launch_bounds__(256) pointwise_sample_kernel(const HogwildPara
     }
 }
 
-template <int DP, bool SAMPLE, bool ATOMIC, bool PEER = false>
+template <int DP, bool SAMPLE, bool ATOMIC, bool PEER = false, bool ROUNDS = false>
 static int launch_hogwild_t(const HogwildParams &p, int reserve_sms, cudaStream_t st) {
     int per_sm = 0;
-    EB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER>, 256, 0));
+    EB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER, ROUNDS>, 256, 0));
     if (per_sm < 1) per_sm = 1;
     int64_t tiles = (p.n + 31) / 32;
     int64_t want = (tiles + 7) / 8;
@@ -512,14 +583,21 @@ static int launch_hogwild_t(const HogwildParams &p, int reserve_sms, cudaStream_
     int64_t grid = (int64_t)sms * per_sm;
     if (want < grid) grid = want;
     if (grid < 1) grid = 1;
-    bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER><<<(unsigned)grid, 256, 0, st>>>(p);
+    if (ROUNDS) {
+        // deterministic rounds (see bpr_hogwild_kernel): a cooperative launch, so every CTA is resident for the grid barriers
+        void *args[] = {const_cast<HogwildParams *>(&p)};
+        EB_CUDA(cudaLaunchCooperativeKernel((const void *)bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER, ROUNDS>, dim3((unsigned)grid),
+                                            dim3(256), args, 0, st));
+    } else {
+        bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER><<<(unsigned)grid, 256, 0, st>>>(p);
+    }
     EB_CUDA(cudaGetLastError());
     return EB_OK;
 }
 
 // EB_L2_PERSIST=1: mark the item table's address range as persisting in L2 for the launch's stream (cudaAccessPolicyWindow) when it
 // fits the device's persisting carve-out — the table is hit by two of every triple's three row accesses, the user table and the
-// CSR are streamed once.  An A/B switch: the measured effect decides the default (DESIGN.md §4.0).
+// CSR are streamed once.  An A/B switch, off by default.
 static void item_table_l2_window(const HogwildParams &p, cudaStream_t st) {
     static const int env = [] { const char *e = getenv("EB_L2_PERSIST"); return e ? atoi(e) : 0; }();
     if (!env || !p.V) return;
@@ -545,8 +623,18 @@ static void item_table_l2_window(const HogwildParams &p, cudaStream_t st) {
 template <bool SAMPLE>
 static int launch_hogwild(const HogwildParams &p, int dp, int flags, cudaStream_t st) {
     const bool atomic = !(flags & 1);
+    const bool rounds = (flags & 64) != 0;
     const int reserve = (flags >> 8) & 0xff;
     item_table_l2_window(p, st);
+    if (rounds) {
+        EB_ARG(atomic && !(flags & 32), "deterministic rounds run in the register kernel with atomic updates");
+#define EB_CASE(DPV) case DPV: return launch_hogwild_t<DPV, SAMPLE, true, false, true>(p, reserve, st);
+        switch (dp) {
+            EB_CASE(8) EB_CASE(16) EB_CASE(32) EB_CASE(64) EB_CASE(128) EB_CASE(256)
+            default: return set_err(EB_ERR_ARG, "row stride ld=%d must be one of 8,16,32,64,128,256 floats", dp);
+        }
+#undef EB_CASE
+    }
     if (use_stage(dp, flags, false)) {
         switch (dp) {
             case 32: return launch_stage_t<32, SAMPLE, false>(p, reserve, st);
@@ -569,6 +657,7 @@ static int launch_hogwild(const HogwildParams &p, int dp, int flags, cudaStream_
 template <bool SAMPLE>
 static int launch_hogwild_peer(const HogwildParams &p, int dp, int flags, cudaStream_t st) {
     const int reserve = (flags >> 8) & 0xff;
+    EB_ARG(!(flags & 64), "deterministic rounds exist for local tables only (other GPUs update peer rows concurrently)");
     if (use_stage(dp, flags, true)) {
         switch (dp) {
             case 32: return launch_stage_t<32, SAMPLE, true>(p, reserve, st);

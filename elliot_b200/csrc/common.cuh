@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for the sm_100a kernels behind include/elliot_b200.h
+// common.cuh — shared helpers for the sm_90a kernels behind include/elliot_b200.h
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -85,7 +85,7 @@ __device__ static inline bool bloom_maybe(const uint32_t *__restrict__ f, int lo
 }
 __device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
-// 128-bit / 32-bit fire-and-forget float adds (REDG.E.ADD.F32x4 / REDG.E.ADD.F32 on sm_100a)
+// 128-bit / 32-bit fire-and-forget float adds (vector / scalar RED instructions)
 __device__ __forceinline__ void red_add_v4(float *p, float4 v) {
     asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
                  "f"(v.w)

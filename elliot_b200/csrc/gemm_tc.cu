@@ -5,11 +5,11 @@
 // Both operands are bf16, K-major (row-major with K contiguous), which is what the Keras Dense
 // layers of the reference need once weights are kept as [out][in]
 // (multi_vae_model.py:44-53,72-78; neural_matrix_factorization_model.py:57-70).  Backward GEMMs
-// use the same kernel on transposed copies (tc_convert_transpose_kernel).
-// Structure = score_topk_tc.cu without the top-k (PTX wrappers shared through tc_ptx.cuh): persistent CTAs, warp 0 TMA producer
-// (4-stage ring of {A 128x64, B 128x64} bf16 tiles, 128B swizzle), warp 1 tcgen05.mma issuer
-// (M=128, N=128, K=16 per instruction, fp32 accumulators double-buffered in TMEM), warps 2-5
-// epilogue (tcgen05.ld -> bias/activation -> global).
+// read MN-major operands directly (A_MN / B_MN below) or use transposed copies (tc_transpose_kernel).
+// Structure (PTX wrappers shared with score_topk_tc.cu through tc_ptx.cuh): persistent CTAs, warp 8 TMA producer
+// (4-stage ring of {A 128x64, B 128x64} bf16 tiles, 128B swizzle), warpgroups 0 and 1 the consumers: each issues
+// wgmma.m64n128k16 for its 64 rows of the 128 x 128 tile (fp32 accumulators in registers, one k-block in flight while the
+// previous stage is released) and writes its rows (bias / activation / split-K reduction) straight from the registers.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -19,13 +19,9 @@
 
 namespace eb {
 
-constexpr int G_BM = 128, G_BN = 128, G_BK = 64, G_STAGES = 4, G_THREADS = 192;
+constexpr int G_BM = 128, G_BN = 128, G_BK = 64, G_STAGES = 4, G_THREADS = 288;
 constexpr int G_STAGE_BYTES = (G_BM + G_BN) * G_BK * 2;      // 32 KB
-// epilogue staging: every epilogue warp owns two [32 rows x 32 fp32] boxes (128-byte rows, 128B swizzle) that TMA
-// stores (or reduce-adds, split-K) into C as full 128-byte lines while the warp converts the next 32 columns
-constexpr int G_EPI_BOX = 32 * 32 * 4;                       // 4 KB
-constexpr int G_EPI_BYTES = 4 * 2 * G_EPI_BOX;               // 32 KB
-constexpr int G_SMEM = G_STAGES * G_STAGE_BYTES + G_EPI_BYTES + 256;
+constexpr int G_SMEM = G_STAGES * G_STAGE_BYTES + 256;
 
 struct GemmParams {
     float *C;
@@ -35,56 +31,42 @@ struct GemmParams {
     int act;             // 0 none, 1 tanh, 2 relu
     float alpha;         // C = alpha * (A B^T) + bias, then activation
     int splits;          // split-K factor: > 1 -> each work item covers a K range and ADDS into a zeroed C (no bias/act)
-    int tma_store;       // 1: epilogue through shared memory + TMA store / reduce (tmC valid); 0: direct row-per-lane stores
     __nv_bfloat16 *Cb;   // optional second output: the same values as bf16 rows (row stride ldcb) — the next layer's operand copy
     int64_t ldcb;
 };
 
+__device__ __forceinline__ float g_act(float x, int act) { return act == 1 ? tanhf(x) : (act == 2 ? fmaxf(x, 0.f) : x); }
+
 // A_MN / B_MN: the operand is given with its M (resp. N) index contiguous — a [K][M] row-major matrix — instead of K-major.
 // TMA then fetches {64 m, 64 k} boxes (two per 128-wide tile) whose 128-byte rows are 64 consecutive M elements, and the
-// shared-memory descriptor says "MN-major": ((8,n),(8,k)) 16-byte units with strides ((1,LBO),(8,SBO)), LBO = the distance
-// between the two 64-wide M blocks (8 KB), SBO = 8 k-rows (1 KB); one K = 16 step advances 16 k-rows = 2 KB.  The weight-gradient
+// shared-memory descriptor says "MN-major" (gmma_desc_sw128_mn; wgmma transposes the operand on the fly).  The weight-gradient
 // GEMMs dW = dY^T . X (K = the batch) and dX = dY . W with W kept [K][N] read their operands this way, so no transposed
 // bf16 copies of activations or weights are ever written.
 template <bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(G_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
     extern __shared__ __align__(1024) uint8_t sm[];
-    uint8_t *epi = sm + G_STAGES * G_STAGE_BYTES;                          // 1024-byte aligned (stages are 32 KB)
-    uint64_t *bars = reinterpret_cast<uint64_t *>(epi + G_EPI_BYTES);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sm + G_STAGES * G_STAGE_BYTES);
     const uint32_t bar0 = smem_u32(bars);
     auto FULL = [&](int s) { return bar0 + 8u * (uint32_t)s; };
     auto EMPTY = [&](int s) { return bar0 + 8u * (uint32_t)(G_STAGES + s); };
-    auto ACC_FULL = [&](int a) { return bar0 + 8u * (uint32_t)(2 * G_STAGES + a); };
-    auto ACC_EMPTY = [&](int a) { return bar0 + 8u * (uint32_t)(2 * G_STAGES + 2 + a); };
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * G_STAGES + 4);
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform (see elect_one_sync)
     const int lane = threadIdx.x & 31;
     const int tiles_m = (p.M + G_BM - 1) / G_BM, tiles_n = (p.N + G_BN - 1) / G_BN;
     const int k_blocks_all = (p.K + G_BK - 1) / G_BK;
     const int kb_per = (k_blocks_all + p.splits - 1) / p.splits;     // k-blocks per split (the last may be shorter)
     const int n_tiles = tiles_m * tiles_n * p.splits;               // work items: (tile, split)
-    const bool vec_ok = ((p.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) &&
-                        (p.bias == nullptr || (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0);
 
     if (threadIdx.x == 0) {
         if (smem_u32(sm) & 1023u) __trap();
-        for (int s = 0; s < G_STAGES; s++) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 1); }
-        for (int a = 0; a < 2; a++) { mbar_init(ACC_FULL(a), 1); mbar_init(ACC_EMPTY(a), 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int s = 0; s < G_STAGES; s++) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 2); }
+        fence_barrier_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(2 * G_BN) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (elect_one_sync()) {
+            tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
             int s = 0; uint32_t ph = 0;
             for (int work = blockIdx.x; work < n_tiles; work += gridDim.x) {
                 const int tile = work / p.splits, split = work % p.splits;
@@ -110,162 +92,67 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == 1) {
-        if (elect_one_sync()) {
-            // instruction descriptor: fp32 accum, bf16 A/B, K-major both, N=128, M=128
-            constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(G_BN >> 3) << 17) | ((uint32_t)(G_BM >> 4) << 24) |
-                                       (A_MN ? (1u << 15) : 0u) | (B_MN ? (1u << 16) : 0u);      // a_major / b_major: 1 = MN-major
-            int s = 0; uint32_t ph = 0; uint32_t it = 0;
-            for (int work = blockIdx.x; work < n_tiles; work += gridDim.x, it++) {
-                const int split = work % p.splits;
-                const int kb0 = split * kb_per, kb1 = min(kb0 + kb_per, k_blocks_all);
-                const int acc = it & 1;
-                mbar_wait(ACC_EMPTY(acc), ((it >> 1) & 1) ^ 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * G_BN);
-                for (int kb = kb0; kb < kb1; kb++) {
-                    mbar_wait(FULL(s), ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t a_addr = smem_u32(sm + s * G_STAGE_BYTES), b_addr = a_addr + G_BM * G_BK * 2;
-#pragma unroll
-                    for (int k = 0; k < 4; k++)
-                        umma_bf16(d_tmem, A_MN ? umma_desc_sw128_mn(a_addr + k * 2048) : umma_desc_sw128(a_addr + k * 32),
-                                  B_MN ? umma_desc_sw128_mn(b_addr + k * 2048) : umma_desc_sw128(b_addr + k * 32), idesc, ((kb - kb0) | k) != 0);
-                    umma_commit(EMPTY(s));
-                    if (++s == G_STAGES) { s = 0; ph ^= 1; }
-                }
-                umma_commit(ACC_FULL(acc));
-            }
-        }
-    } else {
-        const int quad = warp & 3;
-        uint32_t it = 0, chunk = 0;
-        for (int work = blockIdx.x; work < n_tiles; work += gridDim.x, it++) {
+    } else if (warp < 8) {
+        // consumer warpgroup h computes rows [64 h, 64 h + 64) of every 128 x 128 tile
+        const int h = warp >> 2, wq = warp & 3;
+        int s = 0; uint32_t ph = 0;
+        float acc[64];
+        for (int work = blockIdx.x; work < n_tiles; work += gridDim.x) {
             const int tile = work / p.splits, split = work % p.splits;
             const int tm = tile / tiles_n, tn = tile % tiles_n;
-            const bool empty = split * kb_per >= k_blocks_all;          // trailing split without k-blocks: nothing was issued
-            const int acc = it & 1;
-            mbar_wait(ACC_FULL(acc), (it >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int row = tm * G_BM + quad * 32 + lane;
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * G_BN);
-#pragma unroll 1
-            for (int c0 = 0; c0 < G_BN; c0 += 32) {
-                uint32_t r[32];
-                __syncwarp();
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                      "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                      "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                      "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                    : "r"(taddr + (uint32_t)c0)
-                    : "memory");
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (p.tma_store) {
-                    // ---- coalesced path: lane = row of a [32 x 32] fp32 box in shared memory (16-byte chunk j of row r sits at
-                    // chunk j ^ (r & 7): the 128-byte swizzle TMA expects, and conflict-free for these row-per-lane writes),
-                    // then ONE elected lane hands the box to the TMA unit (store, or reduce-add for split-K)
-                    const int col0 = tn * G_BN + c0;
-                    if (!empty && col0 < p.N && tm * G_BM + quad * 32 < p.M) {         // warp-uniform
-                        const uint32_t box = smem_u32(epi + (quad * 2 + (chunk & 1)) * G_EPI_BOX);
-                        // the box used 2 chunks ago has been read (every lane asks: only the one that issued the stores has groups)
-                        asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-                        __syncwarp();
-                        const int my_row = tm * G_BM + quad * 32 + lane;
+            const int kb0 = split * kb_per, kb1 = min(kb0 + kb_per, k_blocks_all);
+            if (kb0 >= kb1) continue;                                   // trailing split without k-blocks: nothing to add
+            int prev = -1;
+            for (int kb = kb0; kb < kb1; kb++) {
+                mbar_wait(FULL(s), ph);
+                const uint32_t a_addr = smem_u32(sm + s * G_STAGE_BYTES) + (uint32_t)h * (64 * G_BK * 2), b_addr = smem_u32(sm + s * G_STAGE_BYTES) + G_BM * G_BK * 2;
+                wgmma_fence();
 #pragma unroll
-                        for (int c = 0; c < 32; c += 4) {
-                            float4 o = make_float4(p.alpha * __uint_as_float(r[c]), p.alpha * __uint_as_float(r[c + 1]),
-                                                   p.alpha * __uint_as_float(r[c + 2]), p.alpha * __uint_as_float(r[c + 3]));
-                            if (p.splits == 1) {
-                                if (p.bias) {
-                                    o.x += __ldg(p.bias + min(col0 + c, p.N - 1)); o.y += __ldg(p.bias + min(col0 + c + 1, p.N - 1));
-                                    o.z += __ldg(p.bias + min(col0 + c + 2, p.N - 1)); o.w += __ldg(p.bias + min(col0 + c + 3, p.N - 1));
-                                }
-                                if (p.act == 1) { o.x = tanhf(o.x); o.y = tanhf(o.y); o.z = tanhf(o.z); o.w = tanhf(o.w); }
-                                else if (p.act == 2) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                            }
-                            const uint32_t dst = box + (uint32_t)lane * 128u + (uint32_t)(((c >> 2) ^ (lane & 7)) << 4);
-                            asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w) : "memory");
-                            if (p.Cb && my_row < p.M) {                 // bf16 copy of the same values, straight from the registers
-                                __nv_bfloat16 *cb = p.Cb + (int64_t)my_row * p.ldcb + col0 + c;
-                                if (col0 + c + 4 <= p.N && (p.ldcb & 3) == 0) {
-                                    const __nv_bfloat162 lo = __floats2bfloat162_rn(o.x, o.y), hi = __floats2bfloat162_rn(o.z, o.w);
-                                    uint2 pk;
-                                    pk.x = *reinterpret_cast<const uint32_t *>(&lo); pk.y = *reinterpret_cast<const uint32_t *>(&hi);
-                                    *reinterpret_cast<uint2 *>(cb) = pk;
-                                } else {
-                                    const float ov[4] = {o.x, o.y, o.z, o.w};
+                for (int k = 0; k < 4; k++)
+                    wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(
+                        acc, A_MN ? gmma_desc_sw128_mn(a_addr + k * 2048) : gmma_desc_sw128(a_addr + k * 32),
+                        B_MN ? gmma_desc_sw128_mn(b_addr + k * 2048) : gmma_desc_sw128(b_addr + k * 32), ((kb - kb0) | k) != 0);
+                wgmma_commit();
+                wgmma_wait<1>();                                        // the previous k-block's MMAs have retired
+                if (prev >= 0 && threadIdx.x % 128 == 0) mbar_arrive(EMPTY(prev));
+                prev = s;
+                if (++s == G_STAGES) { s = 0; ph ^= 1; }
+            }
+            wgmma_wait<0>();
+            wgmma_acc_fence<64>(acc);
+            if (threadIdx.x % 128 == 0) mbar_arrive(EMPTY(prev));
+            const int r0 = tm * G_BM + h * 64 + wq * 16 + (lane >> 2);
+            const bool pair_ok = (p.ldc & 1) == 0 && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+            const bool pair_okb = p.Cb && (p.ldcb & 1) == 0;
 #pragma unroll
-                                    for (int e = 0; e < 4; e++)
-                                        if (col0 + c + e < p.N) cb[e] = __float2bfloat16_rn(ov[e]);
-                                }
-                            }
-                        }
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic-proxy writes -> visible to the TMA unit
-                        __syncwarp();
-                        if (elect_one_sync()) {
-                            const int rr = tm * G_BM + quad * 32;
-                            if (p.splits > 1)
-                                asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
-                                             ::"l"(&tmC), "r"(box), "r"(col0), "r"(rr) : "memory");
-                            else
-                                asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                                             ::"l"(&tmC), "r"(box), "r"(col0), "r"(rr) : "memory");
-                            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                        }
-                        chunk++;
+            for (int half = 0; half < 2; half++) {
+                const int row = r0 + 8 * half;
+                if (row >= p.M) continue;
+                float *crow = p.C + (int64_t)row * p.ldc;
+#pragma unroll
+                for (int j = 0; j < 16; j++) {
+                    const int col = tn * G_BN + 8 * j + 2 * (lane & 3);
+                    if (col >= p.N) continue;
+                    float x0 = p.alpha * acc[4 * j + 2 * half], x1 = p.alpha * acc[4 * j + 2 * half + 1];
+                    const bool two = col + 1 < p.N;
+                    if (p.splits > 1) {
+                        red_add_f32(crow + col, x0);
+                        if (two) red_add_f32(crow + col + 1, x1);
+                        continue;
                     }
-                    continue;
-                }
-                if (row < p.M && !empty) {
-                    float *crow = p.C + (int64_t)row * p.ldc;
-                    const int col0 = tn * G_BN + c0;
-                    if (vec_ok && col0 + 32 <= p.N) {
-                        // each lane owns 32 consecutive floats of its row: 128-bit stores (8 per chunk) instead of 32 scalar ones
-#pragma unroll
-                        for (int c = 0; c < 32; c += 4) {
-                            float4 o = make_float4(p.alpha * __uint_as_float(r[c]), p.alpha * __uint_as_float(r[c + 1]),
-                                                   p.alpha * __uint_as_float(r[c + 2]), p.alpha * __uint_as_float(r[c + 3]));
-                            if (p.splits > 1) {
-                                red_add_v4(crow + col0 + c, o);
-                            } else {
-                                if (p.bias) {
-                                    const float4 bb = __ldg(reinterpret_cast<const float4 *>(p.bias + col0 + c));
-                                    o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
-                                }
-                                if (p.act == 1) { o.x = tanhf(o.x); o.y = tanhf(o.y); o.z = tanhf(o.z); o.w = tanhf(o.w); }
-                                else if (p.act == 2) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                                *reinterpret_cast<float4 *>(crow + col0 + c) = o;
-                            }
-                        }
-                    } else {
-#pragma unroll
-                        for (int c = 0; c < 32; c++) {
-                            const int col = col0 + c;
-                            if (col < p.N) {
-                                float x = p.alpha * __uint_as_float(r[c]);
-                                if (p.splits > 1) { red_add_f32(crow + col, x); continue; }
-                                x += p.bias ? __ldg(p.bias + col) : 0.f;
-                                if (p.act == 1) x = tanhf(x);
-                                else if (p.act == 2) x = fmaxf(x, 0.f);
-                                crow[col] = x;
-                            }
-                        }
+                    if (p.bias) { x0 += __ldg(p.bias + col); if (two) x1 += __ldg(p.bias + col + 1); }
+                    x0 = g_act(x0, p.act); x1 = g_act(x1, p.act);
+                    if (two && pair_ok) *reinterpret_cast<float2 *>(crow + col) = make_float2(x0, x1);
+                    else { crow[col] = x0; if (two) crow[col + 1] = x1; }
+                    if (p.Cb) {                                         // bf16 copy of the same values, straight from the registers
+                        __nv_bfloat16 *cb = p.Cb + (int64_t)row * p.ldcb + col;
+                        if (two && pair_okb) *reinterpret_cast<__nv_bfloat162 *>(cb) = __floats2bfloat162_rn(x0, x1);
+                        else { cb[0] = __float2bfloat16_rn(x0); if (two) cb[1] = __float2bfloat16_rn(x1); }
                     }
                 }
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(ACC_EMPTY(acc));
         }
-        if (p.tma_store) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all boxes written before the CTA retires
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * G_BN) : "memory");
 }
 
 // fp32 [R][C] (row stride ld) -> bf16 [R][dst_ld] (same layout, zero padded columns)
@@ -320,27 +207,6 @@ static int g_make_map(CUtensorMap *m, const void *base, uint64_t rows, uint64_t 
     return EB_OK;
 }
 
-// fp32 C [M][N] (row stride ldc) as {32 cols, 32 rows} boxes, 128-byte swizzle (inner extent = 128 B)
-static int g_make_map_c(CUtensorMap *m, float *C, uint64_t M, uint64_t N, uint64_t ldc) {
-    static GEncodeFn enc = nullptr;
-    if (!enc) {
-        void *fp = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &qres) != cudaSuccess ||
-            qres != cudaDriverEntryPointSuccess)
-            return set_err(EB_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-        enc = (GEncodeFn)fp;
-    }
-    cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)M};
-    cuuint64_t strides[1] = {(cuuint64_t)ldc * 4};
-    cuuint32_t box[2] = {32, 32};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, C, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_err(EB_ERR_CUDA, "cuTensorMapEncodeTiled (C) failed with CUresult %d", (int)r);
-    return EB_OK;
-}
-
 }  // namespace eb
 
 using namespace eb;
@@ -369,24 +235,15 @@ static int gemm_bf16(const void *A_bf16, int64_t lda, bool a_mn, const void *B_b
     EB_ARG(lda % 8 == 0 && ldb % 8 == 0, "lda/ldb must be multiples of 8 bf16 (16-byte TMA strides)");
     EB_ARG(((uintptr_t)A_bf16 % 16) == 0 && ((uintptr_t)B_bf16 % 16) == 0, "operands must be 16-byte aligned");
     EB_ARG(act >= 0 && act <= 2, "act must be 0 (none), 1 (tanh) or 2 (relu)");
-    CUtensorMap ma, mb, mc;
+    EB_ARG(!C_bf16 || (ldcb >= N && ldcb % 8 == 0 && ((uintptr_t)C_bf16 % 8) == 0), "bf16 second output: ldcb must be a multiple of 8 covering N");
+    CUtensorMap ma, mb;
     if (int rc = g_make_map(&ma, A_bf16, (uint64_t)M, (uint64_t)K, (uint64_t)lda, G_BM, a_mn)) return rc;
     if (int rc = g_make_map(&mb, B_bf16, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, G_BN, b_mn)) return rc;
-    // TMA needs a 16-byte aligned base and row stride; otherwise (and with EB_GEMM_TMA_STORE=0) the direct-store epilogue runs
-    static const bool tma_off = [] { const char *e = getenv("EB_GEMM_TMA_STORE"); return e && e[0] == '0'; }();
-    const bool tma_store = !tma_off && (ldc % 4 == 0) && ((uintptr_t)C % 16 == 0);
-    EB_ARG(!C_bf16 || (ldcb >= N && ldcb % 8 == 0 && ((uintptr_t)C_bf16 % 8) == 0), "bf16 second output: ldcb must be a multiple of 8 covering N");
-    if (C_bf16 && !tma_store) {             // odd row stride: plain GEMM, then one conversion pass
-        if (int rc = gemm_bf16(A_bf16, lda, a_mn, B_bf16, ldb, b_mn, C, ldc, M, N, K, bias, alpha, act, stream)) return rc;
-        return eb_convert_bf16(C, M, N, ldc, C_bf16, ldcb, 0, stream);
-    }
-    if (tma_store) { if (int rc = g_make_map_c(&mc, C, (uint64_t)M, (uint64_t)N, (uint64_t)ldc)) return rc; }
-    else mc = ma;
     const int n_out_tiles = ((M + G_BM - 1) / G_BM) * ((N + G_BN - 1) / G_BN);
     const int k_blocks = (K + G_BK - 1) / G_BK;
     // split-K: few output tiles with a long K (dh2 = dlogits . W4: 20 tiles, K = 26 744) leave most SMs idle and each
     // busy CTA load-latency bound; split the K range over the idle SMs and add the partial tiles into a zeroed C
-    // (the partial tiles are ADDED with atomics / TMA reduce: the summation order, hence the last bits, vary from run to run;
+    // (the partial tiles are ADDED with atomics: the summation order, hence the last bits, vary from run to run;
     // EB_GEMM_SPLITK=0 keeps every GEMM single-pass and bit-reproducible at the cost of idle SMs on these shapes)
     static const bool splitk_off = [] { const char *e = getenv("EB_GEMM_SPLITK"); return e && e[0] == '0'; }();
     int splits = 1;
@@ -397,7 +254,7 @@ static int gemm_bf16(const void *A_bf16, int64_t lda, bool a_mn, const void *B_b
         const int per = (k_blocks + splits - 1) / splits;
         splits = (k_blocks + per - 1) / per;                         // no empty trailing splits
     }
-    GemmParams p{C, ldc, bias, M, N, K, act, alpha, splits, tma_store ? 1 : 0, (__nv_bfloat16 *)C_bf16, ldcb};
+    GemmParams p{C, ldc, bias, M, N, K, act, alpha, splits, (__nv_bfloat16 *)C_bf16, ldcb};
     if (splits > 1) {
         if (ldc == N) EB_CUDA(cudaMemsetAsync(C, 0, (size_t)M * N * sizeof(float), (cudaStream_t)stream));
         else EB_CUDA(cudaMemset2DAsync(C, (size_t)ldc * sizeof(float), 0, (size_t)N * sizeof(float), (size_t)M, (cudaStream_t)stream));
@@ -408,7 +265,7 @@ static int gemm_bf16(const void *A_bf16, int64_t lda, bool a_mn, const void *B_b
 #define EB_GEMM_LAUNCH(AM, BM)                                                                                        \
     do {                                                                                                              \
         EB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<AM, BM>, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));   \
-        gemm_tc_kernel<AM, BM><<<grid, G_THREADS, G_SMEM, (cudaStream_t)stream>>>(ma, mb, mc, p);                     \
+        gemm_tc_kernel<AM, BM><<<grid, G_THREADS, G_SMEM, (cudaStream_t)stream>>>(ma, mb, p);                     \
     } while (0)
     if (a_mn && b_mn) EB_GEMM_LAUNCH(true, true);
     else if (a_mn) EB_GEMM_LAUNCH(true, false);

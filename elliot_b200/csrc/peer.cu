@@ -255,11 +255,10 @@ extern "C" int eb_neumf_scatter_peer(const float *Umf, int64_t ldu, float *const
 }
 
 // ---------------------------------------------------------------- batches ordered by owner
-// Measured on 8 B200s (tools/peer_fanout_probe.py, profiles/r2c_peer_fanout_n8.json): 256-byte rows gathered at random from ONE
-// peer arrive at 630 GB/s; the same rows drawn from all 7 peers interleaved arrive at 44 GB/s (with the other 7 GPUs idle, so
-// it is the requester, not the fabric; three peers interleaved, as on 4 GPUs, still run at 615 GB/s); the same ids GROUPED by
-// owner — every rank starting at its right-hand neighbour — arrive at 548 GB/s.  A batch whose rows live on more than four
-// peers is therefore bucketed by owner before the peer kernels see it: a counting sort over <= 64 keys
+// 256-byte rows gathered at random from many peers interleaved arrive far more slowly than the same rows drawn owner by owner
+// (a requester-side limit, tools/peer_fanout_probe.py measures it); the same ids GROUPED by owner — every rank starting at
+// its right-hand neighbour — keep the links busy.  A batch whose rows live on more than four peers is therefore bucketed by
+// owner before the peer kernels see it: a counting sort over <= 64 keys
 //     key = ((owner(id1) - rank) mod W) [* W + ((owner(id2) - rank) mod W)]
 // (order inside a bucket is arbitrary: the samples of a step are exchangeable).
 struct GroupParams {

@@ -1,21 +1,22 @@
-// score_topk_tc.cu — full-catalogue U·Vᵀ on the 5th-gen tensor cores (tcgen05 + TMEM + TMA)
+// score_topk_tc.cu — full-catalogue U·Vᵀ on the Hopper tensor cores (wgmma + TMA + mbarrier)
 // with the per-user masked top-k fused into the epilogue and an exact fp32 re-rank.
 //
 // Replaces BPRMF_batch_model.predict/get_top_k (BPRMF_batch_model.py:82-88) /
 // MFModel.get_user_predictions (BPRMF_model.py:70-85) at catalogue scale: the (users x items)
 // score matrix is never materialised.
 //
-// Pipeline per CTA (persistent, one CTA per SM, 10 warps in the default layout):
-//   warp 0   TMA producer : A tile (128 users x KP, bf16, once per user block) and a ring of
-//                           B tiles (BN items x KP) via cp.async.bulk.tensor, 128B swizzle (+ a narrower-swizzle K tail)
-//   warp 1   MMA issuer   : one ELECTED lane (elect.sync) issues tcgen05.mma.cta_group::1.kind::f16
-//                           (M=128, N=BN, K=16) into one of four TMEM accumulators (4 x 128 columns)
-//   warps 2-5, 6-9        : two epilogue warpgroups (tiles alternate between them, two accumulators each); thread r of a
-//                           group owns user row r: tcgen05.ld 64 columns at a time, a running threshold filters all but the
-//                           group's current top-16 approximate scores (max-tree fast path), survivors are checked against
-//                           the train CSR (block's mask rows cached in shared memory) and kept in a per-row candidate list.
-// Variants behind template switches (TcCfg): one epilogue group (NG = 1), CTA pairs on tcgen05 cta_group::2 (PAIR), the user
-// block in TMEM (ATM), instrumentation (DBG).  DESIGN.md 4.1 has the measurements that chose the default.
+// Pipeline per CTA (persistent, one CTA per SM, NG consumer warpgroups + one TMA warp; NG = 2 by default):
+//   last warp     TMA producer : A tile (128 users x KP, bf16, once per user block) and a ring of
+//                                B tiles (BN items x KP) via cp.async.bulk.tensor, 128B swizzle (+ a narrower-swizzle K tail)
+//   warpgroup g   consumer     : takes every NG-th item tile; issues wgmma.m64nBNk16 twice per K step (users 0-63 and
+//                                64-127) into fp32 register accumulators, hands the B stage back, moves its accumulators
+//                                through a per-warp shared-memory tile so that every thread holds ONE user row, then a
+//                                running threshold filters all but the group's current top-16 approximate scores (max-tree
+//                                fast path), survivors are checked against the train CSR (block's mask rows cached in shared
+//                                memory) and kept in a per-row candidate list.
+// While one warpgroup scans its tile the other one's MMAs run on the tensor cores.  Variants behind template switches (TcCfg):
+// one consumer warpgroup (NG = 1), CTA pairs sharing every item tile through TMA multicast (PAIR), the user block held in
+// registers as the wgmma A operand (ATM), instrumentation (DBG).
 // After the last item tile each warp re-scores its rows' <= 32 candidates (16 per group) EXACTLY in fp32
 // (same summation order as score_topk.cu), sorts them with a 32-lane bitonic network
 // (score desc, index asc) and certifies the result:
@@ -33,10 +34,11 @@
 
 namespace eb {
 
-constexpr int TC_BM = 128;        // users per block (UMMA M)
+constexpr int TC_BM = 128;        // users per block (two wgmma M = 64 halves)
 constexpr int TC_KC = 32;         // candidates kept per user (one per lane in the re-rank)
 
 
+// ---------------------------------------------------------------- parameters
 // ---------------------------------------------------------------- parameters
 struct TcParams {
     // exact-side inputs
@@ -49,7 +51,7 @@ struct TcParams {
     int32_t n_sel;
     int k;
     // prepared by tc_prep kernels
-    const __nv_bfloat16 *ubf;    // bf16 user rows [n_sel][KP] (the A operand), read directly by the A-in-TMEM kernels
+    const __nv_bfloat16 *ubf;    // bf16 user rows [n_sel][KP] (the A operand), read directly by the users-in-registers kernel
     const float *unorm;          // ||u|| per selected user
     const float *vstat;          // [0] = max ||v||, [1] = max |bias|
     const float *bmax_chunk;     // max bias per 32-item chunk (null if no bias)
@@ -62,77 +64,64 @@ struct TcParams {
     float eps_scale;             // c in eps_u = c * ||u|| * max||v|| + 1e-6 * (...)
     long long *prof;             // optional per-kernel cycle counters (8 values), profiling only
     int bias_folded;             // 1: bias already inside the accumulators (extra K columns); the re-rank still adds it exactly
-    int debug_mode;              // profiling only: 1 = TMEM read + max only, 2 = no compaction (results invalid)
+    int debug_mode;              // profiling only: 1 = accumulator read + max only, 2 = no compaction (results invalid)
 };
 
 constexpr int TC_BUF = 64;        // append-buffer slots per user row over all epilogue groups (top-KC kept + pending)
 
 // KP = padded K (multiple of 16): KB full 64-wide blocks (one 128-byte swizzle atom each) + a tail of KT = 0, 16 or 32
 // columns in its own narrower-swizzle block.  (A 48-column tail is rounded up to a full block by the host.)  Padding K
-// to a multiple of 64 instead — as round 1 did — costs 2.0x the MMA work at d = 64 + 2 bias columns (128 vs 80) and
-// 1.33x at d = 128 + 2 (192 vs 144).
-// NG = number of epilogue warpgroups.  NG = 1: warps 2-5 scan every tile, 32 kept candidates in a 64-slot buffer per row.
-// NG = 2: warps 2-5 take the even tiles, warps 6-9 the odd ones (global tile counter), so every scheduler has TWO epilogue
-// warps to overlap the TMEM-load / max-tree latency of one with the other.  Each group keeps KC/2 = 16 candidates in a
-// 32-slot buffer per row: the 16th best of half the stream sits at the same level as the 32nd best of the whole stream, so
-// the insert rate per item is that of NG = 1 (round 2a's NG = 2 kept 32 per group and paid 1.85x the inserts), the shared
+// to a multiple of 64 instead costs 2.0x the MMA work at d = 64 + 2 bias columns (128 vs 80) and 1.33x at d = 128 + 2
+// (192 vs 144).
+// NG = number of consumer warpgroups.  NG = 1: warpgroup 0 takes every tile, 32 kept candidates in a 64-slot buffer per row.
+// NG = 2: warpgroup 0 takes the even tiles, warpgroup 1 the odd ones (global tile counter), so the MMAs of one overlap the
+// scan of the other.  Each group keeps KC/2 = 16 candidates in a 32-slot buffer per row: the 16th best of half the stream
+// sits at the same level as the 32nd best of the whole stream, so the insert rate per item is that of NG = 1, the shared
 // memory is the same 64 KB, and the re-rank reads the two lists side by side (16 + 16 lanes) with tau = max of the two.
-// Each group double-buffers its own accumulator (4 x BN TMEM columns, BN <= 128).
-// PAIR: two CTAs of a cluster (two SMs of one TPC) score 256 users against each item tile with ONE tcgen05.mma.cta_group::2
-// per K step: each CTA keeps its own 128 users (A tile, accumulators, candidate lists, epilogue warps) and loads only HALF of
-// the item tile's rows; the tensor cores of both SMs read the two halves from the two shared memories.  The item table then
-// crosses the L2 -> SM fabric once per 256 users instead of once per 128 — the feed that bounds the single-CTA kernel at
-// large catalogues (9.5 TB/s at 2 M x 144 bf16 with nothing but the MMA running).
-// ATM: the user block (the operand that stays for the whole item stream) lives in TMEM instead of shared memory: the epilogue
-// warps of group 0 write their rows there once per user block (tcgen05.st) and every MMA takes A from TMEM.  A K = 16 step of
-// an M = 128 x N = 128 MMA reads 4 KB of A and 4 KB of B from shared memory in its 64 cycles — all of the SM's 128 B/cycle,
-// before the TMA fill of the next tile and the epilogue's candidate buffers: measured ~100 cycles per step.  Without A it is
-// half.  TMEM: 128 columns for A (KP / 2 used) + 3 accumulators x 128 (tile t -> accumulator t % 3, group t % 2).
+// BN = items per tile (wgmma N).  A warpgroup's accumulators are 128 x BN fp32; they pass through a per-warp shared-memory
+// tile (32 rows x BN) on their way from the wgmma fragment layout to one row per thread, so BN also sets that tile's size:
+// 64 up to KP = 128, 32 above (so that four B stages still fit beside the 64 KB user block).
+// PAIR: two CTAs of a cluster (two SMs) score their own user blocks against the same item tiles; each CTA fetches HALF of
+// every item tile and multicasts it into both shared memories, so the item table crosses the L2 -> SM fabric once per 256
+// users instead of once per 128.  A stage is refilled only after the consumers of BOTH CTAs have released it.
+// ATM: the user block (the operand that stays for the whole item stream) is held in the consumer warpgroups' registers as
+// the wgmma A operand instead of being re-read from shared memory by every MMA; only the item tile is read from shared
+// memory.  (The historical name: the Blackwell kernel kept it in tensor memory.)  Built for KP <= 144 (KP / 2 registers).
 template <int KP, int NG_, bool PAIR_ = false, bool ATM_ = false> struct TcCfg {
     static constexpr int KB = KP / 64;                       // full 64-wide K blocks
     static constexpr int KT = KP % 64;                       // tail columns
     static_assert(KT == 0 || KT == 16 || KT == 32, "K tail must be 0, 16 or 32 columns");
     static constexpr int NG = NG_;
-    static constexpr bool PAIR = PAIR_;
-    // TMEM accumulators: two per epilogue group; PAIR widens the tile to 256 items (one M = 256 x N = 256 instruction per K
-    // step: per SM and MMA cycle the shared memory then serves half the operand bytes of two M = 128 x N = 128 ones) and
-    // keeps one accumulator per group — the groups alternate, so the MMA of one tile still overlaps the scan of the other
-    static constexpr bool ATM = ATM_;
-    static_assert(!(ATM && (PAIR || NG != 2)), "A-in-TMEM is built for the two-group single-CTA kernel");
-    // items per tile of the two-group kernel.  64 (eight accumulators, four per group: deeper MMA / scan decoupling) was measured
-    // SLOWER than 128 (four accumulators): C2 probe 5.22 vs 4.92 ms, C5 slice 24.7 vs 20.0 ms — the per-tile hand-shakes cost more
-    // than the slack buys (profiles/r2c_score_bn64.log).  -DEB_TC_BN2=64 rebuilds that variant.
-#ifndef EB_TC_BN2
-#define EB_TC_BN2 128
-#endif
-    static constexpr int NACC = ATM ? 3 : (PAIR ? NG : (NG == 2 ? 512 / EB_TC_BN2 : 2 * NG));
-    static constexpr int ACC0 = ATM ? 128 : 0;               // first accumulator column
+    static constexpr bool PAIR = PAIR_, ATM = ATM_;
+    static_assert(!(PAIR && ATM) && (!(PAIR || ATM) || NG_ == 2), "CTA pairs / users in registers: two-group kernel only");
+    static_assert(!ATM || KP <= 144, "users in registers: KP <= 144");
+    static constexpr int BN = KP <= 128 ? 64 : 32;
+    static_assert(BN == 32 || BN == 64, "tiles of 32 or 64 items");
+    static constexpr int NCH = BN / 4;                       // 16-byte chunks per staged row
     static constexpr int KCG = TC_KC / NG;                   // candidates kept per row and group
     static constexpr int BUFG = TC_BUF / NG;                 // buffer slots per row and group
     static constexpr int ROWB = BUFG * 4;                    // bytes per buffer row (keys; the ids follow in a second array)
-    static constexpr int BN = PAIR ? (KP <= 208 ? 256 : 128)
-                                   : (NG == 2 ? (ATM ? 128 : (KP <= 208 ? EB_TC_BN2 : 64))
-                                              : (KP <= 128 ? 256 : (KP <= 208 ? 128 : 64)));   // items per tile (UMMA N)
-    static_assert(ACC0 + NACC * BN <= 512, "accumulators exceed TMEM");
-    static constexpr int TMEM_COLS = ATM ? 512 : NACC * BN;  // 256 or 512: a power of two
-    static constexpr int THREADS = 64 + 128 * NG;            // TMA warp + MMA warp + NG x 4 epilogue warps
-    static constexpr int A_BYTES = ATM ? 0 : TC_BM * KP * 2;
-    static constexpr int BNL = PAIR ? BN / 2 : BN;           // item rows of a tile THIS CTA loads
-    static constexpr int B_BYTES = BNL * KP * 2;
+    static constexpr int THREADS = 128 * NG + 32;            // NG consumer warpgroups + the TMA warp
+    static constexpr int A_BYTES = TC_BM * KP * 2;
+    static constexpr int B_BYTES = BN * KP * 2;
+    static constexpr int STG_WARP = 32 * BN * 4;             // accumulator staging per warp
+    static constexpr int STG_BYTES = 4 * NG * STG_WARP;
     static constexpr int CAND_BYTES = TC_BM * TC_BUF * 8;    // all groups together
     static constexpr int MRG_BYTES = 2048;                   // per-row {cnt, thresh} of every group after the last tile
-    static constexpr int FIXED = A_BYTES + CAND_BYTES + MRG_BYTES + 256;
+    static constexpr int FIXED = A_BYTES + STG_BYTES + CAND_BYTES + MRG_BYTES + 256;
     static constexpr int ROOM = (232448 - FIXED) / B_BYTES;  // 227 KB of dynamic shared memory per CTA
-    static constexpr int STAGES = ROOM >= (PAIR ? 6 : 4) ? (PAIR ? 6 : 4) : ROOM;
+    static constexpr int STAGES = ROOM >= 4 ? 4 : ROOM;
     static_assert(STAGES >= 2, "B ring needs two stages");
     static constexpr int USED = FIXED + STAGES * B_BYTES;
     static constexpr int SMEM = 232448;                      // everything: what is left caches the user block's train-mask rows
     static constexpr int MASKC = (SMEM - USED) / 4;          // cached mask entries (int32) per user block
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
+// The user row a thread owns: warp q of a warpgroup holds the accumulators of rows 16 q .. 16 q + 15 of both 64-row halves
+// (wgmma fragment layout), so it takes exactly those 32 rows — lane l < 16 row 16 q + l, lane l >= 16 row 64 + 16 q + l - 16 —
+// and the fragment-to-row transposition stays inside the warp.
+__device__ __forceinline__ int tc_row(int quad, int l) { return (l < 16 ? 0 : 48) + quad * 16 + l; }
+
 
 __device__ __forceinline__ bool cand_better(float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); }
 
@@ -223,7 +212,7 @@ __device__ __noinline__ uint2 tc_compact_rows(uint32_t todo, uint32_t ckey, uint
     while (todo) {
         const int r = __ffs(todo) - 1;
         todo &= todo - 1;
-        const int rrow = quad * 32 + r;
+        const int rrow = tc_row(quad, r);
         const int rl = __shfl_sync(0xffffffffu, mlen, r);
         const int64_t rb = __shfl_sync(0xffffffffu, mbeg, r);
         const int64_t rel = rb - seg_beg;                       // the row's offset inside the block's cached segment
@@ -239,31 +228,29 @@ __device__ __noinline__ uint2 tc_compact_rows(uint32_t todo, uint32_t ckey, uint
     return make_uint2((uint32_t)cnt, __float_as_uint(thresh));
 }
 
-// DBG = false compiles the instrumentation out (cycle counters, dense score dump, EB_TC_DEBUG modes): the clock reads alone
-// were 4 % of the kernel's instructions; the launcher picks DBG = true only when one of them is requested.
+// DBG = false compiles the instrumentation out (cycle counters, dense score dump, EB_TC_DEBUG modes); the launcher picks
+// DBG = true only when one of them is requested.
 template <int KP, bool HAS_BIAS, int NGT, bool PAIR, bool ATM, bool DBG>
 __global__ void __launch_bounds__(TcCfg<KP, NGT, PAIR, ATM>::THREADS, 1)
 score_topk_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmAt, const __grid_constant__ CUtensorMap tmBt, const TcParams p) {
     using C = TcCfg<KP, NGT, PAIR, ATM>;
-    constexpr int KB = C::KB, KT = C::KT, BN = C::BN, BNL = C::BNL, S = C::STAGES, NG = C::NG, NACC = C::NACC;
+    constexpr int KB = C::KB, KT = C::KT, BN = C::BN, S = C::STAGES, NG = C::NG, NCH = C::NCH;
     constexpr int KCG = C::KCG, BUFG = C::BUFG;
     constexpr uint32_t ROWB = C::ROWB, GRPB = TC_BM * BUFG * 8;           // bytes per buffer row / per group (keys + ids)
     const bool DUMP = DBG && p.dump != nullptr;
     const int debug_mode = DBG ? p.debug_mode : 0;
     extern __shared__ __align__(1024) uint8_t sm[];
-    uint8_t *sA = sm;                                   // KB blocks of [128 rows x 128 B]
-    uint8_t *sB = sA + C::A_BYTES;                      // S stages of KB blocks of [BN rows x 128 B]
-    const uint32_t cval = smem_u32(sB + S * C::B_BYTES);                     // float [BUF][128]
+    uint8_t *sA = sm;                                   // KB blocks of [128 rows x 128 B] + the tail block
+    uint8_t *sB = sA + C::A_BYTES;                      // S stages of KB blocks of [BN rows x 128 B] + tail
+    const uint32_t stg = smem_u32(sB + S * C::B_BYTES);                      // per warp: fp32 [32 rows][BN], chunk-swizzled
+    const uint32_t cval = stg + C::STG_BYTES;                                // keys / ids [BUF][128]
     const uint32_t mrg = cval + C::CAND_BYTES;                               // per group: {cnt[128], thresh[128]}
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + S * C::B_BYTES + C::CAND_BYTES + C::MRG_BYTES);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + S * C::B_BYTES + C::STG_BYTES + C::CAND_BYTES + C::MRG_BYTES);
     const uint32_t bar0 = smem_u32(bars);
     auto B_FULL = [&](int s) { return bar0 + 8u * (uint32_t)s; };
     auto B_EMPTY = [&](int s) { return bar0 + 8u * (uint32_t)(S + s); };
     const uint32_t A_FULL = bar0 + 8u * (2 * S), A_EMPTY = bar0 + 8u * (2 * S + 1);
-    auto ACC_FULL = [&](int a) { return bar0 + 8u * (uint32_t)(2 * S + 2 + a); };
-    auto ACC_EMPTY = [&](int a) { return bar0 + 8u * (uint32_t)(2 * S + 2 + NACC + a); };
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * S + 2 + 2 * NACC);
     const uint32_t mcache = smem_u32(sm + C::USED);                          // int32 [MASKC]: the user block's train-mask rows
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform: role branches do not diverge
@@ -275,137 +262,68 @@ score_topk_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
     const int n_units = PAIR ? (n_mblocks + 1) / 2 : n_mblocks;
     const int unit0 = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, unit_step = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    // PAIR: the operand barriers the MMA thread waits on (A_FULL, B_FULL) and the ones it is released by (ACC_EMPTY) live
-    // in the LEADER (rank 0); the ones it releases (A_EMPTY, B_EMPTY, ACC_FULL) exist in both CTAs (multicast commit)
     if (threadIdx.x == 0) {
         if (smem_u32(sm) & 1023u) __trap();             // SWIZZLE_128B tiles need 1024-byte alignment
-        for (int s = 0; s < S; s++) { mbar_init(B_FULL(s), PAIR ? 2 : 1); mbar_init(B_EMPTY(s), 1); }
-        mbar_init(A_FULL, ATM ? 4 : (PAIR ? 2 : 1)); mbar_init(A_EMPTY, 1);
-        for (int a = 0; a < NACC; a++) { mbar_init(ACC_FULL(a), 1); mbar_init(ACC_EMPTY(a), PAIR ? 8 : 4); }
+        for (int s = 0; s < S; s++) { mbar_init(B_FULL(s), 1); mbar_init(B_EMPTY(s), PAIR ? 2 : 1); }
+        mbar_init(A_FULL, 1); mbar_init(A_EMPTY, NG);
         fence_barrier_init();
-        tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
-        if (KT) { tma_prefetch_desc(&tmAt); tma_prefetch_desc(&tmBt); }
     }
-    if (warp == 1) { if (PAIR) tmem_alloc_pair(smem_u32(tmem_slot), C::TMEM_COLS); else tmem_alloc(smem_u32(tmem_slot), C::TMEM_COLS); }
-    tc_fence_before();
-    if (PAIR) cluster_sync_all(); else __syncthreads();   // barriers of BOTH CTAs are initialised before anyone signals them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    if (PAIR) cluster_sync_all(); else __syncthreads();   // PAIR: the peer's barriers exist before anything is multicast to it
 
-    if (warp == 0) {
+    if (warp == 4 * NG) {
         // ===================== TMA producer =====================
         if (elect_one_sync()) {
+            tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
+            if (KT) { tma_prefetch_desc(&tmAt); tma_prefetch_desc(&tmBt); }
             int s = 0; uint32_t ph = 0; uint32_t it = 0;
             const bool prof = DBG && p.prof != nullptr && blockIdx.x == 0;
             long long w_bempty = 0;
-            const uint32_t a_full = PAIR ? mapa_cluster(A_FULL, 0) : A_FULL;
             for (int un = unit0; un < n_units; un += unit_step, it++) {
                 const int mb = PAIR ? 2 * un + (int)rank : un;
-                if (!ATM) mbar_wait(A_EMPTY, (it & 1) ^ 1);
-                if (ATM) {}                                   // the user block goes to TMEM through the epilogue warps
-                else if (!PAIR) mbar_expect_tx(A_FULL, C::A_BYTES);
-                else if (rank == 0) mbar_expect_tx(A_FULL, 2 * C::A_BYTES);     // both CTAs' A tiles are credited to the leader
-                else mbar_arrive_cluster(a_full);
-                for (int kb = 0; kb < KB && !ATM; kb++) {
-                    if (PAIR) tma_load_2d_pair(smem_u32(sA + kb * (TC_BM * 128)), &tmA, a_full, kb * 64, mb * TC_BM);
-                    else tma_load_2d(smem_u32(sA + kb * (TC_BM * 128)), &tmA, A_FULL, kb * 64, mb * TC_BM);
-                }
-                if (KT && !ATM) {
-                    if (PAIR) tma_load_2d_pair(smem_u32(sA + KB * (TC_BM * 128)), &tmAt, a_full, KB * 64, mb * TC_BM);
-                    else tma_load_2d(smem_u32(sA + KB * (TC_BM * 128)), &tmAt, A_FULL, KB * 64, mb * TC_BM);
+                if (!ATM) {                           // ATM: the consumers read the user rows into registers themselves
+                    mbar_wait(A_EMPTY, (it & 1) ^ 1);
+                    mbar_expect_tx(A_FULL, C::A_BYTES);
+                    for (int kb = 0; kb < KB; kb++) tma_load_2d(smem_u32(sA + kb * (TC_BM * 128)), &tmA, A_FULL, kb * 64, mb * TC_BM);
+                    if (KT) tma_load_2d(smem_u32(sA + KB * (TC_BM * 128)), &tmAt, A_FULL, KB * 64, mb * TC_BM);
                 }
                 for (int t = 0; t < n_tiles; t++) {
                     const long long t0 = prof ? clock64() : 0;
                     mbar_wait(B_EMPTY(s), ph ^ 1);
                     if (prof) w_bempty += clock64() - t0;
-                    const uint32_t b_full = PAIR ? mapa_cluster(B_FULL(s), 0) : B_FULL(s);
-                    if (!PAIR) mbar_expect_tx(B_FULL(s), C::B_BYTES);
-                    else if (rank == 0) mbar_expect_tx(B_FULL(s), 2 * C::B_BYTES);
-                    else mbar_arrive_cluster(b_full);
-                    const int row0 = t * BN + (int)rank * BNL;                  // PAIR: this CTA's half of the tile's item rows
-                    for (int kb = 0; kb < KB; kb++) {
-                        if (PAIR) tma_load_2d_pair(smem_u32(sB + s * C::B_BYTES + kb * (BNL * 128)), &tmB, b_full, kb * 64, row0);
-                        else tma_load_2d(smem_u32(sB + s * C::B_BYTES + kb * (BNL * 128)), &tmB, B_FULL(s), kb * 64, row0);
-                    }
-                    if (KT) {
-                        if (PAIR) tma_load_2d_pair(smem_u32(sB + s * C::B_BYTES + KB * (BNL * 128)), &tmBt, b_full, KB * 64, row0);
-                        else tma_load_2d(smem_u32(sB + s * C::B_BYTES + KB * (BNL * 128)), &tmBt, B_FULL(s), KB * 64, row0);
+                    mbar_expect_tx(B_FULL(s), C::B_BYTES);       // PAIR: half from this CTA, half multicast by the peer
+                    if (PAIR) {
+                        constexpr int H = BN / 2;                    // item rows of a tile this CTA fetches for both
+                        for (int kb = 0; kb < KB; kb++)
+                            tma_load_2d_mc(smem_u32(sB + s * C::B_BYTES + kb * (BN * 128) + rank * (H * 128)), &tmB, B_FULL(s), kb * 64,
+                                           t * BN + (int)rank * H, (uint16_t)3);
+                        if (KT) tma_load_2d_mc(smem_u32(sB + s * C::B_BYTES + KB * (BN * 128) + rank * (H * KT * 2)), &tmBt, B_FULL(s),
+                                               KB * 64, t * BN + (int)rank * H, (uint16_t)3);
+                    } else {
+                        for (int kb = 0; kb < KB; kb++)
+                            tma_load_2d(smem_u32(sB + s * C::B_BYTES + kb * (BN * 128)), &tmB, B_FULL(s), kb * 64, t * BN);
+                        if (KT) tma_load_2d(smem_u32(sB + s * C::B_BYTES + KB * (BN * 128)), &tmBt, B_FULL(s), KB * 64, t * BN);
                     }
                     if (++s == S) { s = 0; ph ^= 1; }
                 }
             }
             if (prof) p.prof[12] = w_bempty;
-            if (PAIR) {
-                // drain: the leader's last multicast commits must have landed in this CTA's barriers before it may exit
-                for (int i = 0; i < S; i++) { mbar_wait(B_EMPTY(s), ph ^ 1); if (++s == S) { s = 0; ph ^= 1; } }
-                mbar_wait(A_EMPTY, (it & 1) ^ 1);
-            }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (PAIR: the leader CTA's, for both) =====================
-        if (rank == 0 && elect_one_sync()) {
-            constexpr uint32_t idesc = umma_idesc_bf16(PAIR ? 2 * TC_BM : TC_BM, BN);
-            auto mma = [&](uint32_t d, uint64_t da, uint64_t db, bool accumulate) {
-                if (PAIR) umma_bf16_pair(d, da, db, idesc, accumulate); else umma_bf16(d, da, db, idesc, accumulate);
-            };
-            auto commit = [&](uint32_t bar) { if (PAIR) umma_commit_pair(bar); else umma_commit(bar); };
-            int s = 0; uint32_t ph = 0; uint32_t it = 0; uint32_t tile = 0;
-            const bool prof = DBG && p.prof != nullptr && blockIdx.x == 0;
-            long long w_acc = 0, w_bfull = 0, w_afull = 0, t_all = prof ? clock64() : 0;
-            for (int un = unit0; un < n_units; un += unit_step, it++) {
-                { const long long t0 = prof ? clock64() : 0; mbar_wait(A_FULL, it & 1); if (prof) w_afull += clock64() - t0; }
-                for (int t = 0; t < n_tiles; t++, tile++) {
-                    const int acc = tile % NACC;      // accumulator acc belongs to epilogue group acc % NG
-                    const long long t0 = prof ? clock64() : 0;
-                    mbar_wait(ACC_EMPTY(acc), ((tile / NACC) & 1) ^ 1);
-                    const long long t1 = prof ? clock64() : 0;
-                    mbar_wait(B_FULL(s), ph);
-                    if (prof) { w_acc += t1 - t0; w_bfull += clock64() - t1; }
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(C::ACC0 + acc * BN);
-#pragma unroll
-                    for (int kb = 0; kb < KB; kb++) {
-                        const uint32_t a_addr = smem_u32(sA + kb * (TC_BM * 128));
-                        const uint32_t b_addr = smem_u32(sB + s * C::B_BYTES + kb * (BNL * 128));
-#pragma unroll
-                        for (int k = 0; k < 4; k++) { // UMMA_K = 16 bf16 = 32 B inside the 128-B swizzle atom = 8 TMEM columns of A
-                            if (ATM) umma_bf16_ts(d_tmem, tmem_base + (uint32_t)((kb * 4 + k) * 8), umma_desc_sw128(b_addr + k * 32), idesc, (kb | k) != 0);
-                            else mma(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), (kb | k) != 0);
-                        }
-                    }
-                    if (KT) {                         // K tail: one (16 columns) or two (32) more K = 16 steps
-                        const uint32_t a_addr = smem_u32(sA + KB * (TC_BM * 128));
-                        const uint32_t b_addr = smem_u32(sB + s * C::B_BYTES + KB * (BNL * 128));
-#pragma unroll
-                        for (int k = 0; k < KT / 16; k++) {
-                            if (ATM) umma_bf16_ts(d_tmem, tmem_base + (uint32_t)((KB * 4 + k) * 8), umma_desc_tail<KT ? KT : 16>(b_addr + k * 32), idesc, (KB | k) != 0);
-                            else mma(d_tmem, umma_desc_tail<KT ? KT : 16>(a_addr + k * 32), umma_desc_tail<KT ? KT : 16>(b_addr + k * 32),
-                                     (KB | k) != 0);
-                        }
-                    }
-                    commit(B_EMPTY(s));               // B stage reusable once these MMAs retire
-                    commit(ACC_FULL(acc));            // accumulator ready for the epilogue
-                    if (++s == S) { s = 0; ph ^= 1; }
-                }
-                commit(A_EMPTY);                      // A reusable after the block's last MMA
-            }
-            if (prof) { p.prof[8] = w_acc; p.prof[9] = w_bfull; p.prof[10] = w_afull; p.prof[11] = clock64() - t_all; }
-        }
-    } else {
-        // ===================== epilogue: warps 2..5 (group 0) and, if NG == 2, warps 6..9 (group 1) =====================
-        // Group g owns the tiles with (global tile counter % NG) == g, the TMEM accumulators g and g + NG, and its own
-        // candidate buffers; the re-rank at the end of every user block reads the groups' lists side by side.
-        const int grp = NG == 2 ? ((warp - 2) >> 2) : 0;
-        const int quad = warp & 3;                    // TMEM lane quadrant this warp may read
-        const int row = quad * 32 + lane;             // row inside the 128-user block
+    } else if (warp < 4 * NG) {
+        // ===================== consumers: warpgroup 0 (warps 0-3) and, if NG == 2, warpgroup 1 (warps 4-7) =====================
+        // Group g owns the tiles with (global tile counter % NG) == g and its own candidate buffers; the re-rank at the end of
+        // every user block reads the groups' lists side by side.
+        const int grp = NG == 2 ? (warp >> 2) : 0;
+        const int quad = warp & 3;                    // warp inside the warpgroup
+        const int row = tc_row(quad, lane);           // row inside the 128-user block
         const float NEG = -CUDART_INF_F;
         // candidate buffer: row-major [128 rows][BUFG slots] of sortable keys + item ids; logical slot s of row r
         // lives at physical position (s + r) & (BUFG - 1) (rotation: conflict-free appends AND conflict-free row reads)
         const uint32_t ckey = cval + (uint32_t)grp * GRPB;                    // uint32 keys [128][BUFG], then ids [128][BUFG]
         const uint32_t cidx = ckey + TC_BM * BUFG * 4;
+        const uint32_t stw = stg + (uint32_t)(warp * C::STG_WARP);            // this warp's accumulator staging tile
         uint32_t tile = 0;
         long long c_wait = 0, c_ld = 0, c_scan = 0, c_comp = 0, c_rank = 0, n_comp = 0, n_slow = 0, n_grp = 0;
-        const bool prof = DBG && p.prof != nullptr && warp == 2;
+        const bool prof = DBG && p.prof != nullptr && warp == 0;
         constexpr int EPI_THREADS = 128 * NG;
         uint32_t ublk = 0;                            // user blocks this CTA has started
         for (int un = unit0; un < n_units; un += unit_step, ublk++) {
@@ -421,25 +339,27 @@ score_topk_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                 const int q1 = min(mb * TC_BM + TC_BM, p.n_sel);
                 seg_beg = p.mask_indptr[p.user_begin + mb * TC_BM];
                 n_cached = (int)min(p.mask_indptr[p.user_begin + q1] - seg_beg, (int64_t)C::MASKC);
-                for (int e = (int)threadIdx.x - 64; e < n_cached; e += EPI_THREADS) sts_s32(mcache + 4u * (uint32_t)e, __ldg(p.mask_indices + seg_beg + e));
+                for (int e = (int)threadIdx.x; e < n_cached; e += EPI_THREADS) sts_s32(mcache + 4u * (uint32_t)e, __ldg(p.mask_indices + seg_beg + e));
             }
             named_bar_sync(3, EPI_THREADS);
-            if (ATM && grp == 0) {
-                // this thread's user row -> its TMEM lane, columns [0, KP / 2): pairs of consecutive bf16 K elements per column
-                mbar_wait(A_EMPTY, (ublk & 1) ^ 1);            // the previous block's MMAs no longer read A
-                tc_fence_after();
-                const uint4 *src = reinterpret_cast<const uint4 *>(p.ubf + (int64_t)(valid ? q : 0) * KP);
+            // ATM: this thread's A fragments of both 64-row halves for every K = 16 step, straight from the bf16 user rows
+            uint32_t afr[ATM ? 2 : 1][ATM ? KP / 16 : 1][4];
+            if (ATM) {
 #pragma unroll
-                for (int j = 0; j < KP / 16; j++) {
-                    uint4 lo = make_uint4(0u, 0u, 0u, 0u), hi = lo;
-                    if (valid) { lo = __ldg(src + 2 * j); hi = __ldg(src + 2 * j + 1); }
-                    const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-                    tmem_st8(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(j * 8), w);
+                for (int h = 0; h < 2; h++) {
+#pragma unroll
+                    for (int hf = 0; hf < 2; hf++) {
+                        const int rq = mb * TC_BM + h * 64 + quad * 16 + (lane >> 2) + 8 * hf;
+                        const uint32_t *src = reinterpret_cast<const uint32_t *>(p.ubf + (int64_t)(rq < p.n_sel ? rq : 0) * KP) + (lane & 3);
+#pragma unroll
+                        for (int ks = 0; ks < (ATM ? KP / 16 : 1); ks++) {
+                            afr[h][ks][hf] = rq < p.n_sel ? __ldg(src + ks * 8) : 0u;
+                            afr[h][ks][2 + hf] = rq < p.n_sel ? __ldg(src + ks * 8 + 4) : 0u;
+                        }
+                    }
                 }
-                tmem_st_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(A_FULL);
+            } else {
+                mbar_wait(A_FULL, ublk & 1);          // the block's user rows are in shared memory
             }
             int cnt = 0;                              // filled logical slots of my row
             float thresh = (valid && debug_mode != 1) ? NEG : CUDART_INF_F;   // upper bound of everything dropped so far
@@ -456,44 +376,130 @@ score_topk_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
             };
 
             for (int t = 0; t < n_tiles; t++, tile++) {
-                const int acc = tile % NACC;
                 if (NG == 2 && (int)(tile & 1u) != grp) continue;
+                const int s = (int)(tile % (uint32_t)S);
                 long long t0 = prof ? clock64() : 0;
-                mbar_wait(ACC_FULL(acc), (tile / NACC) & 1);
-                tc_fence_after();
-                if (prof) c_wait += clock64() - t0;
-                const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(C::ACC0 + acc * BN);
-#pragma unroll 1
-                for (int c0 = 0; c0 < BN; c0 += 64) {
-                    float v[64];
-                    __syncwarp();                     // tcgen05.ld is .sync.aligned
-                    long long t1 = prof ? clock64() : 0;
-                    tmem_ld32_nowait(taddr + (uint32_t)c0, v);
-                    tmem_ld32_nowait(taddr + (uint32_t)c0 + 32u, v + 32);
-                    tmem_ld_wait();
-                    if (prof) c_ld += clock64() - t1;
-                    long long t2 = prof ? clock64() : 0;
-                    const int col0 = t * BN + c0;
-                    if (DUMP) {
-                        if (valid)
-                            for (int c = 0; c < 64; c++)
-                                if (col0 + c < p.n_items) p.dump[(int64_t)q * p.n_items + col0 + c] = v[c];
-                    }
-                    // max of each group of 8 columns (fast reject), 3-input max trees
-                    float g[8];
+                named_bar_sync(4 + grp, 128);         // the warpgroup issues its wgmma together
+                mbar_wait(B_FULL(s), (tile / (uint32_t)S) & 1);
+                long long t1 = prof ? clock64() : 0;
+                if (prof) c_wait += t1 - t0;
+                // ---- 128 users x BN items: two wgmma M = 64 halves per K = 16 step
+                float acc0[BN / 2], acc1[BN / 2];
+                {
+                    const uint32_t a_addr = smem_u32(sA), b_addr = smem_u32(sB + s * C::B_BYTES);
+                    wgmma_fence();
+                    if constexpr (ATM) {
 #pragma unroll
-                    for (int s8 = 0; s8 < 8; s8++) {
-                        const float *w = v + s8 * 8;
-                        g[s8] = fmaxf(fmaxf(fmaxf(w[0], w[1]), w[2]), fmaxf(fmaxf(fmaxf(w[3], w[4]), w[5]), fmaxf(w[6], w[7])));
+                        for (int ks = 0; ks < KP / 16; ks++) {
+                            const int kb = ks / 4, k = ks % 4;
+                            const uint64_t db = kb < KB ? gmma_desc_sw128(b_addr + kb * (BN * 128) + k * 32)
+                                                        : gmma_desc_tail<KT ? KT : 16>(b_addr + KB * (BN * 128) + k * 32);
+                            if (BN == 64) {
+                                wgmma_m64n64k16_rs(acc0, afr[0][ks], db, ks != 0);
+                                wgmma_m64n64k16_rs(acc1, afr[ATM ? 1 : 0][ks], db, ks != 0);
+                            } else {
+                                wgmma_m64n32k16_rs(acc0, afr[0][ks], db, ks != 0);
+                                wgmma_m64n32k16_rs(acc1, afr[ATM ? 1 : 0][ks], db, ks != 0);
+                            }
+                        }
                     }
-                    float bm0 = 0.f, bm1 = 0.f;
-                    if (HAS_BIAS) { bm0 = __ldg(p.bmax_chunk + (col0 >> 5)); bm1 = __ldg(p.bmax_chunk + min((col0 >> 5) + 1, (p.n_items - 1) >> 5)); }
-                    const float m64 = HAS_BIAS ? fmaxf(fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3])) + bm0, fmaxf(fmaxf(g[4], g[5]), fmaxf(g[6], g[7])) + bm1)
-                                               : fmaxf(fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3])), fmaxf(fmaxf(g[4], g[5]), fmaxf(g[6], g[7])));
-                    if (!__any_sync(0xffffffffu, m64 > thresh)) { if (prof) c_scan += clock64() - t2; continue; }
+#pragma unroll
+                    for (int kb = 0; kb < (ATM ? 0 : KB); kb++) {
+#pragma unroll
+                        for (int k = 0; k < 4; k++) {     // K = 16 bf16 = 32 B inside the 128-B swizzle atom
+                            const uint64_t db = gmma_desc_sw128(b_addr + kb * (BN * 128) + k * 32);
+                            const uint32_t aa = a_addr + kb * (TC_BM * 128) + k * 32;
+                            const bool accum = (kb | k) != 0;
+                            if (BN == 64) {
+                                wgmma_m64n64k16<0, 0>(acc0, gmma_desc_sw128(aa), db, accum);
+                                wgmma_m64n64k16<0, 0>(acc1, gmma_desc_sw128(aa + 64 * 128), db, accum);
+                            } else {
+                                wgmma_m64n32k16<0, 0>(acc0, gmma_desc_sw128(aa), db, accum);
+                                wgmma_m64n32k16<0, 0>(acc1, gmma_desc_sw128(aa + 64 * 128), db, accum);
+                            }
+                        }
+                    }
+                    if (KT && !ATM) {                     // K tail: one (16 columns) or two (32) more K = 16 steps
+                        constexpr int KTT = KT ? KT : 16;
+#pragma unroll
+                        for (int k = 0; k < KT / 16; k++) {
+                            const uint64_t db = gmma_desc_tail<KTT>(b_addr + KB * (BN * 128) + k * 32);
+                            const uint32_t aa = a_addr + KB * (TC_BM * 128) + k * 32;
+                            const bool accum = (KB | k) != 0;
+                            if (BN == 64) {
+                                wgmma_m64n64k16<0, 0>(acc0, gmma_desc_tail<KTT>(aa), db, accum);
+                                wgmma_m64n64k16<0, 0>(acc1, gmma_desc_tail<KTT>(aa + 64 * KTT * 2), db, accum);
+                            } else {
+                                wgmma_m64n32k16<0, 0>(acc0, gmma_desc_tail<KTT>(aa), db, accum);
+                                wgmma_m64n32k16<0, 0>(acc1, gmma_desc_tail<KTT>(aa + 64 * KTT * 2), db, accum);
+                            }
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_acc_fence<BN / 2>(acc0);
+                    wgmma_acc_fence<BN / 2>(acc1);
+                }
+                if (threadIdx.x % 128 == 0) {         // B stage reusable: this group's MMAs have retired (PAIR: in both CTAs)
+                    mbar_arrive(B_EMPTY(s));
+                    if (PAIR) mbar_arrive_cluster(mapa_cluster(B_EMPTY(s), rank ^ 1u));
+                }
+                // ---- fragments -> one row per thread through this warp's staging tile: 16-byte chunk c of staged row r sits
+                // at chunk c ^ (r % NCH) (conflict-free row-per-lane reads)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const float *a = h ? acc1 : acc0;
+#pragma unroll
+                    for (int j = 0; j < BN / 8; j++) {
+#pragma unroll
+                        for (int hf = 0; hf < 2; hf++) {
+                            const int lr = h * 16 + (lane >> 2) + 8 * hf;
+                            const int col = 8 * j + 2 * (lane & 3);
+                            const uint32_t dst = stw + (uint32_t)(lr * BN * 4) + (uint32_t)((((col >> 2) ^ (lr & (NCH - 1))) << 4) | ((col & 3) << 2));
+                            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(dst), "f"(a[4 * j + 2 * hf]), "f"(a[4 * j + 2 * hf + 1]) : "memory");
+                        }
+                    }
+                }
+                __syncwarp();
+                float v[BN];
+#pragma unroll
+                for (int c = 0; c < NCH; c++) {
+                    const uint32_t src = stw + (uint32_t)(lane * BN * 4) + (uint32_t)((c ^ (lane & (NCH - 1))) << 4);
+                    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                                 : "=f"(v[4 * c]), "=f"(v[4 * c + 1]), "=f"(v[4 * c + 2]), "=f"(v[4 * c + 3]) : "r"(src) : "memory");
+                }
+                if (prof) c_ld += clock64() - t1;
+                long long t2 = prof ? clock64() : 0;
+                const int col0 = t * BN;
+                if (DUMP) {
+                    if (valid)
+                        for (int c = 0; c < BN; c++)
+                            if (col0 + c < p.n_items) p.dump[(int64_t)q * p.n_items + col0 + c] = v[c];
+                }
+                // max of each group of 8 columns (fast reject), 3-input max trees
+                constexpr int NS8 = BN / 8;
+                float g[NS8];
+#pragma unroll
+                for (int s8 = 0; s8 < NS8; s8++) {
+                    const float *w = v + s8 * 8;
+                    g[s8] = fmaxf(fmaxf(fmaxf(w[0], w[1]), w[2]), fmaxf(fmaxf(fmaxf(w[3], w[4]), w[5]), fmaxf(w[6], w[7])));
+                }
+                // bias bound per 32-item chunk (bm1: the second chunk of a 64-item tile)
+                float bm0 = 0.f, bm1 = 0.f;
+                if (HAS_BIAS) {
+                    bm0 = __ldg(p.bmax_chunk + (col0 >> 5));
+                    if (BN == 64) bm1 = __ldg(p.bmax_chunk + min((col0 >> 5) + 1, (p.n_items - 1) >> 5));
+                }
+                float m64;
+                if (BN == 64)
+                    m64 = HAS_BIAS ? fmaxf(fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3])) + bm0, fmaxf(fmaxf(g[NS8 - 4], g[NS8 - 3]), fmaxf(g[NS8 - 2], g[NS8 - 1])) + bm1)
+                                   : fmaxf(fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3])), fmaxf(fmaxf(g[NS8 - 4], g[NS8 - 3]), fmaxf(g[NS8 - 2], g[NS8 - 1])));
+                else
+                    m64 = fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3])) + (HAS_BIAS ? bm0 : 0.f);
+                if (__any_sync(0xffffffffu, m64 > thresh)) {
                     if (DBG) n_slow++;
 #pragma unroll
-                    for (int s8 = 0; s8 < 8; s8++) {
+                    for (int s8 = 0; s8 < NS8; s8++) {
                         const float bm = s8 < 4 ? bm0 : bm1;
                         if (!__any_sync(0xffffffffu, (HAS_BIAS ? g[s8] + bm : g[s8]) > thresh)) continue;
                         if (DBG) n_grp++;
@@ -538,12 +544,10 @@ score_topk_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                             gm = fmaxf(fmaxf(fmaxf(w8[0], w8[1]), w8[2]), fmaxf(fmaxf(fmaxf(w8[3], w8[4]), w8[5]), fmaxf(w8[6], w8[7])));
                         }
                     }
-                    if (prof) c_scan += clock64() - t2;
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) { if (PAIR && rank != 0) mbar_arrive_cluster(mapa_cluster(ACC_EMPTY(acc), 0)); else mbar_arrive(ACC_EMPTY(acc)); }
+                if (prof) c_scan += clock64() - t2;
             }
+            if (!ATM && threadIdx.x % 128 == 0) mbar_arrive(A_EMPTY);  // this group's MMAs of the block have all retired
             // final compaction: every row ends with its <= KC best unmasked candidates in logical slots 0..cnt-1
             __syncwarp();
             long long t4 = prof ? clock64() : 0;
@@ -558,9 +562,9 @@ score_topk_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
             // ---- exact re-rank (rows split between the groups): lane l re-scores candidate l of the row in fp32 with the
             // SAME operation order as score_topk.cu (32 strided partial sums, then the xor-butterfly tree)
             for (int r = (NG == 2 ? grp * 16 : 0); r < (NG == 2 ? grp * 16 + 16 : 32); r++) {
-                const int rrow = quad * 32 + r;
+                const int rrow = tc_row(quad, r);
                 const int rq = mb * TC_BM + rrow;
-                if (rq >= p.n_sel) break;                                 // warp-uniform
+                if (rq >= p.n_sel) continue;                                 // warp-uniform
                 const int ru = p.user_begin + rq;
                 // lanes [g * KCG, g * KCG + cnt_g) take group g's list; everything either group dropped is <= the larger tau
                 const int lg = NG == 2 ? lane / KCG : 0, ls = lane - lg * KCG;
@@ -639,9 +643,7 @@ score_topk_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
             p.prof[5] = n_comp; p.prof[6] = n_slow; p.prof[7] = n_grp;
         }
     }
-    tc_fence_before();
-    if (PAIR) cluster_sync_all(); else __syncthreads();     // nobody leaves while the peer may still signal its barriers
-    if (warp == 1) { if (PAIR) tmem_dealloc_pair(tmem_base, C::TMEM_COLS); else tmem_dealloc(tmem_base, C::TMEM_COLS); }
+    if (PAIR) cluster_sync_all();     // no CTA leaves while its peer may still multicast into it or signal its barriers
 }
 
 // ---------------------------------------------------------------- preparation kernels
@@ -762,7 +764,7 @@ static int launch_tc3(const TcMaps &m, const TcParams &p, int n_mblocks, cudaStr
         if (grid > n_mblocks) grid = n_mblocks;
         kern<<<grid, C::THREADS, C::SMEM, st>>>(m.a, m.b, m.at, m.bt, p);
     } else {
-        // clusters of two CTAs (one TPC): a cluster scores two user blocks against every item tile
+        // clusters of two CTAs: a cluster scores two user blocks against every item tile
         int clusters = sm_count() / 2;
         if (clusters > (n_mblocks + 1) / 2) clusters = (n_mblocks + 1) / 2;
         cudaLaunchConfig_t cfg{};
@@ -780,13 +782,14 @@ static int launch_tc3(const TcMaps &m, const TcParams &p, int n_mblocks, cudaStr
 template <int KP, int NG, bool PAIR, bool ATM>
 static int launch_tc(void *ubf, void *vbf, const TcParams &p, int n_mblocks, cudaStream_t st) {
     using C = TcCfg<KP, NG, PAIR, ATM>;
+    constexpr int BL = PAIR ? C::BN / 2 : C::BN;           // item rows per TMA box (PAIR: each CTA fetches half a tile)
     TcMaps m;
     // a tile without full blocks (KP = 16 / 32) still needs valid descriptors in the unused slots
     const uint32_t bc = C::KB ? 64 : C::KT, tc = C::KT ? C::KT : 64;
     if (int rc = make_map(&m.a, ubf, (uint64_t)p.n_sel, KP, bc, TC_BM)) return rc;
-    if (int rc = make_map(&m.b, vbf, (uint64_t)p.n_items, KP, bc, C::BNL)) return rc;
+    if (int rc = make_map(&m.b, vbf, (uint64_t)p.n_items, KP, bc, BL)) return rc;
     if (int rc = make_map(&m.at, ubf, (uint64_t)p.n_sel, KP, tc, TC_BM)) return rc;
-    if (int rc = make_map(&m.bt, vbf, (uint64_t)p.n_items, KP, tc, C::BNL)) return rc;
+    if (int rc = make_map(&m.bt, vbf, (uint64_t)p.n_items, KP, tc, BL)) return rc;
     const bool hb = p.bias != nullptr && !p.bias_folded;    // epilogue adds the bias only when it is not folded into the MMA
     // the lean kernel exists for the default layout only; the others always carry the instrumentation
     constexpr bool LEAN = NG == 2 && !PAIR && !ATM;
@@ -831,7 +834,7 @@ extern "C" int eb_score_topk_tc_f32(const float *U, const float *V, const float 
     if (n_sel == 0) return EB_OK;
     int cc = 0;
     if (int rc = eb_device_info(nullptr, &cc)) return rc;
-    if (cc < 100) return set_err(EB_ERR_CUDA, "tcgen05 path needs compute capability 10.x (got %d)", cc);
+    if (cc != 90) return set_err(EB_ERR_CUDA, "the wgmma scoring kernel is built for compute capability 9.0 (got %d)", cc);
     const bool fold = item_bias != nullptr && d + 2 <= 256;
     const TcLayout L = tc_layout(n_sel, n_items, d, fold);
     if (workspace_bytes < L.total) return set_err(EB_ERR_WORKSPACE, "workspace %zu < required %zu", workspace_bytes, L.total);
@@ -857,20 +860,20 @@ extern "C" int eb_score_topk_tc_f32(const float *U, const float *V, const float 
     { const char *dbg = getenv("EB_TC_DEBUG"); p.debug_mode = dbg ? atoi(dbg) : 0; }
     p.prof = (stats_host && getenv("EB_TC_PROF")) ? (long long *)(flag_count + 16) : nullptr;
     const int n_mblocks = (int)((n_sel + TC_BM - 1) / TC_BM);
-    // epilogue warpgroups: two by default (see TcCfg); EB_TC_NG=1 selects the single-group kernel for A/B measurements
+    // consumer warpgroups: two by default (see TcCfg); EB_TC_NG=1 selects the single-group kernel for A/B measurements
     int ng = 2;
     { const char *e = getenv("EB_TC_NG"); if (e && atoi(e) == 1) ng = 1; }
-    // CTA pairs (tcgen05 cta_group::2, see TcCfg): EB_TC_PAIR=1 (two epilogue groups only)
+    // CTA pairs sharing every item tile through TMA multicast (see TcCfg): EB_TC_PAIR=1 (two consumer groups only)
     bool pair = false;
     { const char *e = getenv("EB_TC_PAIR"); if (e && atoi(e) == 1 && ng == 2) pair = true; }
-    // the user block in TMEM instead of shared memory (see TcCfg): EB_TC_ATM=1
+    // the user block in registers instead of shared memory (see TcCfg): EB_TC_ATM=1
     bool atm = false;
     { const char *e = getenv("EB_TC_ATM"); if (e && atoi(e) == 1 && ng == 2 && !pair) atm = true; }
     int rc;
     switch (L.KP) {
 #define EB_TC_CASE(K) case K: rc = ng == 2 ? launch_tc<K, 2, false, false>(ubf, vbf, p, n_mblocks, st)                           \
                                           : launch_tc<K, 1, false, false>(ubf, vbf, p, n_mblocks, st); break;
-        // the measured-but-not-faster variants (CTA pairs, users in TMEM) exist for d = 64 and 128 with and without bias
+        // the measured variants (CTA pairs, users in registers) exist for d = 64 and 128 with and without bias
 #define EB_TC_CASE_X(K) case K: rc = pair ? launch_tc<K, 2, true, false>(ubf, vbf, p, n_mblocks, st)                            \
                                          : (atm ? launch_tc<K, 2, false, true>(ubf, vbf, p, n_mblocks, st)                     \
                                                 : (ng == 2 ? launch_tc<K, 2, false, false>(ubf, vbf, p, n_mblocks, st)         \

@@ -1,5 +1,5 @@
-// tc_ptx.cuh — PTX wrappers for the tcgen05 / TMEM / TMA kernels (score_topk_tc.cu, gemm_tc.cu): mbarriers, bulk tensor
-// copies, TMEM allocation and loads, UMMA issue/commit and the shared-memory / instruction descriptor encodings.
+// tc_ptx.cuh — PTX wrappers for the Hopper tensor-core kernels (score_topk_tc.cu, gemm_tc.cu): mbarriers, TMA bulk tensor
+// copies, warpgroup MMA (wgmma) issue / fence / commit / wait and the shared-memory matrix descriptor encodings.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -32,8 +32,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {}
 }
 // One lane of the (converged) warp, chosen by the hardware.  Unlike `lane == 0` the compiler KNOWS a single lane runs the guarded
-// region, so operands of TMA / tcgen05 instructions go to uniform registers directly instead of through a per-instruction
-// "waterfall" loop (ELECT + R2UR.BROADCAST + BRA.U.ANY, ~100 cycles per tcgen05.mma: measured as the MMA issue rate).
+// region, so the operands of the TMA instructions go to uniform registers directly.
 __device__ __forceinline__ bool elect_one_sync() {
     uint32_t pred;
     asm volatile(
@@ -58,31 +57,83 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 inputs, fp32 accumulate, one CTA
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
+// ---------------------------------------------------------------- warpgroup MMA (sm_90a)
+// Every wgmma is issued by all 128 threads of a warpgroup (4 consecutive warps, the first one a multiple of 4).
+// D (64 x N fp32, registers) (+)= A (64 x 16 bf16, shared memory) * B (N x 16 bf16, shared memory)^T.  Accumulator layout:
+// thread t = 32 w + l holds, for every 8-column block j, d[4j + {0, 1}] at row 16 w + l / 4, columns 8 j + 2 (l % 4) + {0, 1},
+// and d[4j + {2, 3}] at the row 8 below.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the compiler must not move reads of the accumulators above the wait that makes them valid
+template <int R>
+__device__ __forceinline__ void wgmma_acc_fence(float *d) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// TA / TB: 0 = the operand is K-major (K contiguous), 1 = MN-major (bf16 only)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n32k16(float *d, uint64_t desc_a, uint64_t desc_b, bool accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// all previously issued MMAs of this thread arrive on the mbarrier when they complete
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"((uint32_t)accumulate), "n"(TA), "n"(TB));
 }
 
-// ---------------------------------------------------------------- CTA pair (cluster of two, tcgen05 cta_group::2)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16(float *d, uint64_t desc_a, uint64_t desc_b, bool accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"((uint32_t)accumulate), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float *d, uint64_t desc_a, uint64_t desc_b, bool accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"((uint32_t)accumulate), "n"(TA), "n"(TB));
+}
+
+// A operand from registers (the user block held by the warpgroup instead of re-read from shared memory every MMA): thread
+// 32 w + l holds a[0] = A[16 w + l / 4][2 (l % 4) + {0, 1}], a[1] the row 8 below, a[2] / a[3] the same 8 columns further.
+__device__ __forceinline__ void wgmma_m64n32k16_rs(float *d, const uint32_t *a, uint64_t desc_b, bool accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"((uint32_t)accumulate));
+}
+
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float *d, const uint32_t *a, uint64_t desc_b, bool accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"((uint32_t)accumulate));
+}
+
+// ---------------------------------------------------------------- clusters of two CTAs (TMA multicast of shared operands)
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
@@ -94,101 +145,36 @@ __device__ __forceinline__ uint32_t mapa_cluster(uint32_t addr, uint32_t rank) {
 }
 // arrive on an mbarrier given by its shared::cluster address (own or peer CTA)
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster) {
-    // default semantics (release at CTA scope), as cutlass::arch::ClusterBarrier::arrive(cta_id): a .release.cluster here costs
-    // a cluster-scope fence per call (measured: +1 500 cycles per accumulator hand-back)
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
 }
-// the box lands in THIS CTA's shared memory, the bytes are credited to the mbarrier at shared::cluster address `bar_cluster`
-// (the pair leader's): what lets one MMA thread wait for both halves of an operand
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap *map, uint32_t bar_cluster, int c0, int c1) {
+// the box lands at the same shared-memory offset in every CTA of `mask`, and its bytes are credited to the mbarrier at the
+// same offset in each of them
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, uint16_t mask) {
     asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1)
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
         : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A * B^T over the pair: M = 256 (128 rows from each CTA's A tile), B's N rows split half/half
-// between the two CTAs' shared memory; issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// when the pair's previously issued MMAs complete, arrive on the mbarrier at this shared-memory offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)3) : "memory");
 }
 
-// A operand in TMEM: D[tmem] (+)= A[tmem] * B[smem]^T.  A occupies lanes = rows, 32-bit columns = pairs of consecutive K elements
-// (8 columns per K = 16 step), so a K step no longer reads 4 KB of A from shared memory
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
+// Shared-memory matrix descriptor (sm_90 GMMA): [0,14) address >> 4, [16,30) leading byte offset >> 4, [32,46) stride byte
+// offset >> 4, [62,64) swizzle: 1 = 128 B, 2 = 64 B, 3 = 32 B.
+// K-major tile with a 128-byte swizzle (what TMA SWIZZLE_128B writes for a {64 bf16, rows} box): rows 128 B apart, 8-row
+// groups 1024 B apart (SBO); a K = 16 step inside the atom advances the start address by 32 B.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// 8 consecutive 32-bit columns of this thread's TMEM lane (quadrant*32 + t) from registers
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t *r) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
+// MN-major tile, 128-byte swizzle (what TMA SWIZZLE_128B writes for a {64 mn, k rows} box of a [K][MN] row-major matrix):
+// 64 MN elements per 128-byte row, 8 k-rows per 1 KB atom (SBO), the next 64 MN elements one 64-row box further
+// (LBO = 64 * 128 B); a K = 16 step advances 16 k-rows = 2 KB.
+__device__ __forceinline__ uint64_t gmma_desc_sw128_mn(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (512ull << 16) | (64ull << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread t gets row (quadrant*32 + t)
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, float *v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-#pragma unroll
-    for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major operand tile in shared memory, 128-byte swizzle (what TMA SWIZZLE_128B writes for
-// a {64 bf16, rows} box): rows are 128 B apart, 8-row groups 1024 B apart.
-// Field layout (cute::UMMA::SmemDescriptor): [0,14) addr>>4, [16,30) LBO>>4 (=1, unused for
-// swizzled K-major), [32,46) SBO>>4 (=64), [46,48) version=1, [61,64) layout=2 (SWIZZLE_128B).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// MN-major operand tile, 128-byte swizzle (what TMA SWIZZLE_128B writes for a {64 mn, k rows} box of a [K][MN] row-major matrix):
-// 16-byte units ((8,n),(8,k)):((1,LBO),(8,SBO)) — 64 MN elements per 128-byte row, 8 k-rows per 1 KB atom (SBO), the next 64 MN
-// elements one 64-row box further (LBO = 64 * 128 B).  cute::UMMA::make_umma_desc<Major::MN>.
-__device__ __forceinline__ uint64_t umma_desc_sw128_mn(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (512ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// K tail (KP % 64 = 16 or 32 columns): the same K-major tile with a 32-byte (layout 6) or 64-byte (layout 4) swizzle,
-// as TMA SWIZZLE_32B / SWIZZLE_64B writes a {16 | 32 bf16, rows} box: rows 32 / 64 B apart, 8-row groups 256 / 512 B apart.
+// K tail (KP % 64 = 16 or 32 columns): the same K-major tile with a 32-byte or 64-byte swizzle, as TMA SWIZZLE_32B /
+// SWIZZLE_64B writes a {16 | 32 bf16, rows} box: rows 32 / 64 B apart, 8-row groups 256 / 512 B apart.
 template <int KT>
-__device__ __forceinline__ uint64_t umma_desc_tail(uint32_t smem_addr) {
-    constexpr uint64_t sbo = KT == 16 ? 16 : 32, layout = KT == 16 ? 6 : 4;
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (sbo << 32) | (1ull << 46) | (layout << 61);
+__device__ __forceinline__ uint64_t gmma_desc_tail(uint32_t smem_addr) {
+    constexpr uint64_t sbo = KT == 16 ? 16 : 32, layout = KT == 16 ? 3 : 2;
+    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (sbo << 32) | (layout << 62);
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (1<<4), a/b format BF16 (1<<7, 1<<10), K-major A and B,
-// n_dim = N>>3 at [17,23), m_dim = M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
 
 }  // namespace eb

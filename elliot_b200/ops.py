@@ -49,7 +49,7 @@ def device_info():
     return sm.value, cc.value
 
 
-def bpr_step_f32(U, V, b, d, tu, ti, tj, lr, reg_u, reg_b, reg_pos, reg_neg, loss=None, racy=False):
+def bpr_step_f32(U, V, b, d, tu, ti, tj, lr, reg_u, reg_b, reg_pos, reg_neg, loss=None, racy=False, deterministic=False):
     """Throughput-mode BPR step on materialised triples (BPRMF_model.py:87-117 semantics)."""
     _need_cuda(U, V, b, tu, ti, tj, loss)
     _chk_idx(tu, ti, tj)
@@ -57,7 +57,8 @@ def bpr_step_f32(U, V, b, d, tu, ti, tj, lr, reg_u, reg_b, reg_pos, reg_neg, los
     assert U.stride(1) == 1 and V.stride(1) == 1 and U.stride(0) == V.stride(0)
     with torch.cuda.device(U.device):
         check(lib().eb_bpr_step_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), _ptr(tu), _ptr(ti), _ptr(tj), tu.numel(),
-                                    lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), 1 if racy else 0, _stream(U)))
+                                    lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), (1 if racy else 0) | (64 if deterministic else 0),
+                                    _stream(U)))
 
 
 def bloom_build(indptr, indices, n_users, words=32):
@@ -72,8 +73,10 @@ def bloom_build(indptr, indices, n_users, words=32):
 
 
 def bpr_step_sampled_f32(U, V, b, d, n_users, n_items, indptr, indices, n, seed, first, lr, reg_u, reg_b, reg_pos,
-                         reg_neg, loss=None, out=None, racy=False, reserve_sms=0, filter=None, _variant=0):
+                         reg_neg, loss=None, out=None, racy=False, reserve_sms=0, filter=None, deterministic=False, _variant=0):
     """Fused sample+update step (custom_sampler.py:24-46 distribution, Philox stream).  filter: bloom_build() output.
+    deterministic: run the launch in rounds (reads, grid barrier, atomic adds, grid barrier) so the same inputs give the same
+    tables on every run up to fp32 summation order; slower than the default free-running Hogwild.
     _variant (profiling): 16 forces the register-staged kernel, 32 the shared-memory-staged one (default: see use_stage)."""
     _need_cuda(U, V, b, indptr, indices, loss, filter)
     assert indptr.dtype == torch.int64 and indices.dtype == torch.int32
@@ -85,7 +88,7 @@ def bpr_step_sampled_f32(U, V, b, d, n_users, n_items, indptr, indices, n, seed,
         check(lib().eb_bpr_step_sampled_filter_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), n_users, n_items, _ptr(indptr),
                                                    _ptr(indices), _ptr(filter), 0 if filter is None else filter.shape[1], n, seed,
                                                    first, lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), _ptr(ou), _ptr(oi),
-                                                   _ptr(oj), (1 if racy else 0) | ((int(reserve_sms) & 0xff) << 8) | int(_variant),
+                                                   _ptr(oj), (1 if racy else 0) | (64 if deterministic else 0) | ((int(reserve_sms) & 0xff) << 8) | int(_variant),
                                                    _stream(U)))
 
 

@@ -1,4 +1,4 @@
-"""BPRMF on B200 behind the reference's model surface.
+"""BPRMF on the H100 behind the reference's model surface.
 
 Mirrors elliot/recommender/latent_factor_models/BPRMF/BPRMF.py:23-129 (constructor contract,
 `_params_list` keys/defaults, name, train(), get_recommendations()) and BPRMF_model.py:14-139
@@ -107,7 +107,7 @@ class MFModel:
 
 
 class BPRMF(RecMixin, BaseRecommenderModel):
-    r"""Bayesian Personalized Ranking MF (https://arxiv.org/abs/1205.2618) on B200.
+    r"""Bayesian Personalized Ranking MF (https://arxiv.org/abs/1205.2618) on the H100.
 
     YAML block identical to the reference's (BPRMF.py:37-56):
         BPRMF: {meta: {...}, epochs, factors, lr, bias_regularization, user_regularization,
@@ -150,8 +150,8 @@ class BPRMF(RecMixin, BaseRecommenderModel):
         np.random.seed(42)                                      # keep the host's global stream where the reference leaves it
         self._hog_counter = 0
         self._loss_dev = torch.zeros(1, dtype=torch.float64, device=self._device)
-        # per-user membership signatures shorten the sampler's load chain on large catalogues (+4 % at 2 M items) and cost
-        # ~10 % on small, L2-resident ones (profiles/r2_hogwild_ab.json); the samples are identical either way
+        # per-user membership signatures shorten the sampler's load chain on large catalogues and cost time on small,
+        # L2-resident ones; the samples are identical either way
         self._filter = ops.bloom_build(self._indptr, self._sorted_idx, self._num_users) \
             if self._mode == "hogwild" and self._num_items >= 500_000 else None
 

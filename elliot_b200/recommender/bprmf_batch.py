@@ -1,4 +1,4 @@
-"""BPRMF_batch on B200 behind the reference's model surface.
+"""BPRMF_batch on the H100 behind the reference's model surface.
 
 Mirrors elliot/recommender/latent_factor_models/BPRMF_batch/BPRMF_batch.py:22-120 (params
 `factors, lr, l_w, l_b`, name "BPRNN", batch semantics: batch_size < 1 -> one batch per epoch,

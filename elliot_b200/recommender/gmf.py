@@ -1,4 +1,4 @@
-"""GMF (Generalized Matrix Factorization, NeuMF's MF branch) on B200 behind the reference's model surface
+"""GMF (Generalized Matrix Factorization, NeuMF's MF branch) on the H100 behind the reference's model surface
 (SURVEY.md §8f #3).
 
 Mirrors elliot/recommender/neural/GeneralizedMF/generalized_matrix_factorization.py:24-120 (params `lr, mf_factors,

@@ -1,5 +1,5 @@
 """MF2020 — pointwise logistic matrix factorisation ("Neural Collaborative Filtering vs. Matrix Factorization
-Revisited") on B200: a sibling of BPRMF on the same gather / dot / scatter shape (SURVEY.md §8f #3).
+Revisited") on the H100: a sibling of BPRMF on the same gather / dot / scatter shape (SURVEY.md §8f #3).
 
 Mirrors elliot/recommender/latent_factor_models/MF2020/MF.py:22-146 (class MF2020: `_params_list` keys/defaults
 factors 10, lr 0.05, reg 0, m 0; name; train(); get_recommendations()), MF_model.py:14-174 (MFModel: init stream,
@@ -105,10 +105,10 @@ class MF2020Model:
 
 
 class MF2020(RecMixin, BaseRecommenderModel):
-    r"""Matrix Factorization as in "NCF vs. MF Revisited" (https://dl.acm.org/doi/pdf/10.1145/3383313.3412488) on B200.
+    r"""Matrix Factorization as in "NCF vs. MF Revisited" (https://dl.acm.org/doi/pdf/10.1145/3383313.3412488) on the H100.
 
     YAML block identical to the reference's (MF.py:41-52): MF2020: {meta: {...}, epochs, factors, lr, reg, m};
-    optional B200 keys `b200_mode` (exact | hogwild), `b200_batch` (samples per Hogwild launch), `b200_eval`,
+    optional keys `b200_mode` (exact | hogwild), `b200_batch` (samples per Hogwild launch), `b200_eval`,
     `b200_device`.
     """
 

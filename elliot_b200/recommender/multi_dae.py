@@ -1,4 +1,4 @@
-"""MultiDAE on B200 behind the reference's model surface (SURVEY.md §8f #3: "VAE minus sampling/KL").
+"""MultiDAE on the H100 behind the reference's model surface (SURVEY.md §8f #3: "VAE minus sampling/KL").
 
 Mirrors elliot/recommender/autoencoders/dae/multi_dae.py:24-110 (same YAML keys as MultiVAE, per-epoch shuffled user
 batches from sparse_sampler.py:13-25) and multi_dae_model.py:20-145: l2-normalised, dropped-out user row ->

@@ -1,4 +1,4 @@
-"""MultiVAE on B200 behind the reference's model surface.
+"""MultiVAE on the H100 behind the reference's model surface.
 
 Mirrors elliot/recommender/autoencoders/vae/multi_vae.py:22-115 (params `intermediate_dim,
 latent_dim, reg_lambda, lr, dropout_pkeep`, anneal schedule min(0.2, step/200000), per-epoch

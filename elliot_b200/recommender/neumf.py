@@ -1,4 +1,4 @@
-"""NeuMF on B200 behind the reference's model surface.
+"""NeuMF on the H100 behind the reference's model surface.
 
 Mirrors elliot/recommender/neural/NeuMF/neural_matrix_factorization.py:24-124 (params `mf_factors, lr, dropout,
 is_mf_train, is_mlp_train, m`; MLP sizes forced to (4f, 2f, f) and mlp_factors = f, :71-72; pointwise BCE,

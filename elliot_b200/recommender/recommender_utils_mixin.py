@@ -21,7 +21,7 @@ class RecMixin:
                      and hasattr(self.evaluator, "eval_tensors") and not self._save_recs and not self._negative_sampling)
         self._losses.append(loss)
         if on_device:
-            # B200 extension: the (users x k) index tensor goes from the scoring kernel straight into the metric
+            # extension: the (users x k) index tensor goes from the scoring kernel straight into the metric
             # kernel; no {user: [(item, score)]} dicts are built (recommender_utils_mixin.py:84-88 / evaluator.py:117-147)
             idx, _ = self.get_recommendations_tensors(self.evaluator.get_needed_recommendations())
             recs = None

@@ -1,4 +1,4 @@
-"""run_experiment(config_path): drives the B200 models from an Elliot YAML file.
+"""run_experiment(config_path): drives the GPU models from an Elliot YAML file.
 
 Mirrors the call contract of elliot/run.py:39-148 for the slice the hot path needs: read the
 YAML (namespace_model.py:64-241 keys), load + split the data (dataset.py:29-161,

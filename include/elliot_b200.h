@@ -1,5 +1,5 @@
 /*
- * elliot_b200.h — C ABI of the B200-native embedding-training core.
+ * elliot_b200.h — C ABI of the H100 (sm_90a) embedding-training core.
  *
  * The reference (sisinflab/elliot v0.3.1) is pure Python and has no FFI of its
  * own; its hot path lives in per-model Python classes.  Every entry point below
@@ -55,8 +55,10 @@ int eb_device_info(int *sm_count, int *cc);
 /* Throughput mode: fp32, one launch over n materialised triples, rows updated
  * with 128-bit vector atomics (Hogwild: reads within a launch may be stale).
  * loss (optional, device double[1]) += sum softplus(-(x_ui-x_uj)).
- * flags: bit0 = plain stores instead of atomics (racy Hogwild); bits 8..15 = number of SMs
- * the persistent grid leaves free (so a collective kernel on another stream can run beside it). */
+ * flags: bit0 = plain stores instead of atomics (racy Hogwild); bit6 = deterministic rounds (cooperative launch: every
+ * triple reads the values left by the previous rounds of reads-then-atomic-adds, so reruns give the same tables up to
+ * fp32 summation order; slower); bits 8..15 = number of SMs the persistent grid leaves free (so a collective kernel on
+ * another stream can run beside it).  The same flags apply to the sampled and host-triple variants below. */
 int eb_bpr_step_f32(float *U, float *V, float *item_bias, int d, int ld,
                     const int32_t *tu, const int32_t *ti, const int32_t *tj, int64_t n,
                     float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
@@ -459,7 +461,7 @@ int eb_group_by_owner_i32(const int32_t *a, const int32_t *b, const int32_t *c, 
 int eb_gather_rows_peer_f32(float *const *shards, int n_shards, int32_t shard_rows, int64_t ld, const int32_t *ids, int64_t n,
                             int width, float *out, int64_t ldo, void *stream);
 
-/* Tensor-core path (tcgen05 + TMEM + TMA, bf16 mainloop, exact fp32 re-rank).  Same contract and
+/* Tensor-core path (wgmma + TMA, bf16 mainloop, exact fp32 re-rank).  Same contract and
  * same RESULT as eb_score_topk_f32 (identical index lists and scores): the kernel keeps the 32
  * best bf16-approximate candidates per user, re-scores them exactly in fp32 and certifies the
  * list with a rounding bound; users it cannot certify are re-done by the exact kernel inside

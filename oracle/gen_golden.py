@@ -1,13 +1,13 @@
 #!/usr/bin/env python
-"""Mint golden vectors from the REFERENCE's own code (run in the build container only).
+"""Mint golden vectors from the REFERENCE's own code (needs a checkout of the original project).
 
 The reference ships no tests/golden vectors (SURVEY.md §4).  This script imports
   elliot/dataset/samplers/custom_sampler.py            (Sampler)
   elliot/recommender/latent_factor_models/BPRMF/BPRMF_model.py   (MFModel)
   elliot.dataset.dataset.DataSet, elliot.evaluation.evaluator.Evaluator
-from /root/reference (read-only), runs them unmodified on small seeded synthetic
-data and writes tests/golden/bprmf_<case>.npz.  /root/reference does not exist on
-the GPU box, so tests only ever read the committed .npz files.
+from the original project (REF below, read-only), runs them unmodified on small seeded synthetic
+data and writes tests/golden/bprmf_<case>.npz.  The tests need no copy of the original project:
+they only ever read the committed .npz files.
 
     python oracle/gen_golden.py            # rewrites tests/golden/*.npz
 """
@@ -20,7 +20,8 @@ from types import SimpleNamespace
 import numpy as np
 import pandas as pd
 
-REF = "/root/reference"
+# a checkout of the original Elliot project: $ELLIOT_REFERENCE, or a directory named `reference` beside this repository
+REF = os.environ.get("ELLIOT_REFERENCE") or os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "reference")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
 

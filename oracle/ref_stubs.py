@@ -4,7 +4,7 @@ dependencies tensorflow==2.3.2 and hyperopt are absent.
 `elliot/recommender/__init__.py:12-25` imports every model eagerly and `elliot/run.py:15` imports hyperopt, so without
 them nothing of the reference — not even the pure-NumPy BPRMF — can be driven through `elliot.run.run_experiment`.
 `install()` puts a meta-path finder in front that serves permissive stub modules for exactly those packages (any
-attribute is a subclassable, callable dummy) and puts /root/reference on sys.path.  Nothing of the reference is stubbed
+attribute is a subclassable, callable dummy) and puts the original project (REF) on sys.path.  Nothing of the reference is stubbed
 or modified; code paths that would really call TensorFlow/hyperopt (the TF models, hyper-parameter search) stay out of
 reach and are never used by the generators/tests that call this.
 
@@ -19,7 +19,8 @@ import os
 import sys
 import types
 
-REF = "/root/reference"
+# a checkout of the original Elliot project: $ELLIOT_REFERENCE, or a directory named `reference` beside this repository
+REF = os.environ.get("ELLIOT_REFERENCE") or os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "reference")
 STUBBED = ("tensorflow", "hyperopt", "tensorflow_probability")
 
 

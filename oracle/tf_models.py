@@ -1,7 +1,7 @@
 """fp64 NumPy restatements of the reference's TensorFlow models.  TEST INFRASTRUCTURE ONLY.
 
 PARITY UNPINNED: tensorflow==2.3.2 (requirements.txt:3) is absent from the build container and
-its source is not under /root/reference, so these follow the reference's model code line by
+its source is not part of the original project, so these follow the reference's model code line by
 line plus the published TF 2.3 semantics they rely on (stated per function).  Nothing here was
 checked against a TensorFlow run.  What IS checked: the backward passes against an independent fp64 autodiff of the
 same forward formulas (tests/test_oracle_autograd.py).

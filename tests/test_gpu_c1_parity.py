@@ -8,7 +8,7 @@ the YAML path (VERDICT r1 #2): the golden tests/golden/bprmf_c1.npz was minted b
   throughput mode : (Hogwild, Philox stream — a different but equally distributed triple sequence) nDCG@10 after the
                     same number of epochs, mean over 3 seeds, within HOGWILD_TOL of the reference's; the tolerance is
                     the measured run-to-run spread of the mode, stated here and in DESIGN.md §5.
-Numbers are also written to gpurun_out/c1_parity.json for profiles/.
+With EB_C1_PARITY_JSON=<file> the measured numbers are also written to that file.
 """
 import json
 import os
@@ -21,7 +21,7 @@ from elliot_b200 import synth_c1
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "bprmf_c1.npz")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HOGWILD_TOL = 0.005          # |mean_seeds nDCG@10(hogwild) - nDCG@10(reference)|, absolute (measured: 0.0009; single seeds <= 0.0033)
+HOGWILD_TOL = 0.005          # |mean_seeds nDCG@10(hogwild) - nDCG@10(reference)|, absolute (H100: 0.0006; single seeds <= 0.0031)
 OUT = {}
 
 
@@ -44,9 +44,10 @@ def _run(d, tsv, g, tag, model_extra="", seed=42):
 
 
 def _dump():
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "c1_parity.json"), "w") as fh:
-        json.dump(OUT, fh, indent=1)
+    path = os.environ.get("EB_C1_PARITY_JSON")           # optional record of the measured numbers; the tree stays untouched
+    if path:
+        with open(path, "w") as fh:
+            json.dump(OUT, fh, indent=1)
 
 
 def test_c1_exact_mode_reproduces_the_reference_run(c1):

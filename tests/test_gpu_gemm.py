@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (dense layers of MultiVAE / NeuMF) vs a bf16-rounded fp64 matmul."""
+"""wgmma GEMM (dense layers of MultiVAE / NeuMF) vs a bf16-rounded fp64 matmul."""
 import pytest
 import torch
 

@@ -135,7 +135,7 @@ def test_sharded_model_at_world_1_tracks_the_ordinary_model():
     from elliot_b200.recommender.neumf import NeuralMatrixFactorizationModel
     from elliot_b200.recommender.neumf_sharded import ShardedNeuMFModel
     dev = torch.device(DEV)
-    NU, NI, F, B = 5000, 3000, 64, 4096                       # the configuration verified on the B200 (tools/neumf_sharded_w1.py)
+    NU, NI, F, B = 5000, 3000, 64, 4096                       # the configuration of tools/neumf_sharded_w1.py
     sh = ShardedNeuMFModel(NU, NI, F, 1e-3, 42, dev); ref = NeuralMatrixFactorizationModel(NU, NI, F, 1e-3, 42, dev)
     g = torch.Generator(device=dev); g.manual_seed(1)
     for s in range(3):

@@ -1,7 +1,7 @@
 """Peer-addressed tables (csrc/peer.cu, PEER mode of csrc/bpr_train.cu; SURVEY.md §8e) on ONE GPU: the kernels only see
 an array of shard base addresses, so several shards (or several replicas) allocated on the same device exercise
 exactly the code that runs over NVLink when the shards sit on different GPUs.  The multi-process mapping itself
-(CUDA IPC handles) is covered by tools/peer_check.py under torchrun (results in profiles/)."""
+(CUDA IPC handles) is covered by tools/peer_check.py under torchrun."""
 import numpy as np
 import pytest
 import torch

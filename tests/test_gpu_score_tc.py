@@ -1,4 +1,4 @@
-"""tcgen05 scoring kernel: (1) raw accumulators equal a bf16-rounded matmul, (2) final lists and
+"""wgmma scoring kernel: (1) raw accumulators equal a bf16-rounded matmul, (2) final lists and
 scores are IDENTICAL to the exact CUDA-core kernel (the certification + re-check make the
 tensor-core path exact), incl. masks, biases, ragged sizes and adversarial near-ties."""
 import numpy as np
@@ -14,8 +14,9 @@ DEV = "cuda:0"
 @pytest.fixture(autouse=True, params=[("2", "0", "0"), ("1", "0", "0"), ("2", "1", "0"), ("2", "0", "1")],
                 ids=["two_epilogue_groups", "one_epilogue_group", "cta_pairs", "users_in_tmem"])
 def _kernel_variant(request, monkeypatch):
-    """every test runs against the four kernels: two epilogue warpgroups, one (EB_TC_NG=1), CTA pairs sharing each item
-    tile through tcgen05 cta_group::2 (EB_TC_PAIR=1), and the user block held in TMEM (EB_TC_ATM=1)"""
+    """every test runs against the four kernels: two consumer warpgroups, one (EB_TC_NG=1), CTA pairs sharing each item
+    tile through TMA multicast (EB_TC_PAIR=1), and the user block held in registers as the wgmma A operand (EB_TC_ATM=1;
+    the id keeps its historical name)"""
     monkeypatch.setenv("EB_TC_NG", request.param[0])
     monkeypatch.setenv("EB_TC_PAIR", request.param[1])
     monkeypatch.setenv("EB_TC_ATM", request.param[2])

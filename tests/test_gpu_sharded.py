@@ -1,6 +1,6 @@
 """Row-sharded item tables (SURVEY.md §8e): kernels + the fetch/update/push protocol at world size 1 against the
 replicated-table kernel and the oracle; the multi-rank exchange itself is covered by tests/test_parallel_cpu.py
-(gloo) and tools/sharded_check.py (torchrun on 2+ GPUs, results in profiles/)."""
+(gloo) and tools/sharded_check.py (torchrun on 2+ GPUs)."""
 import numpy as np
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Split-K path of the tcgen05 GEMM (no bias / activation, few output tiles, long K: partial tiles are added into a
+"""Split-K path of the wgmma GEMM (no bias / activation, few output tiles, long K: partial tiles are added into a
 zeroed C with vector atomics) vs a bf16-rounded fp64 matmul.  The path is also exercised through the MultiVAE tests
 (dh2 = dlogits . W4); this file sorts last on purpose."""
 import pytest

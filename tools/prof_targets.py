@@ -32,7 +32,7 @@ if what in ("hogwild", "hogwild_large"):
         ops.bpr_step_sampled_f32(U, V, b, d, nu, ni, ip, ix, B, 42, s * B, *HP, filter=f)
     torch.cuda.synchronize()
 elif what in ("score_c2", "score_c5"):
-    nu = 148 * 128 * 2
+    nu = 132 * 128 * 2
     ni, d = (100_000, 64) if what == "score_c2" else (2_000_000, 128)
     U = torch.randn(nu, d, device=dev) * 0.1; V = torch.randn(ni, d, device=dev) * 0.1; b = torch.randn(ni, device=dev) * 0.05
     ip, ix = csr(nu, ni, 100, 5)

@@ -26,41 +26,41 @@ def run(nu, ni, d, k, per_user, label):
     print("   identical to exact kernel on 512 users:", torch.equal(i0, i1[:512]), torch.equal(v0, v1[:512]))
 if len(sys.argv) > 1 and sys.argv[1] == "ab":
     # A/B of the epilogue layouts; EB_TC_DEBUG=3 certifies everything (no re-check) so the main kernel is timed alone;
-    # EB_TC_PROF=1 adds warp 2's cycle counters (accumulator wait, TMEM load, scan, compaction, re-rank; counts)
+    # EB_TC_PROF=1 adds warp 0's cycle counters (stage wait, MMA + staging, scan, compaction, re-rank; counts)
     os.environ["EB_TC_PROF"] = "1"
     for ng in ("1", "2"):
         for dbg in ("0", "3"):
             os.environ["EB_TC_NG"] = ng; os.environ["EB_TC_DEBUG"] = dbg
-            run(148 * 128 * 2, 100_000, 64, 10, 100, f"C2 ng={ng} dbg={dbg}")
-            run(148 * 128 * 2, 2_000_000, 128, 10, 100, f"C5 ng={ng} dbg={dbg}")
+            run(132 * 128 * 2, 100_000, 64, 10, 100, f"C2 ng={ng} dbg={dbg}")
+            run(132 * 128 * 2, 2_000_000, 128, 10, 100, f"C5 ng={ng} dbg={dbg}")
     sys.exit(0)
 if len(sys.argv) > 1 and sys.argv[1] == "pair":
-    # single CTAs against CTA pairs (tcgen05 cta_group::2: the item tile is fetched once per 256 users)
+    # single CTAs against CTA pairs (clusters of two, each item tile fetched half by each CTA and multicast to both)
     os.environ["EB_TC_PROF"] = "1"; os.environ["EB_TC_NG"] = "2"
     for pair in ("0", "1"):
         for dbg in ("0", "1"):
             os.environ["EB_TC_PAIR"] = pair; os.environ["EB_TC_DEBUG"] = dbg
-            run(148 * 128 * 2, 100_000, 64, 10, 100, f"C2 pair={pair} dbg={dbg}")
-            run(148 * 128 * 2, 2_000_000, 128, 10, 100, f"C5 pair={pair} dbg={dbg}")
+            run(132 * 128 * 2, 100_000, 64, 10, 100, f"C2 pair={pair} dbg={dbg}")
+            run(132 * 128 * 2, 2_000_000, 128, 10, 100, f"C5 pair={pair} dbg={dbg}")
     sys.exit(0)
 if len(sys.argv) > 1 and sys.argv[1] == "atm":
-    # the user block in shared memory against the user block in TMEM
+    # the user block in shared memory against the user block in registers (wgmma A operand)
     os.environ["EB_TC_PROF"] = "1"; os.environ["EB_TC_NG"] = "2"; os.environ["EB_TC_PAIR"] = "0"
     for atm in ("0", "1"):
         for dbg in ("0", "1"):
             os.environ["EB_TC_ATM"] = atm; os.environ["EB_TC_DEBUG"] = dbg
-            run(148 * 128 * 2, 100_000, 64, 10, 100, f"C2 atm={atm} dbg={dbg}")
-            run(148 * 128 * 2, 2_000_000, 128, 10, 100, f"C5 atm={atm} dbg={dbg}")
+            run(132 * 128 * 2, 100_000, 64, 10, 100, f"C2 atm={atm} dbg={dbg}")
+            run(132 * 128 * 2, 2_000_000, 128, 10, 100, f"C5 atm={atm} dbg={dbg}")
     sys.exit(0)
 if len(sys.argv) > 1 and sys.argv[1] == "feed":
-    # EB_TC_DEBUG=1: the epilogue only reads TMEM and takes the max (no inserts): the TMA/MMA pipeline's own pace
+    # EB_TC_DEBUG=1: the epilogue only reads the accumulators and takes the max (no inserts): the TMA/MMA pipeline's own pace
     os.environ["EB_TC_PROF"] = "1"
     for ng in ("1", "2"):
         for dbg in ("1", "2"):
             os.environ["EB_TC_NG"] = ng; os.environ["EB_TC_DEBUG"] = dbg
-            run(148 * 128 * 2, 100_000, 64, 10, 100, f"C2 ng={ng} dbg={dbg}")
-            run(148 * 128 * 2, 2_000_000, 128, 10, 100, f"C5 ng={ng} dbg={dbg}")
+            run(132 * 128 * 2, 100_000, 64, 10, 100, f"C2 ng={ng} dbg={dbg}")
+            run(132 * 128 * 2, 2_000_000, 128, 10, 100, f"C5 ng={ng} dbg={dbg}")
     sys.exit(0)
-run(148 * 128 * 4, 100_000, 64, 10, 100, "C2-shape")
-run(148 * 128 * 2, 2_000_000, 128, 10, 100, "C5-shape(per-GPU slice)")
+run(132 * 128 * 4, 100_000, 64, 10, 100, "C2-shape")
+run(132 * 128 * 2, 2_000_000, 128, 10, 100, "C5-shape(per-GPU slice)")
 run(6040, 3706, 64, 10, 130, "C1-shape")
