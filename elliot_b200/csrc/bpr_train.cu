@@ -18,7 +18,9 @@
 #include <cub/cub.cuh>
 #include <stdlib.h>
 
-#include "common.cuh"
+#include <type_traits>
+
+#include "bpr_update.cuh"
 
 namespace eb {
 
@@ -27,7 +29,7 @@ struct HogwildParams {
     int ld;
     const int32_t *tu, *ti, *tj;
     int64_t n;
-    float lr, reg_u, reg_b, reg_pos, reg_neg;
+    BprHyper hp;
     double *loss;
     // sampler
     int32_t n_users, n_items;
@@ -36,10 +38,10 @@ struct HogwildParams {
     uint64_t seed, first;
     int32_t *out_u, *out_i, *out_j;
     // PEER mode (item table row-sharded over the GPUs of one NVSwitch box, SURVEY.md §8e): shard s holds item rows
-    // [s*shard_rows, (s+1)*shard_rows) at Vp[s] / bp[s] — local memory for this rank's shard, peer-mapped memory
+    // [s*shards.rows, (s+1)*shards.rows) at Vp[s] / bp[s] — local memory for this rank's shard, peer-mapped memory
     // (cudaIpcOpenMemHandle, peer.cu) for the others; loads and vector atomics go straight over NVLink.
     float *Vp[EB_MAX_PEERS], *bp[EB_MAX_PEERS];
-    uint32_t shard_rows, shard_magic;          // magic = floor(2^32 / shard_rows)
+    ShardMap shards;
     // optional per-user membership signatures (eb_bloom_build): filter_log2bits bits per user
     const uint32_t *filter;
     int filter_log2bits;
@@ -48,15 +50,6 @@ struct HogwildParams {
     int bits_u, bits_i;
     int no_item_updates;      // profiling only (flags bit 2): item rows are read but not updated
 };
-
-// owner shard and row inside it (one multiply-high and one correction instead of an integer division)
-__device__ __forceinline__ void shard_of(const HogwildParams &p, int i, int &owner, int &local) {
-    uint32_t o = __umulhi((uint32_t)i, p.shard_magic);
-    uint32_t r = (uint32_t)i - o * p.shard_rows;
-    if (r >= p.shard_rows) { o++; r -= p.shard_rows; }
-    owner = (int)o; local = (int)r;
-}
-
 
 // u uniform over users, i uniform over the user's train items, j uniform over the
 // complement (rejection against the sorted CSR row) — custom_sampler.py:31-42 semantics,
@@ -102,6 +95,34 @@ __device__ __forceinline__ void sample_triple(const HogwildParams &p, int64_t t,
     j = cand;
 }
 
+// triple t: sampled (and written to out_* when asked), unpacked from the 8-byte host format, or read from three arrays
+template <bool SAMPLE>
+__device__ __forceinline__ void fetch_triple(const HogwildParams &p, int64_t t, int &u, int &i, int &j) {
+    if (SAMPLE) {
+        sample_triple(p, t, u, i, j);
+        if (p.out_u) { p.out_u[t] = u; p.out_i[t] = i; p.out_j[t] = j; }
+    } else if (p.packed) {
+        const uint64_t w = __ldg(p.packed + t);
+        u = (int)(w & ((1ull << p.bits_u) - 1));
+        i = (int)((w >> p.bits_u) & ((1ull << p.bits_i) - 1));
+        j = (int)(w >> (p.bits_u + p.bits_i));
+    } else {
+        u = __ldg(p.tu + t); i = __ldg(p.ti + t); j = __ldg(p.tj + t);
+    }
+}
+
+// item row / bias addresses: one table, or the owner shard's (possibly peer-mapped) memory
+template <bool PEER>
+__device__ __forceinline__ void item_row(const HogwildParams &p, int i, float *&row, float *&bias) {
+    if constexpr (PEER) {
+        int o, l;
+        p.shards.locate(i, o, l);
+        row = p.Vp[o] + (int64_t)l * p.ld; bias = p.bp[o] + l;
+    } else {
+        row = p.V + (int64_t)i * p.ld; bias = p.b + i;
+    }
+}
+
 template <int VPL>
 struct Rows {
     float4 u[VPL], vi[VPL], vj[VPL];
@@ -130,20 +151,10 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
     const int64_t ld = p.ld;
     float loss_acc = 0.f;
 
-    // item row / bias addresses: one table, or the owner shard's (possibly peer-mapped) memory
-    auto item_row = [&](int i, float *&row, float *&bias) {
-        if constexpr (PEER) {
-            int o, l;
-            shard_of(p, i, o, l);
-            row = p.Vp[o] + (int64_t)l * ld; bias = p.bp[o] + l;
-        } else {
-            row = p.V + (int64_t)i * ld; bias = p.b + i;
-        }
-    };
     auto load_rows = [&](Rows<VPL> &r, int u, int i, int j) {
         if (u >= 0) {
             float *ri, *rj, *bi, *bj;
-            item_row(i, ri, bi); item_row(j, rj, bj);
+            item_row<PEER>(p, i, ri, bi); item_row<PEER>(p, j, rj, bj);
             const float4 *pu = reinterpret_cast<const float4 *>(p.U + (int64_t)u * ld);
             const float4 *pi = reinterpret_cast<const float4 *>(ri);
             const float4 *pj = reinterpret_cast<const float4 *>(rj);
@@ -164,21 +175,7 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
     for (int64_t tile = warp_id; tile < tile_end; tile += nwarps) {
         const int64_t t = tile * 32 + lane;
         int u = -1, i = 0, j = 0;
-        if (t < p.n) {
-            if (SAMPLE) {
-                sample_triple(p, t, u, i, j);
-                if (p.out_u) { p.out_u[t] = u; p.out_i[t] = i; p.out_j[t] = j; }
-            } else {
-                if (p.packed) {
-                    const uint64_t w = __ldg(p.packed + t);
-                    u = (int)(w & ((1ull << p.bits_u) - 1));
-                    i = (int)((w >> p.bits_u) & ((1ull << p.bits_i) - 1));
-                    j = (int)(w >> (p.bits_u + p.bits_i));
-                } else {
-                    u = __ldg(p.tu + t); i = __ldg(p.ti + t); j = __ldg(p.tj + t);
-                }
-            }
-        }
+        if (t < p.n) fetch_triple<SAMPLE>(p, t, u, i, j);
         // UNR triples of the group in flight at once: all their row loads are issued before the first reduction
         constexpr int UNR = G >= 4 ? 4 : G;
 #pragma unroll 1
@@ -201,34 +198,19 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
                     float part = 0.f;
                     if (tu_[q] >= 0) {
 #pragma unroll
-                        for (int v = 0; v < VPL; v++) {
-                            part += cur.u[v].x * (cur.vi[v].x - cur.vj[v].x) + cur.u[v].y * (cur.vi[v].y - cur.vj[v].y) +
-                                    cur.u[v].z * (cur.vi[v].z - cur.vj[v].z) + cur.u[v].w * (cur.vi[v].w - cur.vj[v].w);
-                        }
+                        for (int v = 0; v < VPL; v++) part += bpr_partial_dot(cur.u[v], cur.vi[v], cur.vj[v]);
                     }
-#pragma unroll
-                    for (int off = G / 2; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
+                    part = group_sum<G>(part);
                     if (tu_[q] >= 0) {
-                        const float x = part + (cur.bi - cur.bj);
-                        const float z = __fdividef(1.f, 1.f + __expf(x));  // BPRMF_model.py:98
-                        if (gl == 0) loss_acc += fmaxf(-x, 0.f) + __logf(1.f + __expf(-fabsf(x)));
+                        const float z = bpr_sigmoid_loss(part + (cur.bi - cur.bj), loss_acc, gl);
 #pragma unroll
                         for (int v = 0; v < VPL; v++) {
-                            const float4 a = cur.u[v], bi4 = cur.vi[v], bj4 = cur.vj[v];
-                            float4 du, un;
-                            du.x = p.lr * ((bi4.x - bj4.x) * z - p.reg_u * a.x);
-                            du.y = p.lr * ((bi4.y - bj4.y) * z - p.reg_u * a.y);
-                            du.z = p.lr * ((bi4.z - bj4.z) * z - p.reg_u * a.z);
-                            du.w = p.lr * ((bi4.w - bj4.w) * z - p.reg_u * a.w);
-                            un.x = a.x + du.x; un.y = a.y + du.y; un.z = a.z + du.z; un.w = a.w + du.w;
-                            // item rows see the UPDATED user row (view aliasing, BPRMF_model.py:92,109-116)
-                            cur.vi[v] = make_float4(p.lr * (un.x * z - p.reg_pos * bi4.x), p.lr * (un.y * z - p.reg_pos * bi4.y),
-                                                    p.lr * (un.z * z - p.reg_pos * bi4.z), p.lr * (un.w * z - p.reg_pos * bi4.w));
-                            cur.vj[v] = make_float4(p.lr * (-un.x * z - p.reg_neg * bj4.x), p.lr * (-un.y * z - p.reg_neg * bj4.y),
-                                                    p.lr * (-un.z * z - p.reg_neg * bj4.z), p.lr * (-un.w * z - p.reg_neg * bj4.w));
-                            cur.u[v] = du;
+                            float4 du, di, dj;
+                            bpr_row_deltas(cur.u[v], cur.vi[v], cur.vj[v], z, p.hp, du, di, dj);
+                            cur.u[v] = du; cur.vi[v] = di; cur.vj[v] = dj;
                         }
-                        const float dbi = p.lr * (z - p.reg_b * cur.bi), dbj = p.lr * (-z - p.reg_b * cur.bj);
+                        float dbi, dbj;
+                        bpr_bias_deltas(z, cur.bi, cur.bj, p.hp, dbi, dbj);
                         cur.bi = dbi; cur.bj = dbj;
                     }
                 }
@@ -238,7 +220,7 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
                 for (int q = 0; q < UNR; q++) {
                     if (tu_[q] < 0) continue;
                     float *pu = p.U + (int64_t)tu_[q] * ld, *pi, *pj, *pbi, *pbj;
-                    item_row(ti_[q], pi, pbi); item_row(tj_[q], pj, pbj);
+                    item_row<PEER>(p, ti_[q], pi, pbi); item_row<PEER>(p, tj_[q], pj, pbj);
 #pragma unroll
                     for (int v = 0; v < VPL; v++) {
                         const int e = (v * G + gl) * 4;
@@ -255,41 +237,21 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
             for (int q = 0; q < UNR; q++) {
                 const Rows<VPL> &cur = rw[q];
                 const int cu = tu_[q], ci = ti_[q], cj = tj_[q];
-                // ---- score: x = (b_i - b_j) + U[u].(V_i - V_j)
                 float part = 0.f;
                 if (cu >= 0) {
 #pragma unroll
-                    for (int v = 0; v < VPL; v++) {
-                        part += cur.u[v].x * (cur.vi[v].x - cur.vj[v].x) + cur.u[v].y * (cur.vi[v].y - cur.vj[v].y) +
-                                cur.u[v].z * (cur.vi[v].z - cur.vj[v].z) + cur.u[v].w * (cur.vi[v].w - cur.vj[v].w);
-                    }
+                    for (int v = 0; v < VPL; v++) part += bpr_partial_dot(cur.u[v], cur.vi[v], cur.vj[v]);
                 }
-#pragma unroll
-                for (int off = G / 2; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
+                part = group_sum<G>(part);
                 if (cu >= 0) {
-                    const float x = part + (cur.bi - cur.bj);
-                    const float z = __fdividef(1.f, 1.f + __expf(x));  // BPRMF_model.py:98
-                    if (gl == 0) loss_acc += fmaxf(-x, 0.f) + __logf(1.f + __expf(-fabsf(x)));
+                    const float z = bpr_sigmoid_loss(part + (cur.bi - cur.bj), loss_acc, gl);
                     float *pu = p.U + (int64_t)cu * ld, *pi, *pj, *pbi, *pbj;
-                    item_row(ci, pi, pbi); item_row(cj, pj, pbj);
+                    item_row<PEER>(p, ci, pi, pbi); item_row<PEER>(p, cj, pj, pbj);
 #pragma unroll
                     for (int v = 0; v < VPL; v++) {
-                        const float4 a = cur.u[v], bi4 = cur.vi[v], bj4 = cur.vj[v];
-                        float4 du, di, dj, un;
-                        du.x = p.lr * ((bi4.x - bj4.x) * z - p.reg_u * a.x);
-                        du.y = p.lr * ((bi4.y - bj4.y) * z - p.reg_u * a.y);
-                        du.z = p.lr * ((bi4.z - bj4.z) * z - p.reg_u * a.z);
-                        du.w = p.lr * ((bi4.w - bj4.w) * z - p.reg_u * a.w);
-                        un.x = a.x + du.x; un.y = a.y + du.y; un.z = a.z + du.z; un.w = a.w + du.w;
-                        // item rows see the UPDATED user row (view aliasing, BPRMF_model.py:92,109-116)
-                        di.x = p.lr * (un.x * z - p.reg_pos * bi4.x);
-                        di.y = p.lr * (un.y * z - p.reg_pos * bi4.y);
-                        di.z = p.lr * (un.z * z - p.reg_pos * bi4.z);
-                        di.w = p.lr * (un.w * z - p.reg_pos * bi4.w);
-                        dj.x = p.lr * (-un.x * z - p.reg_neg * bj4.x);
-                        dj.y = p.lr * (-un.y * z - p.reg_neg * bj4.y);
-                        dj.z = p.lr * (-un.z * z - p.reg_neg * bj4.z);
-                        dj.w = p.lr * (-un.w * z - p.reg_neg * bj4.w);
+                        const float4 a = cur.u[v], vi = cur.vi[v], vj = cur.vj[v];
+                        float4 du, di, dj;
+                        bpr_row_deltas(a, vi, vj, z, p.hp, du, di, dj);
                         const int e = (v * G + gl) * 4;
                         if (PEER) {
                             red_add_v4(pu + e, du);
@@ -302,15 +264,14 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
                             red_add_v4(pi + e, di);
                             red_add_v4(pj + e, dj);
                         } else {
-                            *reinterpret_cast<float4 *>(pu + e) = un;
-                            *reinterpret_cast<float4 *>(pi + e) =
-                                make_float4(bi4.x + di.x, bi4.y + di.y, bi4.z + di.z, bi4.w + di.w);
-                            *reinterpret_cast<float4 *>(pj + e) =
-                                make_float4(bj4.x + dj.x, bj4.y + dj.y, bj4.z + dj.z, bj4.w + dj.w);
+                            *reinterpret_cast<float4 *>(pu + e) = make_float4(a.x + du.x, a.y + du.y, a.z + du.z, a.w + du.w);
+                            *reinterpret_cast<float4 *>(pi + e) = make_float4(vi.x + di.x, vi.y + di.y, vi.z + di.z, vi.w + di.w);
+                            *reinterpret_cast<float4 *>(pj + e) = make_float4(vj.x + dj.x, vj.y + dj.y, vj.z + dj.z, vj.w + dj.w);
                         }
                     }
                     if (gl == 0) {
-                        const float dbi = p.lr * (z - p.reg_b * cur.bi), dbj = p.lr * (-z - p.reg_b * cur.bj);
+                        float dbi, dbj;
+                        bpr_bias_deltas(z, cur.bi, cur.bj, p.hp, dbi, dbj);
                         if (PEER) { red_add_f32_sys(pbi, dbi); red_add_f32_sys(pbj, dbj); }
                         else if (ATOMIC) { red_add_f32(pbi, dbi); red_add_f32(pbj, dbj); }
                         else { *pbi = cur.bi + dbi; *pbj = cur.bj + dbj; }
@@ -326,9 +287,9 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
     }
 }
 
-// ---------------------------------------------------------------- staged variant of the Hogwild kernel
-// Same arithmetic, same sampler, same atomics as bpr_hogwild_kernel; the difference is HOW the three embedding rows of
-// a triple reach the SM.  There every lane group loads "its" rows into registers (4 triples in flight per group, 118
+// ---------------------------------------------------------------- staged variant of the Hogwild kernel (PEER mode only)
+// Same update, same sampler, same atomics as bpr_hogwild_kernel<..., PEER = true>; the difference is HOW the three
+// embedding rows of a triple reach the SM.  There every lane group loads "its" rows into registers (4 triples in flight per group, 118
 // registers, 16 warps/SM) and the loads of a round cannot start before the previous round's arithmetic has retired.
 // Here every lane, as soon as it has sampled its triple, hands the three rows to the copy engine
 // (cp.async.bulk global -> shared, completion on a per-warp mbarrier): 3 x TT row copies per warp are in flight with NO
@@ -337,13 +298,14 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
 // PEER GPU's memory (PEER mode: 2-3x the latency of local HBM) arrive without stalling the arithmetic.
 // TT rows-triples per warp chunk: 12 KB of shared memory per warp whatever the row length (DP = 32/64/128 floats); halving the
 // chunk to fit 4 CTAs per SM was measured SLOWER (1.32 vs 1.01 ms at C2): the step is not short of resident warps.
-template <int DP, bool SAMPLE, bool PEER, int CHUNK_BYTES = 4096>
+constexpr int STAGE_CHUNK_BYTES = 4096;
+template <int DP, bool SAMPLE>
 __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildParams p) {
     constexpr int NV = DP / 4;                 // float4 per row
     constexpr int G = NV >= 32 ? 32 : NV;      // lanes per triple
     constexpr int VPL = NV / G;                // float4 per lane
     constexpr int ROWB = DP * 4;
-    constexpr int TT = CHUNK_BYTES / ROWB;     // triples per chunk (32 / 16 / 8 at 4 KB of rows per row kind)
+    constexpr int TT = STAGE_CHUNK_BYTES / ROWB;  // triples per chunk (32 / 16 / 8 at 4 KB of rows per row kind)
     constexpr int NGRP = 32 / G;               // triples processed side by side
     static_assert(TT >= NGRP && TT <= 32 && 32 % TT == 0, "chunk shape");
     extern __shared__ __align__(128) uint8_t stage_smem[];
@@ -364,35 +326,15 @@ __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildPar
     const int64_t ld = p.ld;
     float loss_acc = 0.f;
 
-    auto item_row = [&](int i, float *&row, float *&bias) {
-        if constexpr (PEER) {
-            int o, l;
-            shard_of(p, i, o, l);
-            row = p.Vp[o] + (int64_t)l * ld; bias = p.bp[o] + l;
-        } else {
-            row = p.V + (int64_t)i * ld; bias = p.b + i;
-        }
-    };
-
     for (int64_t tile = warp_id; tile * 32 < p.n; tile += nwarps) {
         const int64_t t = tile * 32 + lane;
         int u = -1, i = 0, j = 0;
         float bi = 0.f, bj = 0.f;
         float *pu = nullptr, *pi = nullptr, *pj = nullptr, *pbi = nullptr, *pbj = nullptr;
         if (t < p.n) {
-            if (SAMPLE) {
-                sample_triple(p, t, u, i, j);
-                if (p.out_u) { p.out_u[t] = u; p.out_i[t] = i; p.out_j[t] = j; }
-            } else if (p.packed) {
-                const uint64_t w = __ldg(p.packed + t);
-                u = (int)(w & ((1ull << p.bits_u) - 1));
-                i = (int)((w >> p.bits_u) & ((1ull << p.bits_i) - 1));
-                j = (int)(w >> (p.bits_u + p.bits_i));
-            } else {
-                u = __ldg(p.tu + t); i = __ldg(p.ti + t); j = __ldg(p.tj + t);
-            }
+            fetch_triple<SAMPLE>(p, t, u, i, j);
             pu = p.U + (int64_t)u * ld;
-            item_row(i, pi, pbi); item_row(j, pj, pbj);
+            item_row<true>(p, i, pi, pbi); item_row<true>(p, j, pj, pbj);
         }
         const bool valid = u >= 0;
 #pragma unroll 1
@@ -437,48 +379,26 @@ __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildPar
 #pragma unroll
                 for (int v = 0; v < VPL; v++) {
                     a[v] = su[v * G + gl]; vi[v] = su[NV + v * G + gl]; vj[v] = su[2 * NV + v * G + gl];
-                    part += a[v].x * (vi[v].x - vj[v].x) + a[v].y * (vi[v].y - vj[v].y) + a[v].z * (vi[v].z - vj[v].z) +
-                            a[v].w * (vi[v].w - vj[v].w);
+                    part += bpr_partial_dot(a[v], vi[v], vj[v]);
                 }
                 if (!on) part = 0.f;
-#pragma unroll
-                for (int off = G / 2; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
+                part = group_sum<G>(part);
                 if (on) {
-                    const float x = part + (cbi - cbj);
-                    const float z = __fdividef(1.f, 1.f + __expf(x));  // BPRMF_model.py:98
-                    if (gl == 0) loss_acc += fmaxf(-x, 0.f) + __logf(1.f + __expf(-fabsf(x)));
+                    const float z = bpr_sigmoid_loss(part + (cbi - cbj), loss_acc, gl);
                     float *gu = p.U + (int64_t)cu * ld, *gi, *gj, *gbi, *gbj;
-                    item_row(ci, gi, gbi); item_row(cj, gj, gbj);
+                    item_row<true>(p, ci, gi, gbi); item_row<true>(p, cj, gj, gbj);
 #pragma unroll
                     for (int v = 0; v < VPL; v++) {
-                        const float4 av = a[v], bi4 = vi[v], bj4 = vj[v];
-                        float4 du, di, dj, un;
-                        du.x = p.lr * ((bi4.x - bj4.x) * z - p.reg_u * av.x);
-                        du.y = p.lr * ((bi4.y - bj4.y) * z - p.reg_u * av.y);
-                        du.z = p.lr * ((bi4.z - bj4.z) * z - p.reg_u * av.z);
-                        du.w = p.lr * ((bi4.w - bj4.w) * z - p.reg_u * av.w);
-                        un.x = av.x + du.x; un.y = av.y + du.y; un.z = av.z + du.z; un.w = av.w + du.w;
-                        // item rows see the UPDATED user row (view aliasing, BPRMF_model.py:92,109-116)
-                        di.x = p.lr * (un.x * z - p.reg_pos * bi4.x);
-                        di.y = p.lr * (un.y * z - p.reg_pos * bi4.y);
-                        di.z = p.lr * (un.z * z - p.reg_pos * bi4.z);
-                        di.w = p.lr * (un.w * z - p.reg_pos * bi4.w);
-                        dj.x = p.lr * (-un.x * z - p.reg_neg * bj4.x);
-                        dj.y = p.lr * (-un.y * z - p.reg_neg * bj4.y);
-                        dj.z = p.lr * (-un.z * z - p.reg_neg * bj4.z);
-                        dj.w = p.lr * (-un.w * z - p.reg_neg * bj4.w);
+                        float4 du, di, dj;
+                        bpr_row_deltas(a[v], vi[v], vj[v], z, p.hp, du, di, dj);
                         const int e = (v * G + gl) * 4;
                         red_add_v4(gu + e, du);
-                        if (PEER) {
-                            if (!p.no_item_updates) { red_add_v4_sys(gi + e, di); red_add_v4_sys(gj + e, dj); }
-                        } else {
-                            red_add_v4(gi + e, di); red_add_v4(gj + e, dj);
-                        }
+                        if (!p.no_item_updates) { red_add_v4_sys(gi + e, di); red_add_v4_sys(gj + e, dj); }
                     }
                     if (gl == 0) {
-                        const float dbi = p.lr * (z - p.reg_b * cbi), dbj = p.lr * (-z - p.reg_b * cbj);
-                        if (PEER) { red_add_f32_sys(gbi, dbi); red_add_f32_sys(gbj, dbj); }
-                        else { red_add_f32(gbi, dbi); red_add_f32(gbj, dbj); }
+                        float dbi, dbj;
+                        bpr_bias_deltas(z, cbi, cbj, p.hp, dbi, dbj);
+                        red_add_f32_sys(gbi, dbi); red_add_f32_sys(gbj, dbj);
                     }
                 }
             }
@@ -491,37 +411,32 @@ __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildPar
     }
 }
 
-template <int DP, bool SAMPLE, bool PEER, int CHUNK_BYTES = 4096>
-static int launch_stage_t(const HogwildParams &p, int reserve_sms, cudaStream_t st) {
-    constexpr int SMEM = 8 * 3 * CHUNK_BYTES + 64;         // 8 warps x 3 row kinds x chunk + mbarriers
-    auto kern = bpr_hogwild_stage_kernel<DP, SAMPLE, PEER, CHUNK_BYTES>;
-    EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+// Persistent grid of 256-thread CTAs: one CTA per 8 tiles of 32 triples (a tile per warp), at most what stays resident on the
+// SMs left after `reserve_sms` (SMs left free for a concurrent collective (NCCL) kernel).
+static int persistent_grid(const void *kern, int smem, int64_t n, int reserve_sms, unsigned &grid) {
     int per_sm = 0;
-    EB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, SMEM));
+    EB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem));
     if (per_sm < 1) per_sm = 1;
-    int64_t tiles = (p.n + 31) / 32;
-    int64_t want = (tiles + 7) / 8;
+    const int64_t tiles = (n + 31) / 32;
+    const int64_t want = (tiles + 7) / 8;
     int sms = sm_count() - reserve_sms;
     if (sms < 1) sms = 1;
-    int64_t grid = (int64_t)sms * per_sm;
-    if (want < grid) grid = want;
-    if (grid < 1) grid = 1;
-    kern<<<(unsigned)grid, 256, SMEM, st>>>(p);
-    EB_CUDA(cudaGetLastError());
+    int64_t g = (int64_t)sms * per_sm;
+    if (want < g) g = want;
+    grid = (unsigned)(g < 1 ? 1 : g);
     return EB_OK;
 }
 
-// Which kernel: flags bit 4 (16) forces the register-staged kernel, bit 5 (32) the shared-memory-staged one; otherwise the
-// default — on ONE local table the register kernel; with the item table spread over peer GPUs the staged kernel is the
-// default (`peer_default`): its row copies are in flight without holding registers while the rows cross NVLink.
-static bool use_stage(int dp, int flags, bool peer_default) {
-    static const int env = [] { const char *e = getenv("EB_HOGWILD_STAGE"); return e ? atoi(e) : -1; }();
-    if (!(dp == 32 || dp == 64 || dp == 128)) return false;
-    if (flags & 1) return false;                            // racy (non-atomic) mode exists only in the register kernel
-    if (flags & 16) return false;
-    if (flags & 32) return true;
-    if (env >= 0) return env != 0;
-    return peer_default;
+template <int DP, bool SAMPLE>
+static int launch_stage_t(const HogwildParams &p, int reserve_sms, cudaStream_t st) {
+    constexpr int SMEM = 8 * 3 * STAGE_CHUNK_BYTES + 64;   // 8 warps x 3 row kinds x chunk + mbarriers
+    auto kern = bpr_hogwild_stage_kernel<DP, SAMPLE>;
+    EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    unsigned grid;
+    if (int rc = persistent_grid((const void *)kern, SMEM, p.n, reserve_sms, grid)) return rc;
+    kern<<<grid, 256, SMEM, st>>>(p);
+    EB_CUDA(cudaGetLastError());
+    return EB_OK;
 }
 
 // one warp per user: OR the two signature bits of every train item into the user's words
@@ -571,28 +486,28 @@ __global__ void __launch_bounds__(256) pointwise_sample_kernel(const HogwildPara
     }
 }
 
-template <int DP, bool SAMPLE, bool ATOMIC, bool PEER = false, bool ROUNDS = false>
+template <int DP, bool SAMPLE, bool ATOMIC, bool PEER, bool ROUNDS>
 static int launch_hogwild_t(const HogwildParams &p, int reserve_sms, cudaStream_t st) {
-    int per_sm = 0;
-    EB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER, ROUNDS>, 256, 0));
-    if (per_sm < 1) per_sm = 1;
-    int64_t tiles = (p.n + 31) / 32;
-    int64_t want = (tiles + 7) / 8;
-    int sms = sm_count() - reserve_sms;  // SMs left free for a concurrent collective (NCCL) kernel
-    if (sms < 1) sms = 1;
-    int64_t grid = (int64_t)sms * per_sm;
-    if (want < grid) grid = want;
-    if (grid < 1) grid = 1;
+    auto kern = bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER, ROUNDS>;
+    unsigned grid;
+    if (int rc = persistent_grid((const void *)kern, 0, p.n, reserve_sms, grid)) return rc;
     if (ROUNDS) {
         // deterministic rounds (see bpr_hogwild_kernel): a cooperative launch, so every CTA is resident for the grid barriers
         void *args[] = {const_cast<HogwildParams *>(&p)};
-        EB_CUDA(cudaLaunchCooperativeKernel((const void *)bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER, ROUNDS>, dim3((unsigned)grid),
-                                            dim3(256), args, 0, st));
+        EB_CUDA(cudaLaunchCooperativeKernel((const void *)kern, dim3(grid), dim3(256), args, 0, st));
     } else {
-        bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER><<<(unsigned)grid, 256, 0, st>>>(p);
+        kern<<<grid, 256, 0, st>>>(p);
     }
     EB_CUDA(cudaGetLastError());
     return EB_OK;
+}
+
+// f(std::integral_constant<int, DP>{}) for the row stride DP == dp among the compiled ones (DPS), else EB_ERR_ARG
+template <int... DPS, class F>
+static int with_stride(int dp, const char *strides, F &&f) {
+    int rc = EB_OK;
+    const bool found = ((dp == DPS && (rc = f(std::integral_constant<int, DPS>{}), true)) || ...);
+    return found ? rc : set_err(EB_ERR_ARG, "row stride ld=%d must be one of %s", dp, strides);
 }
 
 // EB_L2_PERSIST=1: mark the item table's address range as persisting in L2 for the launch's stream (cudaAccessPolicyWindow) when it
@@ -625,53 +540,29 @@ static int launch_hogwild(const HogwildParams &p, int dp, int flags, cudaStream_
     const bool atomic = !(flags & 1);
     const bool rounds = (flags & 64) != 0;
     const int reserve = (flags >> 8) & 0xff;
+    EB_ARG(!(flags & 32), "the shared-memory-staged kernel exists for sharded item tables only");
+    EB_ARG(atomic || !rounds, "deterministic rounds run with atomic updates");
     item_table_l2_window(p, st);
-    if (rounds) {
-        EB_ARG(atomic && !(flags & 32), "deterministic rounds run in the register kernel with atomic updates");
-#define EB_CASE(DPV) case DPV: return launch_hogwild_t<DPV, SAMPLE, true, false, true>(p, reserve, st);
-        switch (dp) {
-            EB_CASE(8) EB_CASE(16) EB_CASE(32) EB_CASE(64) EB_CASE(128) EB_CASE(256)
-            default: return set_err(EB_ERR_ARG, "row stride ld=%d must be one of 8,16,32,64,128,256 floats", dp);
-        }
-#undef EB_CASE
-    }
-    if (use_stage(dp, flags, false)) {
-        switch (dp) {
-            case 32: return launch_stage_t<32, SAMPLE, false>(p, reserve, st);
-            case 64: return launch_stage_t<64, SAMPLE, false>(p, reserve, st);
-            default: return launch_stage_t<128, SAMPLE, false>(p, reserve, st);
-        }
-    }
-#define EB_CASE(DPV)                                                                           \
-    case DPV:                                                                                  \
-        return atomic ? launch_hogwild_t<DPV, SAMPLE, true>(p, reserve, st)                           \
-                      : launch_hogwild_t<DPV, SAMPLE, false>(p, reserve, st);
-    switch (dp) {
-        EB_CASE(8) EB_CASE(16) EB_CASE(32) EB_CASE(64) EB_CASE(128) EB_CASE(256)
-        default: return set_err(EB_ERR_ARG, "row stride ld=%d must be one of 8,16,32,64,128,256 floats", dp);
-    }
-#undef EB_CASE
+    return with_stride<8, 16, 32, 64, 128, 256>(dp, "8,16,32,64,128,256 floats", [&](auto dpc) {
+        constexpr int DP = decltype(dpc)::value;
+        if (rounds) return launch_hogwild_t<DP, SAMPLE, true, false, true>(p, reserve, st);
+        return atomic ? launch_hogwild_t<DP, SAMPLE, true, false, false>(p, reserve, st)
+                      : launch_hogwild_t<DP, SAMPLE, false, false, false>(p, reserve, st);
+    });
 }
 
-// PEER mode: atomics only (other GPUs update the same rows), strides the sharded configurations use
+// PEER mode: atomics only (other GPUs update the same rows), strides the sharded configurations use.  The shared-memory-staged
+// kernel is the default (its row copies are in flight without holding registers while the rows cross NVLink); flags bit 4 (16),
+// or bit 0, selects the register kernel (whose peer updates stay atomic).
 template <bool SAMPLE>
 static int launch_hogwild_peer(const HogwildParams &p, int dp, int flags, cudaStream_t st) {
     const int reserve = (flags >> 8) & 0xff;
     EB_ARG(!(flags & 64), "deterministic rounds exist for local tables only (other GPUs update peer rows concurrently)");
-    if (use_stage(dp, flags, true)) {
-        switch (dp) {
-            case 32: return launch_stage_t<32, SAMPLE, true>(p, reserve, st);
-            case 64: return launch_stage_t<64, SAMPLE, true>(p, reserve, st);
-            case 128: return launch_stage_t<128, SAMPLE, true>(p, reserve, st);
-            default: break;
-        }
-    }
-    switch (dp) {
-        case 32: return launch_hogwild_t<32, SAMPLE, true, true>(p, reserve, st);
-        case 64: return launch_hogwild_t<64, SAMPLE, true, true>(p, reserve, st);
-        case 128: return launch_hogwild_t<128, SAMPLE, true, true>(p, reserve, st);
-        default: return set_err(EB_ERR_ARG, "row stride ld=%d must be one of 32,64,128 floats for sharded item tables", dp);
-    }
+    const bool stage = !(flags & (1 | 16));
+    return with_stride<32, 64, 128>(dp, "32,64,128 floats for sharded item tables", [&](auto dpc) {
+        constexpr int DP = decltype(dpc)::value;
+        return stage ? launch_stage_t<DP, SAMPLE>(p, reserve, st) : launch_hogwild_t<DP, SAMPLE, true, true, false>(p, reserve, st);
+    });
 }
 
 static int fill_peer(HogwildParams &p, float *const *V_shards, float *const *b_shards, int n_shards, int32_t shard_rows,
@@ -683,9 +574,7 @@ static int fill_peer(HogwildParams &p, float *const *V_shards, float *const *b_s
         p.Vp[s] = V_shards[s]; p.bp[s] = b_shards[s];
     }
     for (int s = n_shards; s < EB_MAX_PEERS; s++) { p.Vp[s] = V_shards[0]; p.bp[s] = b_shards[0]; }
-    p.shard_rows = (uint32_t)shard_rows;
-    const uint64_t magic = (1ull << 32) / (uint64_t)shard_rows;       // shard_rows == 1 -> 2^32: clamp (the correction step covers it)
-    p.shard_magic = (uint32_t)(magic > 0xffffffffull ? 0xffffffffull : magic);
+    p.shards = shard_map(shard_rows);
     return EB_OK;
 }
 
@@ -866,7 +755,7 @@ extern "C" int eb_bpr_step_f32(float *U, float *V, float *item_bias, int d, int 
     EB_ARG(tu && ti && tj, "null triple arrays");
     HogwildParams p{};
     p.U = U; p.V = V; p.b = item_bias; p.ld = ld; p.tu = tu; p.ti = ti; p.tj = tj; p.n = n;
-    p.lr = lr; p.reg_u = reg_u; p.reg_b = reg_b; p.reg_pos = reg_pos; p.reg_neg = reg_neg; p.loss = loss;
+    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
     return launch_hogwild<false>(p, ld, flags, (cudaStream_t)stream);
 }
 
@@ -915,7 +804,7 @@ extern "C" int eb_bpr_step_sampled_filter_f32(float *U, float *V, float *item_bi
     if (n == 0) return EB_OK;
     HogwildParams p{};
     p.U = U; p.V = V; p.b = item_bias; p.ld = ld; p.n = n;
-    p.lr = lr; p.reg_u = reg_u; p.reg_b = reg_b; p.reg_pos = reg_pos; p.reg_neg = reg_neg; p.loss = loss;
+    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
     p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
     p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
     if (int rc = set_filter(p, filter, filter_words)) return rc;
@@ -933,7 +822,7 @@ extern "C" int eb_bpr_step_peer_f32(float *U, float *const *V_shards, float *con
     if (n == 0) return EB_OK;
     EB_ARG(tu && ti && tj, "null triple arrays");
     p.U = U; p.ld = ld; p.tu = tu; p.ti = ti; p.tj = tj; p.n = n;
-    p.lr = lr; p.reg_u = reg_u; p.reg_b = reg_b; p.reg_pos = reg_pos; p.reg_neg = reg_neg; p.loss = loss;
+    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
     return launch_hogwild_peer<false>(p, ld, flags, (cudaStream_t)stream);
 }
 
@@ -951,7 +840,7 @@ extern "C" int eb_bpr_step_sampled_peer_f32(float *U, float *const *V_shards, fl
     if (int rc = fill_peer(p, V_shards, b_shards, n_shards, shard_rows, n_items)) return rc;
     if (n == 0) return EB_OK;
     p.U = U; p.ld = ld; p.n = n;
-    p.lr = lr; p.reg_u = reg_u; p.reg_b = reg_b; p.reg_pos = reg_pos; p.reg_neg = reg_neg; p.loss = loss;
+    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
     p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
     p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
     p.no_item_updates = (flags >> 2) & 1;
@@ -1034,7 +923,7 @@ extern "C" int eb_bpr_step_host_packed_f32(float *U, float *V, float *item_bias,
         EB_CUDA(cudaMemcpyAsync(staging, packed_host, sizeof(uint64_t) * n, cudaMemcpyHostToDevice, st));   // ONE copy, 8 B / triple
         HogwildParams p{};
         p.U = U; p.V = V; p.b = item_bias; p.ld = ld; p.n = n; p.packed = staging; p.bits_u = bits_u; p.bits_i = bits_i;
-        p.lr = lr; p.reg_u = reg_u; p.reg_b = reg_b; p.reg_pos = reg_pos; p.reg_neg = reg_neg; p.loss = loss_dev;
+        p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss_dev;
         if (int rc = launch_hogwild<false>(p, ld, flags, st)) return rc;
     }
     if (loss_dev && loss_host) EB_CUDA(cudaMemcpyAsync(loss_host, loss_dev, sizeof(double), cudaMemcpyDeviceToHost, st));

@@ -109,4 +109,21 @@ __device__ __forceinline__ float4 ld_sys_v4(const float4 *p) {
     asm volatile("ld.relaxed.sys.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p) : "memory");
     return r;
 }
+
+// Row i of a row-sharded table lives in shard i / rows at local row i % rows: one multiply-high by magic = floor(2^32 / rows)
+// and one correction instead of an integer division.
+struct ShardMap {
+    uint32_t rows, magic;
+    __device__ __forceinline__ void locate(int i, int &owner, int &local) const {
+        uint32_t o = __umulhi((uint32_t)i, magic);
+        uint32_t r = (uint32_t)i - o * rows;
+        if (r >= rows) { o++; r -= rows; }
+        owner = (int)o; local = (int)r;
+    }
+};
+
+static inline ShardMap shard_map(int32_t shard_rows) {
+    const uint64_t m = (1ull << 32) / (uint64_t)shard_rows;       // shard_rows == 1 -> 2^32: clamp (the correction step covers it)
+    return ShardMap{(uint32_t)shard_rows, (uint32_t)(m > 0xffffffffull ? 0xffffffffull : m)};
+}
 }  // namespace eb

@@ -28,21 +28,6 @@ struct PeerTab {
     float *base[EB_MAX_PEERS];
 };
 
-struct ShardMap {
-    uint32_t rows, magic;
-    __device__ __forceinline__ void locate(int i, int &owner, int &local) const {
-        uint32_t o = __umulhi((uint32_t)i, magic);
-        uint32_t r = (uint32_t)i - o * rows;
-        if (r >= rows) { o++; r -= rows; }
-        owner = (int)o; local = (int)r;
-    }
-};
-
-static ShardMap shard_map(int32_t shard_rows) {
-    const uint64_t m = (1ull << 32) / (uint64_t)shard_rows;
-    return ShardMap{(uint32_t)shard_rows, (uint32_t)(m > 0xffffffffull ? 0xffffffffull : m)};
-}
-
 static int fill_tab(PeerTab &t, float *const *ptrs, int n) {
     EB_ARG(ptrs && n >= 1 && n <= EB_MAX_PEERS, "1 <= n_peers <= %d", EB_MAX_PEERS);
     for (int s = 0; s < n; s++) {

@@ -3,14 +3,10 @@
 // ids, done by the host in elliot_b200/parallel.py), owners gather them (eb_gather_rows_f32), the requester
 // runs the BPR update against the fetched copies (eb_bpr_step_rows_f32: user rows are local and updated in
 // place, item-row DELTAS are written per triple), deltas travel back and owners add them
-// (eb_scatter_add_rows_f32).  Same arithmetic as bpr_hogwild_kernel (BPRMF_model.py:91-117).
-#include "common.cuh"
+// (eb_scatter_add_rows_f32).  Same update as bpr_hogwild_kernel (bpr_update.cuh, BPRMF_model.py:91-117).
+#include "bpr_update.cuh"
 
 namespace eb {
-
-__device__ __forceinline__ void sred4(float *p, float4 v) {
-    asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
 
 // out[t][0..w) = table[ids[t]][0..w)   (w % 4 == 0)
 __global__ void __launch_bounds__(256) gather_rows_kernel(const float *table, int64_t ld, const int32_t *ids, int64_t n, int w,
@@ -27,7 +23,7 @@ __global__ void __launch_bounds__(256) scatter_add_rows_kernel(float *table, int
     const int64_t total = n * (w / 4);
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
         const int64_t t = e / (w / 4); const int c = (int)(e - t * (w / 4)) * 4;
-        sred4(table + (int64_t)ids[t] * ld + c, *reinterpret_cast<const float4 *>(rows + t * ldr + c));
+        red_add_v4(table + (int64_t)ids[t] * ld + c, *reinterpret_cast<const float4 *>(rows + t * ldr + c));
     }
 }
 
@@ -35,8 +31,8 @@ __global__ void __launch_bounds__(256) scatter_add_rows_kernel(float *table, int
 // The fetched item buffers carry the item bias in column `d` when bias_col >= 0 (tables padded so that d < ld).
 template <int DP>
 __global__ void __launch_bounds__(256) bpr_rows_kernel(float *U, int64_t ldu, const int32_t *tu, const float *Ri, const float *Rj,
-                                                       int64_t ldr, int64_t n, int bias_col, float lr, float reg_u, float reg_b,
-                                                       float reg_pos, float reg_neg, float *dRi, float *dRj, double *loss) {
+                                                       int64_t ldr, int64_t n, int bias_col, const BprHyper h, float *dRi, float *dRj,
+                                                       double *loss) {
     constexpr int NV = DP / 4, G = NV >= 32 ? 32 : NV, VPL = NV / G;
     const int lane = threadIdx.x & 31, gl = lane % G;
     const int64_t grp = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * (32 / G) + lane / G;
@@ -70,32 +66,25 @@ __global__ void __launch_bounds__(256) bpr_rows_kernel(float *U, int64_t ldu, co
                         m2 * a[v].z * (vi[v].z - vj[v].z) + m3 * a[v].w * (vi[v].w - vj[v].w);
             }
         }
-#pragma unroll
-        for (int off = G / 2; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
+        part = group_sum<G>(part);
         if (!on) continue;
-        const float x = part + (bi - bj);
-        const float z = __fdividef(1.f, 1.f + __expf(x));
-        if (gl == 0) loss_acc += fmaxf(-x, 0.f) + __logf(1.f + __expf(-fabsf(x)));
+        const float z = bpr_sigmoid_loss(part + (bi - bj), loss_acc, gl);
 #pragma unroll
         for (int v = 0; v < VPL; v++) {
             const int e = (v * G + gl) * 4;
-            const float av[4] = {a[v].x, a[v].y, a[v].z, a[v].w}, iv[4] = {vi[v].x, vi[v].y, vi[v].z, vi[v].w},
-                        jv[4] = {vj[v].x, vj[v].y, vj[v].z, vj[v].w};
-            float du[4], di[4], dj[4];
-#pragma unroll
-            for (int c = 0; c < 4; c++) {
-                if (e + c == bias_col) {          // bias entries of the item rows: b_i += lr (z - reg_b b_i), b_j += lr (-z - reg_b b_j)
-                    du[c] = 0.f; di[c] = lr * (z - reg_b * iv[c]); dj[c] = lr * (-z - reg_b * jv[c]);
-                } else {
-                    du[c] = lr * ((iv[c] - jv[c]) * z - reg_u * av[c]);
-                    const float un = av[c] + du[c];
-                    di[c] = lr * (un * z - reg_pos * iv[c]);
-                    dj[c] = lr * (-un * z - reg_neg * jv[c]);
-                }
-            }
-            sred4(U + (int64_t)u * ldu + e, make_float4(du[0], du[1], du[2], du[3]));
-            *reinterpret_cast<float4 *>(dRi + t * ldr + e) = make_float4(di[0], di[1], di[2], di[3]);
-            *reinterpret_cast<float4 *>(dRj + t * ldr + e) = make_float4(dj[0], dj[1], dj[2], dj[3]);
+            float4 du, di, dj;
+            bpr_row_deltas(a[v], vi[v], vj[v], z, h, du, di, dj);
+            // the bias entries of the item rows take the bias update; the user row has no bias
+            auto bias_entry = [&](int c, float &du_c, float &di_c, float &dj_c, float bi_c, float bj_c) {
+                if (e + c == bias_col) { du_c = 0.f; bpr_bias_deltas(z, bi_c, bj_c, h, di_c, dj_c); }
+            };
+            bias_entry(0, du.x, di.x, dj.x, vi[v].x, vj[v].x);
+            bias_entry(1, du.y, di.y, dj.y, vi[v].y, vj[v].y);
+            bias_entry(2, du.z, di.z, dj.z, vi[v].z, vj[v].z);
+            bias_entry(3, du.w, di.w, dj.w, vi[v].w, vj[v].w);
+            red_add_v4(U + (int64_t)u * ldu + e, du);
+            *reinterpret_cast<float4 *>(dRi + t * ldr + e) = di;
+            *reinterpret_cast<float4 *>(dRj + t * ldr + e) = dj;
         }
     }
     if (loss) {
@@ -142,7 +131,8 @@ extern "C" int eb_bpr_step_rows_f32(float *U, int64_t ldu, const int32_t *tu, co
     if (n == 0) return EB_OK;
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned grid = sgrid(n * 16);
-#define EB_ROWS(DPV) case DPV: bpr_rows_kernel<DPV><<<grid, 256, 0, st>>>(U, ldu, tu, Ri, Rj, ldr, n, bias_col, lr, reg_u, reg_b, reg_pos, reg_neg, dRi, dRj, loss); break;
+    const BprHyper h{lr, reg_u, reg_b, reg_pos, reg_neg};
+#define EB_ROWS(DPV) case DPV: bpr_rows_kernel<DPV><<<grid, 256, 0, st>>>(U, ldu, tu, Ri, Rj, ldr, n, bias_col, h, dRi, dRj, loss); break;
     switch ((int)ldr) {
         EB_ROWS(8) EB_ROWS(16) EB_ROWS(32) EB_ROWS(64) EB_ROWS(128) EB_ROWS(256)
         default: return set_err(EB_ERR_ARG, "row stride %lld must be one of 8,16,32,64,128,256 floats", (long long)ldr);

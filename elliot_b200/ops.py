@@ -77,7 +77,8 @@ def bpr_step_sampled_f32(U, V, b, d, n_users, n_items, indptr, indices, n, seed,
     """Fused sample+update step (custom_sampler.py:24-46 distribution, Philox stream).  filter: bloom_build() output.
     deterministic: run the launch in rounds (reads, grid barrier, atomic adds, grid barrier) so the same inputs give the same
     tables on every run up to fp32 summation order; slower than the default free-running Hogwild.
-    _variant (profiling): 16 forces the register-staged kernel, 32 the shared-memory-staged one (default: see use_stage)."""
+    _variant (profiling): one table always runs the register-staged kernel (16 or 0); 32, the shared-memory-staged kernel,
+    exists for sharded item tables only and is refused here."""
     _need_cuda(U, V, b, indptr, indices, loss, filter)
     assert indptr.dtype == torch.int64 and indices.dtype == torch.int32
     ou = oi = oj = None
@@ -681,7 +682,7 @@ def _ptr_array(ptrs):
 def bpr_step_peer_f32(U, V_shards, b_shards, shard_rows, d, n_items, tu, ti, tj, lr, reg_u, reg_b, reg_pos, reg_neg, loss=None,
                       _variant=0):
     """BPR step on materialised triples, item table + biases row-sharded (shard s = rows [s*shard_rows, (s+1)*shard_rows)).
-    _variant (profiling): 16 forces the register-staged kernel, 32 the shared-memory-staged one."""
+    _variant (profiling): 16 forces the register-staged kernel, 32 the shared-memory-staged one (the default)."""
     _need_cuda(U, tu, ti, tj, loss); _chk_idx(tu, ti, tj)
     va, n = _ptr_array(V_shards); ba, nb = _ptr_array(b_shards)
     assert n == nb and U.dtype == torch.float32 and U.stride(1) == 1
@@ -693,7 +694,8 @@ def bpr_step_peer_f32(U, V_shards, b_shards, shard_rows, d, n_items, tu, ti, tj,
 def bpr_step_sampled_peer_f32(U, V_shards, b_shards, shard_rows, d, n_users, n_items, indptr, indices, n, seed, first, lr, reg_u,
                               reg_b, reg_pos, reg_neg, loss=None, out=None, reserve_sms=0, filter=None, _no_item_updates=False,
                               _variant=0):
-    """Fused sample+update step with the item table row-sharded over the GPUs of the box (loads / atomics over NVLink)."""
+    """Fused sample+update step with the item table row-sharded over the GPUs of the box (loads / atomics over NVLink).
+    _variant (profiling): 16 forces the register-staged kernel, 32 the shared-memory-staged one (the default)."""
     _need_cuda(U, indptr, indices, loss)
     assert indptr.dtype == torch.int64 and indices.dtype == torch.int32 and U.dtype == torch.float32 and U.stride(1) == 1
     va, ns = _ptr_array(V_shards); ba, nb = _ptr_array(b_shards)

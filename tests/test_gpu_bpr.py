@@ -152,6 +152,68 @@ def test_hogwild_f32_conflict_free_batch_equals_sequential(golden, racy):
     assert abs(loss.item() - l0) < 1e-3 * max(1.0, l0)
 
 
+@pytest.mark.parametrize("d", [5, 16, 30, 64, 100, 256])
+def test_hogwild_variants_agree_bitwise_on_conflict_free_batch(golden_small, d):
+    """Without row conflicts every triple's update is formed from the initial rows, so the kernel variants must leave
+    bit-identical tables: register + atomics (default), deterministic rounds, packed host triples, and on the strides the
+    sharded item table supports the peer step (shared-memory-staged on 1 and 3 shards, register on 3).  Racy stores differ
+    from the atomic result in the last bit.  The loss is summed per lane group in a kernel-dependent order: 1e-6 relative."""
+    from elliot_b200.parallel import ceil_shard
+    g = golden_small
+    rs = np.random.RandomState(d)
+    nu, ni = len(g["users"]), len(g["items"])
+    ld = ops.padded_dim(d)
+    hp = (0.05, 0.0025, 0.01, 0.0025, 0.00025)
+    keep = _conflict_free(g["tu"], g["ti"], g["tj"])
+    tu, ti, tj = (torch.from_numpy(g[k][keep].astype(np.int32)) for k in ("tu", "ti", "tj"))
+    U0 = _pad(rs.normal(0, 0.1, (nu, d)), ld, np.float32); V0 = _pad(rs.normal(0, 0.1, (ni, d)), ld, np.float32)
+    b0 = torch.from_numpy(rs.normal(0, 0.05, ni).astype(np.float32)).to(DEV)
+    dev_t = [x.to(DEV) for x in (tu, ti, tj)]
+
+    def local(**kw):
+        U, V, b = U0.clone(), V0.clone(), b0.clone()
+        loss = torch.zeros(1, dtype=torch.float64, device=DEV)
+        ops.bpr_step_f32(U, V, b, d, *dev_t, *hp, loss=loss, **kw)
+        return U, V, b, loss.item()
+
+    def packed():
+        U, V, b = U0.clone(), V0.clone(), b0.clone()
+        host = ops.pack_triples(tu, ti, tj, nu, ni).pin_memory()
+        staging = torch.empty(host.numel(), dtype=torch.int64, device=DEV)
+        ld_, lh = torch.zeros(1, dtype=torch.float64, device=DEV), torch.zeros(1, dtype=torch.float64).pin_memory()
+        ops.bpr_step_host_packed_f32(U, V, b, d, host, nu, ni, *hp, staging, ld_, lh)
+        return U, V, b, lh.item()
+
+    def peer(n_shards, variant=0):
+        sr = ceil_shard(ni, n_shards)
+        Vs = [torch.zeros((sr, ld), device=DEV) for _ in range(n_shards)]
+        bs = [torch.zeros(sr, device=DEV) for _ in range(n_shards)]
+        for s in range(n_shards):
+            blk = slice(s * sr, min((s + 1) * sr, ni))
+            Vs[s][:blk.stop - blk.start] = V0[blk]; bs[s][:blk.stop - blk.start] = b0[blk]
+        U = U0.clone()
+        loss = torch.zeros(1, dtype=torch.float64, device=DEV)
+        ops.bpr_step_peer_f32(U, Vs, bs, sr, d, ni, *dev_t, *hp, loss=loss, _variant=variant)
+        return U, torch.cat(Vs)[:ni], torch.cat(bs)[:ni], loss.item()
+
+    runs = {"racy": local(racy=True), "deterministic": local(deterministic=True), "packed": packed()}
+    if ld in (32, 64, 128):
+        runs.update({"peer1": peer(1), "peer3": peer(3), "peer3_register": peer(3, 16)})
+    ref = local()
+    torch.cuda.synchronize()
+    assert not torch.equal(ref[0], U0) and ref[3] > 0
+    for name, got in runs.items():
+        for k, (a, c) in enumerate(zip(got[:3], ref[:3])):
+            if name == "racy":
+                # a plain store rounds once (row + lr * g contracts to one FMA), an atomic add rounds the delta and then the
+                # sum: the last bit of the larger entries differs, 2^-25 at most on these inputs
+                ok = (a - c).abs().max().item() <= 2.0 ** -25
+            else:
+                ok = torch.equal(a, c)
+            assert ok, (name, "UVb"[k], (a - c).abs().max().item())
+        assert abs(got[3] - ref[3]) <= 1e-6 * ref[3], (name, got[3], ref[3])
+
+
 def test_hogwild_f32_epoch_tracks_sequential(golden_small):
     """A full epoch in one Hogwild launch (heavy staleness) stays close to sequential SGD:
     loss on the epoch's triples drops and the tables correlate > 0.98 with the oracle's."""
@@ -370,3 +432,18 @@ def test_deterministic_rounds_are_refused_where_they_do_not_exist(golden_tiny):
     from elliot_b200._lib import EbError
     with pytest.raises(EbError):
         ops.bpr_step_f32(Ud, Vd, bd, d, t, t, t, 0.05, 0, 0, 0, 0, racy=True, deterministic=True)
+
+
+def test_shared_memory_staged_kernel_is_refused_on_one_table(golden_tiny):
+    """The shared-memory-staged kernel (_variant=32) exists for sharded item tables only."""
+    from elliot_b200._lib import EbError
+    g = golden_tiny
+    d = int(g["d"]); ld = ops.padded_dim(d)
+    nu, ni = len(g["users"]), len(g["items"])
+    indptr, _, srt = _csr_dev(g)
+    Ud, Vd = _pad(g["U0"], ld, np.float32), _pad(g["V0"], ld, np.float32)
+    bd = torch.zeros(ni, dtype=torch.float32, device=DEV)
+    with pytest.raises(EbError, match="sharded item tables only"):
+        ops.bpr_step_sampled_f32(Ud, Vd, bd, d, nu, ni, indptr, srt, 64, 1, 0, 0.05, 0, 0, 0, 0, _variant=32)
+    ops.bpr_step_sampled_f32(Ud, Vd, bd, d, nu, ni, indptr, srt, 64, 1, 0, 0.05, 0, 0, 0, 0, _variant=16)
+    torch.cuda.synchronize()
