@@ -127,6 +127,12 @@ SIGNATURES = {
     "eb_score_topk_tc_workspace_bytes": (c_size, [c_i64, c_i32, c_int]),
     "eb_score_topk_tc_f32": (c_int, [c_void, c_void, c_void, c_i32, c_int, c_int, c_void, c_void, c_i32, c_i64, c_int,
                                      c_void, c_void, c_void, c_void, c_size, c_void, c_void]),
+    "eb_csr_to_dense_bf16": (c_int, [c_void, c_void, c_void, c_i32, c_i32, c_i32, c_f32, c_void, c_i64, c_void, c_void, c_void]),
+    "eb_knn_neighbors_f32": (c_int, [c_void, c_i64, c_i32, c_i32, c_i32, c_void, c_int, c_f32, c_int, c_void, c_void, c_void,
+                                     c_void]),
+    "eb_knn_score_tile_cols": (c_int, []),
+    "eb_knn_score_topk_f32": (c_int, [c_void, c_void, c_void, c_void, c_void, c_void, c_i32, c_void, c_void, c_void, c_i32, c_i64,
+                                      c_int, c_int, c_void, c_void, c_void]),
 }
 
 _lib = None

@@ -483,6 +483,61 @@ def colsum(src, out=None):
     return out
 
 
+def csr_to_dense_bf16(indptr, indices, values, n_cols, scale=1.0, row0=0, n_rows=None, row_sq=False, col_sq=False):
+    """Rows [row0, row0 + n_rows) of a CSR (values None: ones) times `scale` as a zero-filled bf16 [n_rows][pad8(n_cols)]
+    matrix, plus optionally the fp32 squared norms of its rows and of its columns.  Returns (X, row_sq or None, col_sq or None)."""
+    _need_cuda(indptr, indices, values)
+    assert indptr.dtype == torch.int64 and indices.dtype == torch.int32 and (values is None or values.dtype == torch.float32)
+    if n_rows is None:
+        n_rows = indptr.numel() - 1 - row0
+    dev = indptr.device
+    ld = (n_cols + 7) // 8 * 8
+    X = torch.empty((n_rows, ld), dtype=torch.bfloat16, device=dev)
+    rs = torch.empty(n_rows, dtype=torch.float32, device=dev) if row_sq else None
+    cs = torch.empty(n_cols, dtype=torch.float32, device=dev) if col_sq else None
+    _call("eb_csr_to_dense_bf16", indptr, _ptr(indptr), _ptr(indices), _ptr(values), row0, n_rows, n_cols, float(scale), _ptr(X),
+          ld, _ptr(rs), _ptr(cs))
+    return X, rs, cs
+
+
+def knn_neighbors(slab, n, row0, diag, k, cosine=True, dot_scale=1.0):
+    """Neighbour lists of Gram rows row0 .. row0 + slab.shape[0] (slab: fp32 [S][>= n], overwritten with the similarity
+    values): (idx int32 [S][k], val fp32 [S][k], cnt int32 [S]), value desc then column asc, -1 / 0 padded."""
+    _need_cuda(slab, diag)
+    assert slab.dtype == torch.float32 and slab.stride(1) == 1 and diag.dtype == torch.float32
+    S = slab.shape[0]
+    idx = torch.empty((S, k), dtype=torch.int32, device=slab.device)
+    val = torch.empty((S, k), dtype=torch.float32, device=slab.device)
+    cnt = torch.empty(S, dtype=torch.int32, device=slab.device)
+    _call("eb_knn_neighbors_f32", slab, _ptr(slab), slab.stride(0), S, n, row0, _ptr(diag), 1 if cosine else 0, float(dot_scale), k,
+          _ptr(idx), _ptr(val), _ptr(cnt))
+    return idx, val, cnt
+
+
+def knn_score_tile_cols():
+    return int(lib().eb_knn_score_tile_cols())
+
+
+def knn_score_topk(A, B, n_cols, k, frac_bits, mask_indptr=None, mask_indices=None, users=None, user_begin=0, n_sel=None):
+    """Top k of the rows of A @ B (A, B: (indptr int64, indices int32, values fp32) CSRs on the device, B's rows sorted by
+    column) with the masked columns excluded, (score desc, column asc): (idx int32 [n_sel][k], val fp32 [n_sel][k]).
+    Each product is rounded to a multiple of 2^-frac_bits and the sums are exact (see eb_knn_score_topk_f32)."""
+    (ap, ai, av), (bp, bi, bv) = A, B
+    _need_cuda(ap, ai, av, bp, bi, bv, mask_indptr, mask_indices, users)
+    assert ap.dtype == bp.dtype == torch.int64 and av.dtype == bv.dtype == torch.float32
+    _chk_idx(ai, bi)
+    if users is not None:
+        _chk_idx(users)
+        n_sel = users.numel()
+    elif n_sel is None:
+        n_sel = ap.numel() - 1 - user_begin
+    idx = torch.empty((n_sel, k), dtype=torch.int32, device=ap.device)
+    val = torch.empty((n_sel, k), dtype=torch.float32, device=ap.device)
+    _call("eb_knn_score_topk_f32", ap, _ptr(ap), _ptr(ai), _ptr(av), _ptr(bp), _ptr(bi), _ptr(bv), n_cols, _ptr(mask_indptr),
+          _ptr(mask_indices), _ptr(users), user_begin, n_sel, k, int(frac_bits), _ptr(idx), _ptr(val))
+    return idx, val
+
+
 def dense_topk(scores, k, mask_indptr=None, mask_indices=None, rows=None, shift=None):
     _need_cuda(scores, mask_indptr, mask_indices, rows, shift)
     n = scores.shape[0]

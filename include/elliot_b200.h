@@ -479,6 +479,33 @@ int eb_score_topk_tc_f32(const float *U, const float *V, const float *item_bias,
                          int32_t *out_idx, float *out_val, float *dump,
                          void *workspace, size_t workspace_bytes, int64_t *stats_host, void *stream);
 
+/* ------------------------------------------------------------------------
+ * ItemKNN / UserKNN, standard implementation (knn/item_knn/item_knn_similarity.py, knn/user_knn/user_knn_similarity.py).
+ * eb_csr_to_dense_bf16: rows [row0, row0 + n_rows) of a CSR (values NULL: ones), times `scale`, into a bf16 matrix
+ * [n_rows][ld] that the call zero-fills first; row_sq[r] / col_sq[c] (optional) receive the squared norms of the scaled
+ * rows / columns.  With every scaled value an integer of magnitude <= 256 and every squared norm < 2^24, the operand is
+ * exact and so is the Gram matrix eb_gemm_bf16 makes of it, and these norms are its diagonal.
+ * eb_knn_neighbors_f32: per row s of a Gram slab (rows row0.. of G, n columns, row stride ld), replaces the row by its
+ * similarity values, cosine = fp32((double)G_rc / sqrt((double)G_rr * (double)G_cc)) (0 when a norm is 0) or
+ * dot = G_rc * dot_scale, and writes the k largest nonzero ones ordered by value desc, column asc: out_idx/out_val
+ * [n_rows][k] (unused slots -1 / 0) and out_cnt[n_rows].  1 <= k <= 1024.
+ * eb_knn_score_topk_f32: for output row q (user users[q], or user_begin + q when users is NULL) the scores
+ * sum_j A[u, j] * B[j, :] over n_cols columns, each term rounded to a multiple of 2^-frac_bits and summed exactly in
+ * int64 (the caller keeps max_u sum_j |A[u, j]| * max |B| * 2^frac_bits below 2^62), so the result does not depend on the
+ * order of the sums; train items (mask CSR, rows sorted) are excluded; the k best by (score desc, column asc) go to
+ * out_idx/out_val [n_sel][k], padded with -1 / -inf when fewer than k columns are unmasked.  B rows sorted by column.
+ * The columns are processed in tiles of eb_knn_score_tile_cols() columns.  1 <= k <= 1024.
+ * ------------------------------------------------------------------------ */
+int eb_csr_to_dense_bf16(const int64_t *indptr, const int32_t *indices, const float *values, int32_t row0, int32_t n_rows,
+                         int32_t n_cols, float scale, void *dst_bf16, int64_t ld, float *row_sq, float *col_sq, void *stream);
+int eb_knn_neighbors_f32(float *slab, int64_t ld, int32_t n_rows, int32_t n, int32_t row0, const float *diag, int cosine,
+                         float dot_scale, int k, int32_t *out_idx, float *out_val, int32_t *out_cnt, void *stream);
+int eb_knn_score_tile_cols(void);
+int eb_knn_score_topk_f32(const int64_t *a_indptr, const int32_t *a_indices, const float *a_values, const int64_t *b_indptr,
+                          const int32_t *b_indices, const float *b_values, int32_t n_cols, const int64_t *mask_indptr,
+                          const int32_t *mask_indices, const int32_t *users, int32_t user_begin, int64_t n_sel, int k,
+                          int frac_bits, int32_t *out_idx, float *out_val, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
