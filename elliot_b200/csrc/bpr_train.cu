@@ -10,7 +10,9 @@
 //    the scatter-add.  Each lane of a warp first fetches/samples ONE triple (coalesced
 //    index loads or Philox), the groups then walk the warp's 32 triples with shuffles,
 //    prefetching the next triple's rows while the current one is reduced.
-//  * bpr_exact_kernel    — exact mode, fp64.  Same arithmetic, but sequentially
+//  * bpr_grouped_kernel  — the free-running sampled step on local tables: the same update, applied to the triples
+//    grouped by user (user_key_kernel + a stable radix sort first), the user row kept in registers across a run.
+//  * bpr_exact_kernel   — exact mode, fp64.  Same arithmetic, but sequentially
 //    consistent with the array order of the triples: every row carries a turn counter,
 //    a triple waits until each of its three rows has seen exactly the touches that
 //    precede it in the sequence (ranks come from a radix sort of (row, position)).
@@ -49,17 +51,18 @@ struct HogwildParams {
     const uint64_t *packed;
     int bits_u, bits_i;
     int no_item_updates;      // profiling only (flags bit 2): item rows are read but not updated
+    // grouped sampled step: the call's triple indices ordered by user (ascending u, then ascending t)
+    const int32_t *order;
 };
 
-// u uniform over users, i uniform over the user's train items, j uniform over the
-// complement (rejection against the sorted CSR row) — custom_sampler.py:31-42 semantics,
-// Philox stream instead of MT19937.
-__device__ __forceinline__ void sample_triple(const HogwildParams &p, int64_t t, int &u, int &i, int &j) {
-    uint32_t r[4];
+// u of triple t: uniform over the users that own at least one and not every item.  r keeps the Philox block that drew the
+// accepted u (its other words pick i and j), beg / len the user's CSR row.
+__device__ __forceinline__ void sample_user(const HogwildParams &p, int64_t t, uint32_t (&r)[4], int &u, int64_t &beg, int &len) {
     Philox::gen(p.seed, p.first + (uint64_t)t, 0u, r);
     u = (int)bounded(r[0], (uint32_t)p.n_users);
-    int64_t beg = __ldg(p.indptr + u), end = __ldg(p.indptr + u + 1);
-    int len = (int)(end - beg);
+    beg = __ldg(p.indptr + u);
+    int64_t end = __ldg(p.indptr + u + 1);
+    len = (int)(end - beg);
     uint32_t attempt = 0;
     while (len == 0 || len >= p.n_items) {  // users without train items never appear in the reference's dict; a user owning
                                             // every item has no negative at all (the reference would loop forever)
@@ -67,6 +70,17 @@ __device__ __forceinline__ void sample_triple(const HogwildParams &p, int64_t t,
         u = (int)bounded(r[0], (uint32_t)p.n_users);
         beg = __ldg(p.indptr + u); end = __ldg(p.indptr + u + 1); len = (int)(end - beg);
     }
+}
+
+// u uniform over users, i uniform over the user's train items, j uniform over the
+// complement (rejection against the sorted CSR row) — custom_sampler.py:31-42 semantics,
+// Philox stream instead of MT19937.
+__device__ __forceinline__ void sample_triple(const HogwildParams &p, int64_t t, int &u, int &i, int &j) {
+    uint32_t r[4];
+    int64_t beg;
+    int len;
+    sample_user(p, t, r, u, beg, len);
+    uint32_t attempt = 0;
     const int32_t *row = p.indices + beg;
     int cand = (int)bounded(r[2], (uint32_t)p.n_items);
     // the signature words depend on u only: their loads are in flight together with the pick of i
@@ -279,6 +293,136 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
                 }
             }
         }
+    }
+    if (p.loss) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, off);
+        if (lane == 0 && loss_acc != 0.f) atomicAdd(p.loss, (double)loss_acc);
+    }
+}
+
+// ---------------------------------------------------------------- grouped sampled step (local tables, free-running)
+// The sampled step on local tables applies its triples grouped by user.  user_key_kernel writes the user every triple will
+// draw, a stable radix sort orders the triple indices by it, and bpr_grouped_kernel walks the sorted indices: a warp takes a
+// window of 32 consecutive entries, each lane samples ITS triple t (same Philox draw as sample order, emitted at index t), and
+// each lane group walks a contiguous slice of the window in order.  The group keeps the current user row in registers (`cur`,
+// which triple k+1 of a run reads as triple k left it) and the run's summed update (`acc`), and adds acc to U once per run
+// and slice.  So a visited user row is read and written about once per step instead of once per triple, in ascending
+// address order, and the sampler's CSR row and indptr loads of one user are shared through L1.  Item rows and biases keep
+// their per-triple vector atomics.  A run of one triple performs exactly the per-triple kernel's arithmetic.
+__global__ void __launch_bounds__(256) user_key_kernel(const HogwildParams p, uint32_t *__restrict__ key, int32_t *__restrict__ val) {
+    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; t < p.n; t += stride) {
+        uint32_t r[4];
+        int u, len;
+        int64_t beg;
+        sample_user(p, t, r, u, beg, len);
+        key[t] = (uint32_t)u; val[t] = (int32_t)t;
+    }
+}
+
+template <int DP, bool ATOMIC>
+__global__ void __launch_bounds__(256) bpr_grouped_kernel(const HogwildParams p) {
+    constexpr int NV = DP / 4;                 // float4 per row
+    constexpr int G = NV >= 32 ? 32 : NV;      // lanes per triple
+    constexpr int VPL = NV / G;                // float4 per lane
+    constexpr int UNR = G >= 4 ? 4 : G;        // triples of the slice whose rows are in flight at once
+    const int lane = threadIdx.x & 31;
+    const int gl = lane % G;
+    const int gbase = lane - gl;
+    const int64_t warp_id = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const int64_t ld = p.ld;
+    float loss_acc = 0.f;
+
+    const int64_t n_tiles = (p.n + 31) / 32;
+    for (int64_t tile = warp_id; tile < n_tiles; tile += nwarps) {
+        const int64_t pos = tile * 32 + lane;
+        int u = -1, i = 0, j = 0;
+        if (pos < p.n) fetch_triple<true>(p, __ldg(p.order + pos), u, i, j);
+        // the group's run: user cu (-1: none yet), its row as the run left it, the run's summed update
+        int cu = -1;
+        float4 cur[VPL], acc[VPL];
+        auto flush = [&]() {
+            float *pu = p.U + (int64_t)cu * ld;
+#pragma unroll
+            for (int v = 0; v < VPL; v++) {
+                float *e = pu + (v * G + gl) * 4;
+                if (ATOMIC) red_add_v4(e, acc[v]);
+                else *reinterpret_cast<float4 *>(e) = cur[v];
+            }
+        };
+#pragma unroll 1
+        for (int s0 = 0; s0 < G; s0 += UNR) {
+            Rows<VPL> rw[UNR];
+            int tu_[UNR], ti_[UNR], tj_[UNR];
+#pragma unroll
+            for (int q = 0; q < UNR; q++) {
+                tu_[q] = __shfl_sync(0xffffffffu, u, gbase + s0 + q);
+                ti_[q] = __shfl_sync(0xffffffffu, i, gbase + s0 + q);
+                tj_[q] = __shfl_sync(0xffffffffu, j, gbase + s0 + q);
+                if (tu_[q] >= 0) {
+                    // the user row only where a run starts: inside a run the row is `cur`
+                    if (tu_[q] != (q == 0 ? cu : tu_[q - 1])) {
+                        const float4 *pu = reinterpret_cast<const float4 *>(p.U + (int64_t)tu_[q] * ld);
+#pragma unroll
+                        for (int v = 0; v < VPL; v++) rw[q].u[v] = pu[v * G + gl];
+                    }
+                    const float4 *pi = reinterpret_cast<const float4 *>(p.V + (int64_t)ti_[q] * ld);
+                    const float4 *pj = reinterpret_cast<const float4 *>(p.V + (int64_t)tj_[q] * ld);
+#pragma unroll
+                    for (int v = 0; v < VPL; v++) { rw[q].vi[v] = pi[v * G + gl]; rw[q].vj[v] = pj[v * G + gl]; }
+                    rw[q].bi = p.b[ti_[q]];
+                    rw[q].bj = p.b[tj_[q]];
+                }
+            }
+#pragma unroll
+            for (int q = 0; q < UNR; q++) {
+                const Rows<VPL> &nx = rw[q];
+                const int qu = tu_[q], qi = ti_[q], qj = tj_[q];
+                const bool start = qu != cu;                       // group-uniform
+                if (start) {
+                    if (cu >= 0) flush();
+                    cu = qu;
+#pragma unroll
+                    for (int v = 0; v < VPL; v++) cur[v] = nx.u[v];
+                }
+                float part = 0.f;
+                if (qu >= 0) {
+#pragma unroll
+                    for (int v = 0; v < VPL; v++) part += bpr_partial_dot(cur[v], nx.vi[v], nx.vj[v]);
+                }
+                part = group_sum<G>(part);
+                if (qu >= 0) {
+                    const float z = bpr_sigmoid_loss(part + (nx.bi - nx.bj), loss_acc, gl);
+                    float *pi = p.V + (int64_t)qi * ld, *pj = p.V + (int64_t)qj * ld;
+#pragma unroll
+                    for (int v = 0; v < VPL; v++) {
+                        const float4 a = cur[v], vi = nx.vi[v], vj = nx.vj[v];
+                        float4 du, di, dj;
+                        bpr_row_deltas(a, vi, vj, z, p.hp, du, di, dj);
+                        cur[v] = make_float4(a.x + du.x, a.y + du.y, a.z + du.z, a.w + du.w);
+                        acc[v] = start ? du : make_float4(acc[v].x + du.x, acc[v].y + du.y, acc[v].z + du.z, acc[v].w + du.w);
+                        const int e = (v * G + gl) * 4;
+                        if (ATOMIC) {
+                            red_add_v4(pi + e, di);
+                            red_add_v4(pj + e, dj);
+                        } else {
+                            *reinterpret_cast<float4 *>(pi + e) = make_float4(vi.x + di.x, vi.y + di.y, vi.z + di.z, vi.w + di.w);
+                            *reinterpret_cast<float4 *>(pj + e) = make_float4(vj.x + dj.x, vj.y + dj.y, vj.z + dj.z, vj.w + dj.w);
+                        }
+                    }
+                    if (gl == 0) {
+                        float dbi, dbj;
+                        bpr_bias_deltas(z, nx.bi, nx.bj, p.hp, dbi, dbj);
+                        if (ATOMIC) { red_add_f32(p.b + qi, dbi); red_add_f32(p.b + qj, dbj); }
+                        else { p.b[qi] = nx.bi + dbi; p.b[qj] = nx.bj + dbj; }
+                    }
+                }
+            }
+        }
+        if (cu >= 0) flush();
     }
     if (p.loss) {
 #pragma unroll
@@ -535,19 +679,104 @@ static void item_table_l2_window(const HogwildParams &p, cudaStream_t st) {
     cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &attr);
 }
 
+template <int DP, bool ATOMIC>
+static int launch_grouped_t(const HogwildParams &p, int reserve_sms, cudaStream_t st) {
+    auto kern = bpr_grouped_kernel<DP, ATOMIC>;
+    unsigned grid;
+    if (int rc = persistent_grid((const void *)kern, 0, p.n, reserve_sms, grid)) return rc;
+    kern<<<grid, 256, 0, st>>>(p);
+    EB_CUDA(cudaGetLastError());
+    return EB_OK;
+}
+
+static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
+
+static int bits_for(uint64_t v) { int b = 1; while ((v >> b) != 0) b++; return b; }
+
+// The grouped step sorts the triple indices of at most GROUP_MAX triples at a time (int32 offsets); longer calls run as
+// consecutive sub-steps of that size.
+constexpr int64_t GROUP_MAX = (int64_t)INT32_MAX;
+
+struct GroupLayout {
+    size_t key_a, key_b, val_a, val_b, cub, cub_bytes, total;
+};
+
+// 16 B per triple (user keys and triple indices, each double-buffered for the sort) + cub's temporary storage
+static GroupLayout group_layout(int64_t n, int32_t n_users) {
+    const int64_t m = n < GROUP_MAX ? n : GROUP_MAX;
+    GroupLayout L;
+    size_t off = 0;
+    L.key_a = off; off += align_up(sizeof(uint32_t) * (size_t)m);
+    L.key_b = off; off += align_up(sizeof(uint32_t) * (size_t)m);
+    L.val_a = off; off += align_up(sizeof(int32_t) * (size_t)m);
+    L.val_b = off; off += align_up(sizeof(int32_t) * (size_t)m);
+    cub::DoubleBuffer<uint32_t> keys(nullptr, nullptr);
+    cub::DoubleBuffer<int32_t> vals(nullptr, nullptr);
+    size_t cb = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, cb, keys, vals, (int)m, 0, bits_for((uint64_t)n_users));
+    L.cub_bytes = cb;
+    L.cub = off; off += align_up(cb);
+    L.total = off;
+    return L;
+}
+
+// Sampled step on local tables, free-running: per sub-step, the user keys, the stable sort of the triple indices by user,
+// then the grouped update.  The key pass and the update leave `reserve` SMs free; cub's sort kernels size their own grids.
+template <int DP, bool ATOMIC>
+static int launch_grouped(HogwildParams p, int reserve, char *ws, const GroupLayout &L, cudaStream_t st) {
+    const int ubits = bits_for((uint64_t)p.n_users);
+    const int64_t n = p.n;
+    const uint64_t first = p.first;
+    int32_t *out_u = p.out_u, *out_i = p.out_i, *out_j = p.out_j;
+    int sms = sm_count() - reserve;
+    if (sms < 1) sms = 1;
+    for (int64_t c0 = 0; c0 < n; c0 += GROUP_MAX) {
+        p.n = n - c0 < GROUP_MAX ? n - c0 : GROUP_MAX;
+        p.first = first + (uint64_t)c0;
+        if (out_u) { p.out_u = out_u + c0; p.out_i = out_i + c0; p.out_j = out_j + c0; }
+        cub::DoubleBuffer<uint32_t> keys((uint32_t *)(ws + L.key_a), (uint32_t *)(ws + L.key_b));
+        cub::DoubleBuffer<int32_t> vals((int32_t *)(ws + L.val_a), (int32_t *)(ws + L.val_b));
+        int64_t grid = (p.n + 255) / 256;
+        if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
+        user_key_kernel<<<(unsigned)grid, 256, 0, st>>>(p, keys.Current(), vals.Current());
+        EB_CUDA(cudaGetLastError());
+        size_t cb = L.cub_bytes;
+        EB_CUDA(cub::DeviceRadixSort::SortPairs(ws + L.cub, cb, keys, vals, (int)p.n, 0, ubits, st));
+        p.order = vals.Current();
+        if (int rc = launch_grouped_t<DP, ATOMIC>(p, reserve, st)) return rc;
+    }
+    return EB_OK;
+}
+
+// SAMPLE: the sampled step; free-running on local tables it runs grouped by user (ws: eb_bpr_step_sampled_workspace_bytes)
 template <bool SAMPLE>
-static int launch_hogwild(const HogwildParams &p, int dp, int flags, cudaStream_t st) {
+static int launch_hogwild(const HogwildParams &p, int dp, int flags, cudaStream_t st, void *ws = nullptr, size_t ws_bytes = 0) {
     const bool atomic = !(flags & 1);
     const bool rounds = (flags & 64) != 0;
     const int reserve = (flags >> 8) & 0xff;
     EB_ARG(!(flags & 32), "the shared-memory-staged kernel exists for sharded item tables only");
     EB_ARG(atomic || !rounds, "deterministic rounds run with atomic updates");
+    if constexpr (SAMPLE) {
+        if (!rounds) {
+            const GroupLayout L = group_layout(p.n, p.n_users);
+            if (!ws || ws_bytes < L.total) return set_err(EB_ERR_WORKSPACE, "workspace %zu < required %zu", ws ? ws_bytes : 0, L.total);
+            // the row stride is checked before anything is launched
+            return with_stride<8, 16, 32, 64, 128, 256>(dp, "8,16,32,64,128,256 floats", [&](auto dpc) {
+                constexpr int DP = decltype(dpc)::value;
+                item_table_l2_window(p, st);
+                return atomic ? launch_grouped<DP, true>(p, reserve, (char *)ws, L, st)
+                              : launch_grouped<DP, false>(p, reserve, (char *)ws, L, st);
+            });
+        }
+    }
     item_table_l2_window(p, st);
     return with_stride<8, 16, 32, 64, 128, 256>(dp, "8,16,32,64,128,256 floats", [&](auto dpc) {
         constexpr int DP = decltype(dpc)::value;
-        if (rounds) return launch_hogwild_t<DP, SAMPLE, true, false, true>(p, reserve, st);
-        return atomic ? launch_hogwild_t<DP, SAMPLE, true, false, false>(p, reserve, st)
-                      : launch_hogwild_t<DP, SAMPLE, false, false, false>(p, reserve, st);
+        if constexpr (!SAMPLE) {
+            if (!rounds) return atomic ? launch_hogwild_t<DP, false, true, false, false>(p, reserve, st)
+                                       : launch_hogwild_t<DP, false, false, false, false>(p, reserve, st);
+        }
+        return launch_hogwild_t<DP, SAMPLE, true, false, true>(p, reserve, st);   // deterministic rounds
     });
 }
 
@@ -716,10 +945,6 @@ __global__ void ranks_kernel(const uint64_t *keys, int64_t m, int ebits, int is_
     else ka[ev >> 1] = rank;
 }
 
-static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
-
-static int bits_for(uint64_t v) { int b = 1; while ((v >> b) != 0) b++; return b; }
-
 struct ExactLayout {
     size_t keys_in, keys_out, ku, ki, kj, cnt, cub, total, cub_bytes;
 };
@@ -786,9 +1011,16 @@ extern "C" int eb_bpr_step_sampled_f32(float *U, float *V, float *item_bias, int
                                        int32_t n_items, const int64_t *csr_indptr, const int32_t *csr_indices,
                                        int64_t n, uint64_t seed, uint64_t first_triple, float lr, float reg_u,
                                        float reg_b, float reg_pos, float reg_neg, double *loss, int32_t *out_u,
-                                       int32_t *out_i, int32_t *out_j, int flags, void *stream) {
+                                       int32_t *out_i, int32_t *out_j, void *workspace, size_t workspace_bytes, int flags,
+                                       void *stream) {
     return eb_bpr_step_sampled_filter_f32(U, V, item_bias, d, ld, n_users, n_items, csr_indptr, csr_indices, nullptr, 0, n, seed,
-                                          first_triple, lr, reg_u, reg_b, reg_pos, reg_neg, loss, out_u, out_i, out_j, flags, stream);
+                                          first_triple, lr, reg_u, reg_b, reg_pos, reg_neg, loss, out_u, out_i, out_j, workspace,
+                                          workspace_bytes, flags, stream);
+}
+
+extern "C" size_t eb_bpr_step_sampled_workspace_bytes(int64_t n, int32_t n_users) {
+    if (n <= 0 || n_users <= 0) return 256;
+    return group_layout(n, n_users).total;
 }
 
 extern "C" int eb_bpr_step_sampled_filter_f32(float *U, float *V, float *item_bias, int d, int ld, int32_t n_users,
@@ -796,7 +1028,7 @@ extern "C" int eb_bpr_step_sampled_filter_f32(float *U, float *V, float *item_bi
                                               const uint32_t *filter, int filter_words, int64_t n, uint64_t seed,
                                               uint64_t first_triple, float lr, float reg_u, float reg_b, float reg_pos,
                                               float reg_neg, double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
-                                              int flags, void *stream) {
+                                              void *workspace, size_t workspace_bytes, int flags, void *stream) {
     if (int rc = check_tables(U, V, item_bias, d, ld)) return rc;
     EB_ARG(n >= 0 && n_users > 0 && n_items > 1, "bad sizes");
     EB_ARG(csr_indptr && csr_indices, "null CSR");
@@ -808,7 +1040,7 @@ extern "C" int eb_bpr_step_sampled_filter_f32(float *U, float *V, float *item_bi
     p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
     p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
     if (int rc = set_filter(p, filter, filter_words)) return rc;
-    return launch_hogwild<true>(p, ld, flags, (cudaStream_t)stream);
+    return launch_hogwild<true>(p, ld, flags, (cudaStream_t)stream, workspace, workspace_bytes);
 }
 
 extern "C" int eb_bpr_step_peer_f32(float *U, float *const *V_shards, float *const *b_shards, int n_shards, int32_t shard_rows,

@@ -75,6 +75,8 @@ def bloom_build(indptr, indices, n_users, words=32):
 def bpr_step_sampled_f32(U, V, b, d, n_users, n_items, indptr, indices, n, seed, first, lr, reg_u, reg_b, reg_pos,
                          reg_neg, loss=None, out=None, racy=False, reserve_sms=0, filter=None, deterministic=False, _variant=0):
     """Fused sample+update step (custom_sampler.py:24-46 distribution, Philox stream).  filter: bloom_build() output.
+    The default free-running Hogwild step applies the triples grouped by user (key pass, stable sort, update; see
+    eb_bpr_step_sampled_f32) with a grow-only device workspace of this module.
     deterministic: run the launch in rounds (reads, grid barrier, atomic adds, grid barrier) so the same inputs give the same
     tables on every run up to fp32 summation order; slower than the default free-running Hogwild.
     _variant (profiling): one table always runs the register-staged kernel (16 or 0); 32, the shared-memory-staged kernel,
@@ -85,11 +87,15 @@ def bpr_step_sampled_f32(U, V, b, d, n_users, n_items, indptr, indices, n, seed,
     if out is not None:
         ou, oi, oj = out
         _need_cuda(ou, oi, oj); _chk_idx(ou, oi, oj)
+    ws = None
+    if not deterministic:
+        ws = _ws_grouped.get(lib().eb_bpr_step_sampled_workspace_bytes(n, n_users), U.device)
     with torch.cuda.device(U.device):
         check(lib().eb_bpr_step_sampled_filter_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), n_users, n_items, _ptr(indptr),
                                                    _ptr(indices), _ptr(filter), 0 if filter is None else filter.shape[1], n, seed,
                                                    first, lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), _ptr(ou), _ptr(oi),
-                                                   _ptr(oj), (1 if racy else 0) | (64 if deterministic else 0) | ((int(reserve_sms) & 0xff) << 8) | int(_variant),
+                                                   _ptr(oj), _ptr(ws), 0 if ws is None else ws.numel(),
+                                                   (1 if racy else 0) | (64 if deterministic else 0) | ((int(reserve_sms) & 0xff) << 8) | int(_variant),
                                                    _stream(U)))
 
 
@@ -157,7 +163,7 @@ class _Workspace:
         return self.buf
 
 
-_ws_exact, _ws_sampler, _ws_score = _Workspace(), _Workspace(), _Workspace()
+_ws_exact, _ws_sampler, _ws_score, _ws_grouped = _Workspace(), _Workspace(), _Workspace(), _Workspace()
 
 
 def bpr_exact_f64(U, V, b, d, tu, ti, tj, lr, reg_u, reg_b, reg_pos, reg_neg, loss=None):

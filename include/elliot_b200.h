@@ -70,14 +70,23 @@ int eb_bpr_step_f32(float *U, float *V, float *item_bias, int d, int ld,
  * u's train items, j uniform over items not in u's train set, by rejection)
  * but a different stream (Philox4x32-10 keyed by seed, counter = triple index
  * `first_triple`+t), then applies the update above.  csr_indices rows must be
- * sorted ascending.  out_u/out_i/out_j (optional) receive the sampled triples. */
+ * sorted ascending.  out_u/out_i/out_j (optional) receive the sampled triples, triple t at index t.
+ * Free-running (flags bit 6 clear), the call is a key pass that writes the user each triple draws, a stable cub radix
+ * sort of the triple indices by user (a histogram kernel, a scan kernel and one pass per 8 key bits: 3 at 1 M users), and
+ * the update, which applies the triples grouped by user in
+ * ascending user order, keeping a user's row in registers across its triples and adding the run's summed update to it
+ * once (a Hogwild launch applies its triples in no fixed order; which triples are drawn does not change).
+ * workspace: device scratch of at least eb_bpr_step_sampled_workspace_bytes(n, n_users) bytes, else EB_ERR_WORKSPACE;
+ * deterministic rounds (flags bit 6) apply the triples in sampler order and may pass NULL.  Flags bits 8..15: the key
+ * pass and the update leave that many SMs free; the sort's kernels size their own grids and do not. */
+size_t eb_bpr_step_sampled_workspace_bytes(int64_t n, int32_t n_users);
 int eb_bpr_step_sampled_f32(float *U, float *V, float *item_bias, int d, int ld,
                             int32_t n_users, int32_t n_items,
                             const int64_t *csr_indptr, const int32_t *csr_indices,
                             int64_t n, uint64_t seed, uint64_t first_triple,
                             float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
                             double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
-                            int flags, void *stream);
+                            void *workspace, size_t workspace_bytes, int flags, void *stream);
 
 /* Per-user membership signatures for the sampler's rejection test (`j in ui`, custom_sampler.py:40-41): a Bloom
  * filter of 32*filter_words bits (filter_words a power of two, 32 = 1024 bits suits ~100 items/user) with 2 hash
@@ -94,7 +103,7 @@ int eb_bpr_step_sampled_filter_f32(float *U, float *V, float *item_bias, int d, 
                                    int64_t n, uint64_t seed, uint64_t first_triple,
                                    float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
                                    double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
-                                   int flags, void *stream);
+                                   void *workspace, size_t workspace_bytes, int flags, void *stream);
 int eb_bpr_sample_philox_filter(int32_t n_users, int32_t n_items, const int64_t *csr_indptr,
                                 const int32_t *csr_indices, const uint32_t *filter, int filter_words, int64_t n,
                                 uint64_t seed, uint64_t first_triple, int32_t *out_u, int32_t *out_i, int32_t *out_j,
