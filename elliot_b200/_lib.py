@@ -134,6 +134,11 @@ SIGNATURES = {
     "eb_knn_score_tile_cols": (c_int, []),
     "eb_knn_score_topk_f32": (c_int, [c_void, c_void, c_void, c_void, c_void, c_void, c_i32, c_void, c_void, c_void, c_i32, c_i64,
                                       c_int, c_int, c_void, c_void, c_void]),
+    "eb_gram_f64_workspace_bytes": (c_size, [c_i64, c_int]),
+    "eb_gram_f64": (c_int, [c_void, c_i64, c_int, c_i64, c_void, c_void, c_size, c_void]),
+    "eb_als_small_d_max": (c_int, []),
+    "eb_als_solve_f64": (c_int, [c_void, c_void, c_i64, c_int, c_void, c_void, c_void, c_void, c_void, c_i64, c_f64, c_void, c_i64,
+                                 c_void]),
 }
 
 _lib = None

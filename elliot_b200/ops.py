@@ -544,6 +544,45 @@ def knn_score_topk(A, B, n_cols, k, frac_bits, mask_indptr=None, mask_indices=No
     return idx, val
 
 
+_ws_gram = _Workspace()
+
+
+def gram_f64(Y, d, n=None, out=None):
+    """G = Y[:n, :d]^T Y[:n, :d] as a fp64 [d][d] tensor, bit-reproducible (eb_gram_f64)."""
+    _need_cuda(Y, out)
+    assert Y.dtype == torch.float64 and Y.stride(1) == 1
+    n = Y.shape[0] if n is None else n
+    if out is None:
+        out = torch.empty((d, d), dtype=torch.float64, device=Y.device)
+    assert out.dtype == torch.float64 and out.is_contiguous() and out.numel() == d * d
+    ws = _ws_gram.get(lib().eb_gram_f64_workspace_bytes(n, d), Y.device)
+    _call("eb_gram_f64", Y, _ptr(Y), n, d, Y.stride(0), _ptr(out), _ptr(ws), ws.numel())
+    return out
+
+
+def als_small_d_max():
+    """Largest d solved one row per warp by als_solve_f64 (larger d: one row per CTA)."""
+    return int(lib().eb_als_small_d_max())
+
+
+def _nonempty(t):
+    """The C ABI takes no NULL arrays: an empty one is passed as a one-element dummy."""
+    return t if t.numel() else torch.zeros(1, dtype=t.dtype, device=t.device)
+
+
+def als_solve_f64(G, Y, d, indptr, indices, w, c, order, reg, X):
+    """X[r] = (G + sum_e w_e y_e y_e^T + reg I)^-1 sum_e c_e y_e for r in `order` (eb_als_solve_f64); the other rows of
+    X are left alone.  Raises EbError (code EB_ERR_DATA) naming the smallest row whose matrix is not positive definite."""
+    _need_cuda(G, Y, indptr, indices, w, c, order, X)
+    assert G.dtype == Y.dtype == X.dtype == w.dtype == c.dtype == torch.float64 and indptr.dtype == torch.int64
+    assert G.is_contiguous() and Y.stride(1) == 1 and X.stride(1) == 1 and w.is_contiguous() and c.is_contiguous()
+    _chk_idx(indices, order)
+    indices, w, c = _nonempty(indices), _nonempty(w), _nonempty(c)
+    _call("eb_als_solve_f64", Y, _ptr(G), _ptr(Y), Y.stride(0), d, _ptr(indptr), _ptr(indices), _ptr(w), _ptr(c), _ptr(order),
+          order.numel(), float(reg), _ptr(X), X.stride(0))
+    return X
+
+
 def dense_topk(scores, k, mask_indptr=None, mask_indices=None, rows=None, shift=None):
     _need_cuda(scores, mask_indptr, mask_indices, rows, shift)
     n = scores.shape[0]

@@ -8,3 +8,4 @@ from .mf2020 import MF2020, MF2020Model  # noqa: F401
 from .multi_dae import MultiDAE, DenoisingAutoEncoder  # noqa: F401
 from .gmf import GMF, GeneralizedMatrixFactorizationModel  # noqa: F401
 from .knn import ItemKNN, UserKNN, KNNModel  # noqa: F401
+from .als import iALS, WRMF, ALSModel  # noqa: F401

@@ -515,6 +515,29 @@ int eb_knn_score_topk_f32(const int64_t *a_indptr, const int32_t *a_indices, con
                           const int32_t *mask_indices, const int32_t *users, int32_t user_begin, int64_t n_sel, int k,
                           int frac_bits, int32_t *out_idx, float *out_val, void *stream);
 
+/* ------------------------------------------------------------------------
+ * iALS / WRMF alternating least squares, fp64 (latent_factor_models/iALS/iALS_model.py:37-65,
+ * latent_factor_models/WRMF/wrmf_model.py:41-58).  Tables are row-major fp64, 1 <= d <= 200.
+ * eb_gram_f64: G[d][d] = Y^T Y over the n rows of Y (row stride ld).  The rows are split into a number of parts that
+ * depends on n only, each summed in row order, and the parts are added in order, so the result is bit-reproducible.
+ * workspace: at least eb_gram_f64_workspace_bytes(n, d) bytes, else EB_ERR_WORKSPACE.
+ * eb_als_solve_f64: for s < n_rows and r = order[s], with the row's entries e in [indptr[r], indptr[r + 1]):
+ *   A = G + sum_e w[e] y y^T + reg I,  b = sum_e c[e] y   (y = Y[indices[e]], row stride ld_y),
+ *   X[r] = A^-1 b (Cholesky factorisation and two triangular solves; row stride ld_x, padding columns untouched).
+ * Rows not listed in `order` are left untouched.  `order` only balances the load (longest rows first is best): the
+ * result of a row does not depend on it, nor on which CTA solves it.  The rank-k updates run on the fp64 tensor cores.
+ * d <= eb_als_small_d_max() solves one row per warp, larger d one row per CTA.  The call synchronises `stream`.  If a
+ * pivot is <= 0 (A not positive definite) the row is not written and EB_ERR_DATA names the smallest such row.  Calls
+ * must not run concurrently on one device (they share the status word).
+ * ------------------------------------------------------------------------ */
+size_t eb_gram_f64_workspace_bytes(int64_t n, int d);
+int eb_gram_f64(const double *Y, int64_t n, int d, int64_t ld, double *G, void *workspace, size_t workspace_bytes,
+                void *stream);
+int eb_als_small_d_max(void);
+int eb_als_solve_f64(const double *G, const double *Y, int64_t ld_y, int d, const int64_t *indptr, const int32_t *indices,
+                     const double *w, const double *c, const int32_t *order, int64_t n_rows, double reg, double *X,
+                     int64_t ld_x, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
