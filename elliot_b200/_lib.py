@@ -139,6 +139,12 @@ SIGNATURES = {
     "eb_als_small_d_max": (c_int, []),
     "eb_als_solve_f64": (c_int, [c_void, c_void, c_i64, c_int, c_void, c_void, c_void, c_void, c_void, c_i64, c_f64, c_void, c_i64,
                                  c_void]),
+    "eb_inverse_f64_workspace_bytes": (c_size, [c_i64]),
+    "eb_inverse_f64": (c_int, [c_void, c_i64, c_i64, c_void, c_size, c_void]),
+    "eb_ease_normal_f64": (c_int, [c_void, c_i64, c_i32, c_i64, c_i64, c_void, c_f64, c_f64, c_void, c_i64, c_void]),
+    "eb_ease_weights_f32": (c_int, [c_void, c_i64, c_i64, c_void, c_i64, c_void]),
+    "eb_dense_score_topk_f32": (c_int, [c_void, c_void, c_void, c_void, c_i64, c_i32, c_void, c_void, c_void, c_i32, c_i64,
+                                        c_int, c_int, c_void, c_void, c_void]),
 }
 
 _lib = None

@@ -13,6 +13,7 @@
 #include <limits.h>
 
 #include "common.cuh"
+#include "dmma.cuh"
 
 namespace eb {
 
@@ -30,14 +31,6 @@ __device__ __forceinline__ int pk(int i, int j) { return i * (i + 1) / 2 + j; }
 
 // row stride of a staged chunk: 16-column tiles plus 4, so the fragment loads of a half-warp hit 16 distinct banks
 __host__ __device__ __forceinline__ int stage_ld(int d) { return (d + 15) / 16 * 16 + 4; }
-
-__device__ __forceinline__ void dmma(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
-    asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
-        "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
-        : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
-        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
-          "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
-}
 
 // One warp: A (packed lower, d x d) += sum_k ws[k] ys[k] ys[k]^T over k < 16 * ksteps, for the lower 16x8 tiles
 // t with t % tstride == t0.  Fragment layouts (PTX ISA, m16n8k16 .f64): g = lane / 4, q = lane % 4;

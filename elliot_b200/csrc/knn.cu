@@ -6,7 +6,9 @@
 //   eb_knn_neighbors_f32    : per row of a Gram slab, cosine (or dot) values and the k largest nonzero ones
 //                             (value desc, column asc) by a three-pass radix select;
 //   eb_knn_score_topk_f32   : pred[p, :] = sum_q A[p, q] B[q, :] (Gustavson, int64 fixed-point accumulators in shared
-//                             memory, order independent), masked, and its top k; the dense score row never reaches HBM.
+//                             memory, order independent), masked, and its top k; the dense score row never reaches HBM;
+//   eb_dense_score_topk_f32 : the same kernel with a dense fp32 B (EASE^R's weights): one thread per column of a tile
+//                             sums that column's terms in a register, so the output equals the sparse path's bit for bit.
 #include <cuda_bf16.h>
 #include <math_constants.h>
 
@@ -246,6 +248,8 @@ struct ScoreKnnParams {
     int k, frac_bits, tile;
     int32_t *out_idx;
     float *out_val;
+    const float *b_dense;       // DENSE: B as a row-major [>= n_mid][ldb] matrix (b_indptr / b_indices / b_values unused)
+    int64_t ldb;
 };
 
 __device__ __forceinline__ int64_t lower_bound64(const int32_t *__restrict__ a, int64_t lo, int64_t hi, int32_t key) {
@@ -256,6 +260,7 @@ __device__ __forceinline__ int64_t lower_bound64(const int32_t *__restrict__ a, 
     return lo;
 }
 
+template <bool DENSE>
 __global__ void __launch_bounds__(KNN_NT) knn_score_topk_kernel(const ScoreKnnParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     long long *acc = reinterpret_cast<long long *>(smem_raw);                       // [tile]
@@ -271,20 +276,34 @@ __global__ void __launch_bounds__(KNN_NT) knn_score_topk_kernel(const ScoreKnnPa
         int cur = 0;
         for (int c0 = 0; c0 < p.n_cols; c0 += p.tile) {
             const int tn = min(p.tile, p.n_cols - c0);
-            for (int i = threadIdx.x; i < tn; i += KNN_NT) acc[i] = 0;
-            __syncthreads();
-            // Gustavson: one warp per A entry walks the B row's part inside this tile
-            for (int64_t e = a0 + warp; e < a1; e += KNN_NT / 32) {
-                const int32_t qq = __ldg(p.a_indices + e);
-                const double a = (double)__ldg(p.a_values + e) * up;
-                const int64_t b0 = p.b_indptr[qq], b1 = p.b_indptr[qq + 1];
-                const int64_t j0 = c0 == 0 ? b0 : lower_bound64(p.b_indices, b0, b1, c0);
-                for (int64_t j = j0 + lane; j < b1; j += 32) {
-                    const int32_t c = __ldg(p.b_indices + j);
-                    if (c >= c0 + tn) break;                                  // rows are sorted
-                    // a * b is exact in double; one rounding to the fixed-point grid per term, then exact int64 sums
-                    const long long t = __double2ll_rn(a * (double)__ldg(p.b_values + j));
-                    atomicAdd(reinterpret_cast<unsigned long long *>(acc + (c - c0)), (unsigned long long)t);
+            if (DENSE) {
+                // one thread per column: the same fixed-point terms as below, summed in a register (B rows coalesced)
+                for (int i = threadIdx.x; i < tn; i += KNN_NT) {
+                    unsigned long long s = 0;
+                    const float *bc = p.b_dense + c0 + i;
+#pragma unroll 4
+                    for (int64_t e = a0; e < a1; e++) {
+                        const double a = (double)__ldg(p.a_values + e) * up;
+                        s += (unsigned long long)__double2ll_rn(a * (double)__ldg(bc + (int64_t)__ldg(p.a_indices + e) * p.ldb));
+                    }
+                    acc[i] = (long long)s;
+                }
+            } else {
+                for (int i = threadIdx.x; i < tn; i += KNN_NT) acc[i] = 0;
+                __syncthreads();
+                // Gustavson: one warp per A entry walks the B row's part inside this tile
+                for (int64_t e = a0 + warp; e < a1; e += KNN_NT / 32) {
+                    const int32_t qq = __ldg(p.a_indices + e);
+                    const double a = (double)__ldg(p.a_values + e) * up;
+                    const int64_t b0 = p.b_indptr[qq], b1 = p.b_indptr[qq + 1];
+                    const int64_t j0 = c0 == 0 ? b0 : lower_bound64(p.b_indices, b0, b1, c0);
+                    for (int64_t j = j0 + lane; j < b1; j += 32) {
+                        const int32_t c = __ldg(p.b_indices + j);
+                        if (c >= c0 + tn) break;                                  // rows are sorted
+                        // a * b is exact in double; one rounding to the fixed-point grid per term, then exact int64 sums
+                        const long long t = __double2ll_rn(a * (double)__ldg(p.b_values + j));
+                        atomicAdd(reinterpret_cast<unsigned long long *>(acc + (c - c0)), (unsigned long long)t);
+                    }
                 }
             }
             __syncthreads();
@@ -320,6 +339,20 @@ __global__ void __launch_bounds__(KNN_NT) knn_score_topk_kernel(const ScoreKnnPa
 static int knn_tile(int32_t n_cols) {
     const int t = (n_cols + 255) / 256 * 256;
     return t < KNN_TILE ? t : KNN_TILE;
+}
+
+template <bool DENSE>
+static int launch_score_topk(const ScoreKnnParams &p, void *stream) {
+    const size_t smem = (size_t)p.tile * 8 + (size_t)2 * KNN_KMAX * 8;
+    EB_CUDA(cudaFuncSetAttribute(knn_score_topk_kernel<DENSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    EB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, knn_score_topk_kernel<DENSE>, KNN_NT, smem));
+    if (per_sm < 1) per_sm = 1;
+    int64_t grid = (int64_t)sm_count() * per_sm;
+    if (grid > p.n_sel) grid = p.n_sel;
+    knn_score_topk_kernel<DENSE><<<(unsigned)grid, KNN_NT, smem, (cudaStream_t)stream>>>(p);
+    EB_CUDA(cudaGetLastError());
+    return EB_OK;
 }
 
 }  // namespace eb
@@ -374,17 +407,23 @@ extern "C" int eb_knn_score_topk_f32(const int64_t *a_indptr, const int32_t *a_i
     EB_ARG(frac_bits >= -1000 && frac_bits <= 1000, "frac_bits=%d out of range", frac_bits);
     EB_ARG((mask_indptr == nullptr) == (mask_indices == nullptr), "mask CSR: both or neither");
     if (n_sel == 0) return EB_OK;
-    const int tile = knn_tile(n_cols);
-    const size_t smem = (size_t)tile * 8 + (size_t)2 * KNN_KMAX * 8;
-    EB_CUDA(cudaFuncSetAttribute(knn_score_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    EB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, knn_score_topk_kernel, KNN_NT, smem));
-    if (per_sm < 1) per_sm = 1;
-    int64_t grid = (int64_t)sm_count() * per_sm;
-    if (grid > n_sel) grid = n_sel;
     ScoreKnnParams p{a_indptr, a_indices, a_values, b_indptr, b_indices, b_values, n_cols, mask_indptr, mask_indices, users,
-                     user_begin, n_sel, k, frac_bits, tile, out_idx, out_val};
-    knn_score_topk_kernel<<<(unsigned)grid, KNN_NT, smem, (cudaStream_t)stream>>>(p);
-    EB_CUDA(cudaGetLastError());
-    return EB_OK;
+                     user_begin, n_sel, k, frac_bits, knn_tile(n_cols), out_idx, out_val, nullptr, 0};
+    return launch_score_topk<false>(p, stream);
+}
+
+extern "C" int eb_dense_score_topk_f32(const int64_t *a_indptr, const int32_t *a_indices, const float *a_values,
+                                       const float *b, int64_t ldb, int32_t n_cols, const int64_t *mask_indptr,
+                                       const int32_t *mask_indices, const int32_t *users, int32_t user_begin, int64_t n_sel,
+                                       int k, int frac_bits, int32_t *out_idx, float *out_val, void *stream) {
+    EB_ARG(a_indptr && a_indices && a_values && b && out_idx && out_val, "null pointer");
+    EB_ARG(n_cols >= 1 && ldb >= n_cols && n_sel >= 0 && user_begin >= 0, "bad shape n_cols=%d ldb=%lld n_sel=%lld", n_cols,
+           (long long)ldb, (long long)n_sel);
+    EB_ARG(k >= 1 && k <= KNN_KMAX, "k=%d outside [1, %d]", k, KNN_KMAX);
+    EB_ARG(frac_bits >= -1000 && frac_bits <= 1000, "frac_bits=%d out of range", frac_bits);
+    EB_ARG((mask_indptr == nullptr) == (mask_indices == nullptr), "mask CSR: both or neither");
+    if (n_sel == 0) return EB_OK;
+    ScoreKnnParams p{a_indptr, a_indices, a_values, nullptr, nullptr, nullptr, n_cols, mask_indptr, mask_indices, users,
+                     user_begin, n_sel, k, frac_bits, knn_tile(n_cols), out_idx, out_val, b, ldb};
+    return launch_score_topk<true>(p, stream);
 }

@@ -583,6 +583,63 @@ def als_solve_f64(G, Y, d, indptr, indices, w, c, order, reg, X):
     return X
 
 
+def inverse_f64(A, n=None):
+    """A[:n, :n] <- its inverse in place (eb_inverse_f64; A fp64, row-major, row stride >= n; padding columns untouched).
+    Raises EbError (code EB_ERR_DATA) naming the column when a pivot is zero or not finite.  The workspace is freed on
+    return."""
+    _need_cuda(A)
+    assert A.dtype == torch.float64 and A.stride(1) == 1
+    n = A.shape[0] if n is None else n
+    assert A.shape[0] >= n and A.shape[1] >= n
+    ws = torch.empty(max(int(lib().eb_inverse_f64_workspace_bytes(n)), 256), dtype=torch.uint8, device=A.device)
+    _call("eb_inverse_f64", A, _ptr(A), n, A.stride(0), _ptr(ws), ws.numel())
+    return A
+
+
+def ease_normal_f64(slab, row0, count, l2_norm, scale, A):
+    """Rows row0 .. row0 + slab.shape[0] of EASE^R's normal matrix into A (fp64 [n][>= n]) from an fp32 Gram slab
+    [S][>= n]: off-diagonal slab * scale, diagonal fp32(count + l2_norm) (eb_ease_normal_f64)."""
+    _need_cuda(slab, count, A)
+    assert slab.dtype == torch.float32 and slab.stride(1) == 1 and A.dtype == torch.float64 and A.stride(1) == 1
+    assert count.dtype == torch.int32 and count.is_contiguous()
+    _call("eb_ease_normal_f64", A, _ptr(slab), slab.stride(0), slab.shape[0], A.shape[0], row0, _ptr(count), float(l2_norm),
+          float(scale), _ptr(A), A.stride(0))
+    return A
+
+
+def ease_weights_f32(P, out=None):
+    """B = fp32(-P / diag(P)) column by column with B[j][j] = 0 (eb_ease_weights_f32).  Raises EbError (code EB_ERR_DATA)
+    naming the column when P[j][j] is zero."""
+    _need_cuda(P, out)
+    assert P.dtype == torch.float64 and P.stride(1) == 1
+    n = P.shape[0]
+    if out is None:
+        out = torch.empty((n, n), dtype=torch.float32, device=P.device)
+    assert out.dtype == torch.float32 and out.stride(1) == 1 and out.shape[1] >= n
+    _call("eb_ease_weights_f32", P, _ptr(P), P.stride(0), n, _ptr(out), out.stride(0))
+    return out
+
+
+def dense_score_topk(A, B, k, frac_bits, mask_indptr=None, mask_indices=None, users=None, user_begin=0, n_sel=None):
+    """knn_score_topk with a dense fp32 B [n_mid][n_cols] (row stride >= n_cols): the same fixed-point terms and selection,
+    so the output equals knn_score_topk's for B as a CSR, bit for bit (eb_dense_score_topk_f32)."""
+    ap, ai, av = A
+    _need_cuda(ap, ai, av, B, mask_indptr, mask_indices, users)
+    assert ap.dtype == torch.int64 and av.dtype == B.dtype == torch.float32 and B.stride(1) == 1
+    _chk_idx(ai)
+    if users is not None:
+        _chk_idx(users)
+        n_sel = users.numel()
+    elif n_sel is None:
+        n_sel = ap.numel() - 1 - user_begin
+    idx = torch.empty((n_sel, k), dtype=torch.int32, device=ap.device)
+    val = torch.empty((n_sel, k), dtype=torch.float32, device=ap.device)
+    ai, av = _nonempty(ai), _nonempty(av)
+    _call("eb_dense_score_topk_f32", ap, _ptr(ap), _ptr(ai), _ptr(av), _ptr(B), B.stride(0), B.shape[1],
+          _ptr(mask_indptr), _ptr(mask_indices), _ptr(users), user_begin, n_sel, k, int(frac_bits), _ptr(idx), _ptr(val))
+    return idx, val
+
+
 def dense_topk(scores, k, mask_indptr=None, mask_indices=None, rows=None, shift=None):
     _need_cuda(scores, mask_indptr, mask_indices, rows, shift)
     n = scores.shape[0]

@@ -9,3 +9,4 @@ from .multi_dae import MultiDAE, DenoisingAutoEncoder  # noqa: F401
 from .gmf import GMF, GeneralizedMatrixFactorizationModel  # noqa: F401
 from .knn import ItemKNN, UserKNN, KNNModel  # noqa: F401
 from .als import iALS, WRMF, ALSModel  # noqa: F401
+from .ease import EASER, EASEModel  # noqa: F401

@@ -28,7 +28,7 @@ SLAB_BYTES = 2 << 30            # fp32 Gram rows computed per GEMM call
 EXACT_LIMIT = float(1 << 24)    # every integer below it is exact in fp32
 
 
-def exactness_scale(values):
+def exactness_scale(values, who="ItemKNN/UserKNN need"):
     """Smallest s in 0..4 such that every value * 2^s is an integer of magnitude <= 256.  Refuses other data: the bf16
     Gram is exact only for such values, and there is no other path."""
     v = np.asarray(values, dtype=np.float64)
@@ -36,7 +36,7 @@ def exactness_scale(values):
         x = v * (1 << s)
         if np.all(x == np.round(x)) and np.abs(x).max(initial=0.0) <= 256:
             return s
-    raise ValueError("ItemKNN/UserKNN need ratings that become integers of magnitude <= 256 when multiplied by 1, 2, 4, 8 "
+    raise ValueError(f"{who} ratings that become integers of magnitude <= 256 when multiplied by 1, 2, 4, 8 "
                      "or 16 (for example 1-5, half stars, implicit ones); these ratings do not, and the tensor-core "
                      "Gram matrix would not be exact")
 
@@ -60,11 +60,12 @@ def _bound(A, B):
     return float(_row_abs_sums(A[0], A[2]).max().item()) * float(B[2].abs().max().item())
 
 
-def neighbours(urm, n_users, n_items, over, k, cosine, slab_rows=None):
-    """Neighbour lists of every item (over="items") or user (over="users").  urm: (indptr, indices, values) on the device.
-    Returns (idx int32 [n][k], val fp32 [n][k]): value desc then index asc, -1 / 0 padded."""
+def dense_operand(urm, n_users, n_items, over, who="ItemKNN/UserKNN need"):
+    """The exact bf16 Gram operand of the ratings: (X = ratings * 2^s as bf16 [n_users][pad8(n_items)], s, the Gram
+    diagonal as fp32).  urm: (indptr, indices, values) on the device.  Refuses ratings for which the tensor-core Gram
+    would not be exact."""
     indptr, indices, values = urm
-    s = exactness_scale(values.cpu().numpy())
+    s = exactness_scale(values.cpu().numpy(), who)
     dev = indptr.device
     ld = (n_items + 7) // 8 * 8
     need = n_users * ld * 2
@@ -79,13 +80,19 @@ def neighbours(urm, n_users, n_items, over, k, cosine, slab_rows=None):
     if n and float(diag.max().item()) >= EXACT_LIMIT:
         raise ValueError(f"a squared {'item' if items else 'user'} norm of the scaled ratings reaches 2^24: the fp32 Gram "
                          f"matrix would not be exact")
+    return X, s, diag
+
+
+def gram_slabs(X, n_users, n_items, over, slab_rows=None):
+    """The exact fp32 Gram matrix of dense_operand()'s X (X^T X for over="items", X X^T for "users"), in row slabs: yields
+    (j0, C) with C the rows j0 .. j0 + C.shape[0], in order.  C is one buffer, overwritten by the next slab."""
+    items = over == "items"
+    n = n_items if items else n_users
     if slab_rows is None:
         slab_rows = max(8, SLAB_BYTES // (4 * max(n, 1)) // 8 * 8)
     slab_rows = min(slab_rows, (n + 7) // 8 * 8)
     assert slab_rows % 8 == 0, "slab starts must stay 16-byte aligned"
-    slab = torch.empty((slab_rows, n), dtype=torch.float32, device=dev)
-    idx = torch.empty((n, k), dtype=torch.int32, device=dev)
-    val = torch.empty((n, k), dtype=torch.float32, device=dev)
+    slab = torch.empty((slab_rows, n), dtype=torch.float32, device=X.device)
     for j0 in range(0, n, slab_rows):
         S = min(slab_rows, n - j0)
         C = slab[:S]
@@ -93,8 +100,19 @@ def neighbours(urm, n_users, n_items, over, k, cosine, slab_rows=None):
             ops.gemm_bf16(X[:, j0:], X, S, n, n_users, a_rows_are_k=True, b_rows_are_k=True, out=C)
         else:           # rows j0.. of X X^T
             ops.gemm_bf16(X[j0:], X, S, n, n_items, out=C)
+        yield j0, C
+
+
+def neighbours(urm, n_users, n_items, over, k, cosine, slab_rows=None):
+    """Neighbour lists of every item (over="items") or user (over="users").  urm: (indptr, indices, values) on the device.
+    Returns (idx int32 [n][k], val fp32 [n][k]): value desc then index asc, -1 / 0 padded."""
+    X, s, diag = dense_operand(urm, n_users, n_items, over)
+    n = n_items if over == "items" else n_users
+    idx = torch.empty((n, k), dtype=torch.int32, device=X.device)
+    val = torch.empty((n, k), dtype=torch.float32, device=X.device)
+    for j0, C in gram_slabs(X, n_users, n_items, over, slab_rows):
         i, v, _ = ops.knn_neighbors(C, n, j0, diag, k, cosine=cosine, dot_scale=4.0 ** -s)
-        idx[j0:j0 + S], val[j0:j0 + S] = i, v
+        idx[j0:j0 + C.shape[0]], val[j0:j0 + C.shape[0]] = i, v
     return idx, val
 
 

@@ -538,6 +538,33 @@ int eb_als_solve_f64(const double *G, const double *Y, int64_t ld_y, int d, cons
                      const double *w, const double *c, const int32_t *order, int64_t n_rows, double reg, double *X,
                      int64_t ld_x, void *stream);
 
+/* ------------------------------------------------------------------------
+ * EASE^R (autoencoders/EASE_R/ease_r.py:69-91) and the dense linear algebra it needs, fp64.
+ * eb_inverse_f64: A[n][n] (row stride ld >= n; padding columns untouched) is replaced by its inverse.  Blocked
+ * Gauss-Jordan elimination with partial pivoting: the pivot of a column is its largest |a| on or below the diagonal
+ * (the lowest row on a tie); the trailing updates are fp64 tensor-core GEMMs.  Works for any nonsingular matrix, definite
+ * or not.  Reruns are bit-identical.  workspace: at least eb_inverse_f64_workspace_bytes(n) bytes, else
+ * EB_ERR_WORKSPACE.  A pivot that is exactly zero or not finite stops the call with EB_ERR_DATA naming the column (A is
+ * then left partly transformed).  The call synchronises `stream`; calls must not run concurrently on one device (they
+ * share the status word).  1 <= n <= 4 194 240.
+ * eb_ease_normal_f64: rows row0 .. row0 + n_rows of EASE^R's normal matrix from the same rows of an fp32 Gram slab (row
+ * stride ld_slab): A[i][j] = slab[i - row0][j] * scale for j != i and A[i][i] = (double)(float)(count[i] + l2_norm),
+ * the fp64 sum rounded to fp32 as the reference stores it into its float32 matrix.
+ * eb_ease_weights_f32: B[i][j] = (float)(-P[i][j] / P[j][j]) (one fp64 divide, one rounding) and B[j][j] = 0.  A zero
+ * P[j][j] returns EB_ERR_DATA naming the smallest such j.  The call synchronises `stream`.
+ * eb_dense_score_topk_f32: eb_knn_score_topk_f32 with a dense row-major B (row stride ldb): the same fixed-point terms,
+ * mask and selection, so its output equals eb_knn_score_topk_f32's for the same B given as a CSR, bit for bit.
+ * ------------------------------------------------------------------------ */
+size_t eb_inverse_f64_workspace_bytes(int64_t n);
+int eb_inverse_f64(double *A, int64_t n, int64_t ld, void *workspace, size_t workspace_bytes, void *stream);
+int eb_ease_normal_f64(const float *slab, int64_t ld_slab, int32_t n_rows, int64_t n, int64_t row0, const int32_t *count,
+                       double l2_norm, double scale, double *A, int64_t ld, void *stream);
+int eb_ease_weights_f32(const double *P, int64_t ld_p, int64_t n, float *B, int64_t ld_b, void *stream);
+int eb_dense_score_topk_f32(const int64_t *a_indptr, const int32_t *a_indices, const float *a_values, const float *b,
+                            int64_t ldb, int32_t n_cols, const int64_t *mask_indptr, const int32_t *mask_indices,
+                            const int32_t *users, int32_t user_begin, int64_t n_sel, int k, int frac_bits,
+                            int32_t *out_idx, float *out_val, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
