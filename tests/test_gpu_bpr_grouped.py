@@ -78,8 +78,9 @@ def _heavy():
 def test_grouped_step_with_heavy_user_repetition():
     """50 users and 200K triples per call: user runs straddle lane-group and window boundaries and many warps add partial
     updates to the same user row.  Emitted triples equal the sampler's; with zero regularisation the column sums of V and the
-    sum of b are invariant (every triple adds +lr z u' to V_i and -lr z u' to V_j); the batch loss drops and the tables
-    track sequential SGD on the emitted triples (correlation > 0.98); lr = 0 leaves the tables bit-identical."""
+    sum of b are invariant (every triple adds +lr z u' to V_i and -lr z u' to V_j); the batch loss drops and the user rows
+    move as sequential SGD on the emitted triples moves them (relative Frobenius error of U1 - U0, which a lost or doubled
+    flush of a run would blow up); lr = 0 leaves the tables bit-identical."""
     nu, ni, d, rows = _heavy()
     indptr, idx = _csr(rows)
     n = 200_000
@@ -105,8 +106,12 @@ def test_grouped_step_with_heavy_user_repetition():
     Uh, Vh = U[:, :d].double().cpu().numpy(), V[:, :d].double().cpu().numpy()
     l1 = oracle.bpr_loss(Uh, Vh, b.double().cpu().numpy(), tu, ti, tj)
     assert l1 < l0
-    cu = np.corrcoef(Uh.ravel(), Us.ravel())[0, 1]; cv = np.corrcoef(Vh.ravel(), Vs.ravel())[0, 1]
-    assert cu > 0.98 and cv > 0.98, (cu, cv)
+    # Hogwild staleness alone: 0.134-0.136 over 5 runs on an H100 80GB HBM3 (700 W); bound with 1.5x margin
+    U0h = U0[:, :d].double().cpu().numpy()
+    eu = np.linalg.norm((Uh - U0h) - (Us - U0h)) / np.linalg.norm(Us - U0h)
+    assert eu < 0.2, eu
+    cv = np.corrcoef(Vh.ravel(), Vs.ravel())[0, 1]
+    assert cv > 0.98, cv
 
     U, V, b = U0.clone(), V0.clone(), b0.clone()
     _fused(U, V, b, d, nu, ni, indptr, idx, n, 10, (0.0,) + HP[1:])
