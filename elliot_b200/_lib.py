@@ -145,6 +145,16 @@ SIGNATURES = {
     "eb_ease_weights_f32": (c_int, [c_void, c_i64, c_i64, c_void, c_i64, c_void]),
     "eb_dense_score_topk_f32": (c_int, [c_void, c_void, c_void, c_void, c_i64, c_i32, c_void, c_void, c_void, c_i32, c_i64,
                                         c_int, c_int, c_void, c_void, c_void]),
+    "eb_rp3_tile_cols": (c_int, []),
+    "eb_rp3_row_workspace_bytes": (c_size, [c_i32]),
+    "eb_rp3_similarity_f32": (c_int, [c_void, c_void, c_void, c_void, c_void, c_void, c_void, c_i32, c_void, c_int, c_i64,
+                                      c_void, c_void, c_void, c_void, c_size, c_void]),
+    "eb_rp3_l1_rows_f32": (c_int, [c_i32, c_i64, c_void, c_void, c_void]),
+    "eb_rp3_prune_workspace_bytes": (c_size, [c_i32, c_i64, c_i64]),
+    "eb_rp3_prune_cols_f32": (c_int, [c_i32, c_i64, c_void, c_void, c_void, c_i64, c_int, c_void, c_void, c_void, c_void, c_size,
+                                      c_void]),
+    "eb_rp3_score_topk_f32": (c_int, [c_void, c_void, c_void, c_void, c_void, c_void, c_i32, c_void, c_void, c_void, c_i32, c_i64,
+                                      c_void, c_int, c_void, c_void, c_void, c_size, c_void]),
 }
 
 _lib = None

@@ -640,6 +640,87 @@ def dense_score_topk(A, B, k, frac_bits, mask_indptr=None, mask_indices=None, us
     return idx, val
 
 
+def rp3_tile_cols():
+    return int(lib().eb_rp3_tile_cols())
+
+
+def _rp3_row_ws(n_cols, device):
+    return torch.empty(max(int(lib().eb_rp3_row_workspace_bytes(n_cols)), 1), dtype=torch.uint8, device=device)
+
+
+def rp3_similarity(A, B, degree, k, order=None):
+    """RP3beta's neighbour lists (eb_rp3_similarity_f32): per row i of the ordered fp32 product A . B (A = Piu, B = Pui
+    with rows sorted by column; (indptr int64, indices int32, values fp32) on the device), times degree (fp64) with the
+    diagonal zeroed, the min(k, n) largest nonzero values in column order.  Returns (idx int32 [n][kk], val fp32 [n][kk],
+    cnt int32 [n]) with kk = min(k, n)."""
+    (ap, ai, av), (bp, bi, bv) = A, B
+    _need_cuda(ap, ai, av, bp, bi, bv, degree, order)
+    assert ap.dtype == bp.dtype == torch.int64 and av.dtype == bv.dtype == torch.float32 and degree.dtype == torch.float64
+    _chk_idx(ai, bi)
+    n = degree.numel()
+    kk = min(k, n)
+    idx = torch.empty((n, kk), dtype=torch.int32, device=ap.device)
+    val = torch.empty((n, kk), dtype=torch.float32, device=ap.device)
+    cnt = torch.empty(n, dtype=torch.int32, device=ap.device)
+    if order is not None:
+        _chk_idx(order)
+    ws = _rp3_row_ws(n, ap.device)
+    ai, av, bi, bv = _nonempty(ai), _nonempty(av), _nonempty(bi), _nonempty(bv)
+    _call("eb_rp3_similarity_f32", ap, _ptr(ap), _ptr(ai), _ptr(av), _ptr(bp), _ptr(bi), _ptr(bv), _ptr(degree), n, _ptr(order),
+          k, kk, _ptr(idx), _ptr(val), _ptr(cnt), _ptr(ws), ws.numel())
+    return idx, val, cnt
+
+
+def rp3_l1_rows(val, cnt):
+    """val[r, :cnt[r]] <- fp32(v / sum |v|) in place, the sum in fp64 in stored order (eb_rp3_l1_rows_f32)."""
+    _need_cuda(val, cnt)
+    assert val.dtype == torch.float32 and val.stride(1) == 1 and cnt.dtype == torch.int32 and cnt.is_contiguous()
+    _call("eb_rp3_l1_rows_f32", val, val.shape[0], val.stride(0), _ptr(cnt), _ptr(val))
+    return val
+
+
+def rp3_prune_cols(idx, val, cnt, k):
+    """W as a CSR (indptr int64, indices int32, values fp32) from rp3_similarity's lists, keeping per column the k largest
+    nonzero values, ties to the lowest row (eb_rp3_prune_cols_f32).  Rows list their columns ascending."""
+    _need_cuda(idx, val, cnt)
+    assert idx.is_contiguous() and val.is_contiguous() and idx.shape == val.shape
+    n, stride = idx.shape
+    nnz = int(cnt.sum().item())
+    dev = idx.device
+    indptr = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    indices = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
+    values = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
+    ws = torch.empty(int(lib().eb_rp3_prune_workspace_bytes(n, stride, nnz)), dtype=torch.uint8, device=dev)
+    _call("eb_rp3_prune_cols_f32", idx, n, stride, _ptr(cnt), _ptr(idx), _ptr(val), nnz, k, _ptr(indptr), _ptr(indices),
+          _ptr(values), _ptr(ws), ws.numel())
+    m = int(indptr[-1].item())
+    return indptr, indices[:m].clone(), values[:m].clone()
+
+
+def rp3_score_topk(A, B, n_cols, k, mask_indptr=None, mask_indices=None, users=None, user_begin=0, n_sel=None, order=None):
+    """Top k of the rows of the ordered fp32 product A . B (eb_rp3_score_topk_f32; A's rows summed in stored order, B's
+    rows sorted by column) with the masked columns excluded, (score desc, column asc): (idx int32 [n_sel][k], val fp32
+    [n_sel][k])."""
+    (ap, ai, av), (bp, bi, bv) = A, B
+    _need_cuda(ap, ai, av, bp, bi, bv, mask_indptr, mask_indices, users, order)
+    assert ap.dtype == bp.dtype == torch.int64 and av.dtype == bv.dtype == torch.float32
+    _chk_idx(ai, bi)
+    if users is not None:
+        _chk_idx(users)
+        n_sel = users.numel()
+    elif n_sel is None:
+        n_sel = ap.numel() - 1 - user_begin
+    if order is not None:
+        _chk_idx(order)
+    idx = torch.empty((n_sel, k), dtype=torch.int32, device=ap.device)
+    val = torch.empty((n_sel, k), dtype=torch.float32, device=ap.device)
+    ws = _rp3_row_ws(n_cols, ap.device)
+    ai, av, bi, bv = _nonempty(ai), _nonempty(av), _nonempty(bi), _nonempty(bv)
+    _call("eb_rp3_score_topk_f32", ap, _ptr(ap), _ptr(ai), _ptr(av), _ptr(bp), _ptr(bi), _ptr(bv), n_cols, _ptr(mask_indptr),
+          _ptr(mask_indices), _ptr(users), user_begin, n_sel, _ptr(order), k, _ptr(idx), _ptr(val), _ptr(ws), ws.numel())
+    return idx, val
+
+
 def dense_topk(scores, k, mask_indptr=None, mask_indices=None, rows=None, shift=None):
     _need_cuda(scores, mask_indptr, mask_indices, rows, shift)
     n = scores.shape[0]

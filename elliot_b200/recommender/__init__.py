@@ -10,3 +10,4 @@ from .gmf import GMF, GeneralizedMatrixFactorizationModel  # noqa: F401
 from .knn import ItemKNN, UserKNN, KNNModel  # noqa: F401
 from .als import iALS, WRMF, ALSModel  # noqa: F401
 from .ease import EASER, EASEModel  # noqa: F401
+from .rp3beta import RP3beta, RP3Model  # noqa: F401

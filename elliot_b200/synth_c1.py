@@ -120,6 +120,36 @@ def ease_yaml(tsv, out_dir, extra="", model_extra=""):
 {model_extra}"""
 
 
+def rp3beta_yaml(tsv, out_dir, extra="", model_extra=""):
+    """config_files/recsys_config.yml's RP3beta block (neighborhood 546, alpha 1.0807, beta 0.7029, normalize_similarity
+    True) with save_recs, over the C1 layout above."""
+    return f"""experiment:
+  dataset: c1_synth
+  data_config:
+    strategy: dataset
+    dataset_path: {tsv}
+  splitting:
+    test_splitting:
+      strategy: random_subsampling
+      test_ratio: 0.2
+  top_k: 10
+  evaluation:
+    simple_metrics: [nDCG, HR, Precision, Recall]
+  path_output_rec_result: {out_dir}/recs
+  path_output_rec_weight: {out_dir}/weights
+  path_output_rec_performance: {out_dir}/performance
+  path_log_folder: {out_dir}/log
+{extra}  models:
+    RP3beta:
+      meta:
+        save_recs: True
+      neighborhood: 546
+      alpha: 1.0807
+      beta: 0.7029
+      normalize_similarity: True
+{model_extra}"""
+
+
 def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra="", seed=42):
     """The reference's YAML layout (sample_hello_world.yml:1-19 with a `BPRMF:` block, BPRMF.py:43-56 keys)."""
     return f"""experiment:

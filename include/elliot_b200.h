@@ -565,6 +565,42 @@ int eb_dense_score_topk_f32(const int64_t *a_indptr, const int32_t *a_indices, c
                             const int32_t *users, int32_t user_begin, int64_t n_sel, int k, int frac_bits,
                             int32_t *out_idx, float *out_val, void *stream);
 
+/* ------------------------------------------------------------------------
+ * RP3beta (graph_based/RP3beta/rp3beta.py:73-176).  The float32 sparse products are SciPy's, bit for bit: output row r of
+ * A . B is acc[c] = fp32(acc[c] + fp32(A[r, e] * B[e, c])) over A's row entries e in stored order (one rounded product,
+ * one rounded add, no FMA, no atomics).  B's rows are sorted by column.  Output rows are visited in `order` (a
+ * permutation of 0 .. n_sel - 1, NULL: ascending), which balances the load only.  Catalogues wider than
+ * eb_rp3_tile_cols() columns are processed in column tiles and need a workspace of eb_rp3_row_workspace_bytes(n_cols)
+ * bytes (0 otherwise), else EB_ERR_WORKSPACE.
+ * eb_rp3_similarity_f32: row i of A . B (A = Piu, users ascending; B = Pui), each value times degree[c] in fp64 and the
+ * diagonal zeroed; the min(k, n_items) largest nonzero fp64 values (ties: lowest column first) go to out_idx/out_val
+ * [n_items][stride] as fp32, in column order, with out_cnt[n_items].
+ * eb_rp3_l1_rows_f32: val[r][j] = fp32(val[r][j] / sum_j |val[r][j]|) for j < cnt[r], the sum in fp64 in stored order
+ * (rows that sum to 0 are left alone).
+ * eb_rp3_prune_cols_f32: W given as eb_rp3_similarity_f32's lists (nnz = sum of cnt); per column the k largest nonzero
+ * values (ties: lowest row first) are kept and written as a CSR (out_indptr [n + 1], out_indices / out_values with room
+ * for nnz entries, columns ascending in every row).  workspace: eb_rp3_prune_workspace_bytes(n, stride, nnz) bytes.
+ * eb_rp3_score_topk_f32: for output row q (user users[q], or user_begin + q when users is NULL) the scores A[u] . B over
+ * n_cols columns; train items (mask CSR) are excluded; the k best by (score desc, column asc) go to out_idx/out_val
+ * [n_sel][k], padded with -1 / -inf when fewer than k columns are unmasked.  1 <= k <= 1024.
+ * ------------------------------------------------------------------------ */
+int eb_rp3_tile_cols(void);
+size_t eb_rp3_row_workspace_bytes(int32_t n_cols);
+int eb_rp3_similarity_f32(const int64_t *a_indptr, const int32_t *a_indices, const float *a_values, const int64_t *b_indptr,
+                          const int32_t *b_indices, const float *b_values, const double *degree, int32_t n_items,
+                          const int32_t *order, int k, int64_t stride, int32_t *out_idx, float *out_val, int32_t *out_cnt,
+                          void *workspace, size_t workspace_bytes, void *stream);
+int eb_rp3_l1_rows_f32(int32_t n_rows, int64_t stride, const int32_t *cnt, float *val, void *stream);
+size_t eb_rp3_prune_workspace_bytes(int32_t n, int64_t stride, int64_t nnz);
+int eb_rp3_prune_cols_f32(int32_t n, int64_t stride, const int32_t *cnt, const int32_t *idx, const float *val, int64_t nnz,
+                          int k, int64_t *out_indptr, int32_t *out_indices, float *out_values, void *workspace,
+                          size_t workspace_bytes, void *stream);
+int eb_rp3_score_topk_f32(const int64_t *a_indptr, const int32_t *a_indices, const float *a_values, const int64_t *b_indptr,
+                          const int32_t *b_indices, const float *b_values, int32_t n_cols, const int64_t *mask_indptr,
+                          const int32_t *mask_indices, const int32_t *users, int32_t user_begin, int64_t n_sel,
+                          const int32_t *order, int k, int32_t *out_idx, float *out_val, void *workspace,
+                          size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
