@@ -9,160 +9,25 @@
 //                             memory, order independent), masked, and its top k; the dense score row never reaches HBM;
 //   eb_dense_score_topk_f32 : the same kernel with a dense fp32 B (EASE^R's weights): one thread per column of a tile
 //                             sums that column's terms in a register, so the output equals the sparse path's bit for bit.
+// Both selects run block_select.cuh on 32-bit float keys with 11-bit digits and sort 64-bit (value, column) pair keys.
 #include <cuda_bf16.h>
 #include <math_constants.h>
 
+#include "block_select.cuh"
 #include "common.cuh"
 
 namespace eb {
 
 constexpr int KNN_NT = 512;                  // threads per CTA, both selection kernels
-constexpr int KNN_BINS = 2048;               // radix digit: 11 + 11 + 10 bits
-constexpr int KNN_KMAX = 1024;
+constexpr int KNN_BITS = 11;                 // radix digit: 11 + 11 + 10 bits of the float keys
 constexpr int KNN_TILE = 24576;              // int64 accumulators per score tile (192 KB of shared memory)
 constexpr long long KNN_MASKED = (long long)0x8000000000000000ull;
 
-// order-preserving map of a float onto uint32 (larger value -> larger key)
-__device__ __forceinline__ uint32_t fkey(float v) {
-    const uint32_t u = __float_as_uint(v);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-__device__ __forceinline__ bool before(float va, int ia, float vb, int ib) {   // (value desc, index asc)
-    return va > vb || (va == vb && ia < ib);
-}
-
-struct SelShared {
-    uint32_t hist[KNN_BINS];
-    int warp_sum[KNN_NT / 32];
-    int bin, above, total, base, placed;
-};
-
-// exclusive prefix of `flag` over the block in thread order; every thread gets the block total in `total`
-__device__ __forceinline__ int block_excl_scan(int x, SelShared &sh, int &total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int v = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += y;
-    }
-    if (lane == 31) sh.warp_sum[warp] = v;
-    __syncthreads();
-    int before_w = 0, t = 0;
-#pragma unroll
-    for (int w = 0; w < KNN_NT / 32; w++) {
-        const int s = sh.warp_sum[w];
-        if (w < warp) before_w += s;
-        t += s;
-    }
-    __syncthreads();
-    total = t;
-    return before_w + v - x;
-}
-
-// Histogram done: find the bin (counted from the top) where the running count of candidates reaches `need`.
-// Sets sh.bin and sh.above (candidates in higher bins) and sh.total (all candidates in the histogram).
-__device__ void find_bin(SelShared &sh, int need) {
-    constexpr int PER = KNN_BINS / KNN_NT;
-    const int top = KNN_BINS - 1 - PER * (int)threadIdx.x;                  // this thread's bins: top, top-1, ...
-    int s = 0;
-#pragma unroll
-    for (int j = 0; j < PER; j++) s += (int)sh.hist[top - j];
-    int total;
-    const int pre = block_excl_scan(s, sh, total);
-    if (threadIdx.x == 0) sh.total = total;
-    if (pre < need && need <= pre + s) {
-        int c = pre;
-#pragma unroll
-        for (int j = 0; j < PER; j++) {
-            const int h = (int)sh.hist[top - j];
-            if (c + h >= need) { sh.bin = top - j; sh.above = c; break; }
-            c += h;
-        }
-    }
-    __syncthreads();
-}
-
-// Top-k threshold of the candidates get(i, v) (i in [0, n)): returns the key T of the k-th best and the number of
-// candidates with key == T to take (the first ones by index).  When there are at most k candidates, T = 0 and every
-// candidate is taken (no float has key 0 except a NaN pattern, which never occurs here).
-template <class Get>
-__device__ void radix_threshold(const Get &get, int n, int k, SelShared &sh, uint32_t &T, int &need_eq) {
-    uint32_t prefix = 0, hi_mask = 0;
-    int need = k;
-    const int shifts[3] = {21, 10, 0}, widths[3] = {11, 11, 10};
-    for (int pass = 0; pass < 3; pass++) {
-        for (int b = threadIdx.x; b < KNN_BINS; b += KNN_NT) sh.hist[b] = 0;
-        __syncthreads();
-        const int sft = shifts[pass];
-        const uint32_t dmask = (1u << widths[pass]) - 1u;
-        for (int i = threadIdx.x; i < n; i += KNN_NT) {
-            float v;
-            if (!get(i, v)) continue;
-            const uint32_t key = fkey(v);
-            if ((key & hi_mask) == prefix) atomicAdd(&sh.hist[(key >> sft) & dmask], 1u);
-        }
-        __syncthreads();
-        find_bin(sh, need);
-        if (pass == 0 && sh.total <= k) { T = 0; need_eq = 0; return; }   // uniform: every candidate is taken
-        prefix |= (uint32_t)sh.bin << sft;
-        hi_mask |= dmask << sft;
-        need -= sh.above;
-        __syncthreads();
-    }
-    T = prefix;
-    need_eq = need;
-}
-
-// Appends the selected candidates (key > T, then the first need_eq with key == T in index order) to (bv, bi)[base..).
-// Returns how many were appended (placement order is arbitrary; the caller sorts).
-template <class Get>
-__device__ int collect(const Get &get, int n, uint32_t T, int need_eq, float *bv, int *bi, int base, int idx_offset,
-                       SelShared &sh) {
-    if (threadIdx.x == 0) sh.placed = 0;
-    int eq_seen = 0;
-    __syncthreads();
-    for (int i0 = 0; i0 < n; i0 += KNN_NT) {
-        const int i = i0 + (int)threadIdx.x;
-        float v = 0.f;
-        const bool c = i < n && get(i, v);
-        const uint32_t key = c ? fkey(v) : 0u;
-        const bool eq = c && key == T && need_eq > 0;
-        int eq_total;
-        const int r = block_excl_scan(eq ? 1 : 0, sh, eq_total);             // uniform call
-        const bool take = (c && key > T) || (eq && eq_seen + r < need_eq);
-        if (take) {
-            const int slot = atomicAdd(&sh.placed, 1);
-            bv[base + slot] = v;
-            bi[base + slot] = i + idx_offset;
-        }
-        eq_seen += eq_total;
-    }
-    __syncthreads();
-    return sh.placed;
-}
-
-// bitonic sort of (bv, bi)[0..m) by (value desc, index asc); slots [m, pow2) are padded with sentinels
-__device__ void sort_pairs(float *bv, int *bi, int m) {
-    int P = 1;
-    while (P < m) P <<= 1;
-    for (int i = m + (int)threadIdx.x; i < P; i += KNN_NT) { bv[i] = -CUDART_INF_F; bi[i] = 0x7fffffff; }
-    __syncthreads();
-    for (int size = 2; size <= P; size <<= 1) {
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int t = threadIdx.x; t < P / 2; t += KNN_NT) {
-                const int lo = 2 * t - (t & (stride - 1));
-                const int hi = lo + stride;
-                const bool up = (lo & size) == 0;                             // ascending in (before) order
-                const float va = bv[lo], vb = bv[hi];
-                const int ia = bi[lo], ib = bi[hi];
-                if (before(vb, ib, va, ia) == up) { bv[lo] = vb; bi[lo] = ib; bv[hi] = va; bi[hi] = ia; }
-            }
-            __syncthreads();
-        }
-    }
-}
+// Both kernels key a candidate value v by fkey(v) for the select and by pair_key(v, column) for the sort.  pair_key order
+// is (v desc, column asc) under the order of the float bits, which differs from the order of the values only for -0.0 vs
+// +0.0 and for NaN.  Neither is ever a candidate: the neighbour rows drop v == 0 and hold cosine or dot values of an exact
+// Gram, which are finite; a score is fp32((double)x * 2^-f) of an int64 x, never -0.0 or NaN.
+using KnnShared = SelectShared<KNN_NT, KNN_BITS>;
 
 // ---------------------------------------------------------------- densify
 __global__ void csr_to_dense_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
@@ -203,9 +68,8 @@ struct NbrParams {
 };
 
 __global__ void __launch_bounds__(KNN_NT) knn_neighbors_kernel(const NbrParams p) {
-    __shared__ SelShared sh;
-    __shared__ float bv[KNN_KMAX];
-    __shared__ int bi[KNN_KMAX];
+    __shared__ KnnShared sh;
+    __shared__ uint64_t keys[SELECT_KMAX];
     for (int s = blockIdx.x; s < p.n_rows; s += gridDim.x) {
         float *row = p.slab + (int64_t)s * p.ld;
         const double grr = (double)p.diag[p.row0 + s];
@@ -221,16 +85,18 @@ __global__ void __launch_bounds__(KNN_NT) knn_neighbors_kernel(const NbrParams p
             row[c] = v;
         }
         __syncthreads();
-        auto get = [row](int i, float &v) { v = row[i]; return v != 0.f; };
+        auto get = [row](int i, uint32_t &key) {
+            const float v = row[i];
+            key = fkey(v);
+            return v != 0.f;
+        };
         uint32_t T;
         int need_eq;
         radix_threshold(get, p.n, p.k, sh, T, need_eq);
-        const int m = collect(get, p.n, T, need_eq, bv, bi, 0, 0, sh);
-        sort_pairs(bv, bi, m);
-        for (int j = threadIdx.x; j < p.k; j += KNN_NT) {
-            p.out_idx[(int64_t)s * p.k + j] = j < m ? bi[j] : -1;
-            p.out_val[(int64_t)s * p.k + j] = j < m ? bv[j] : 0.f;
-        }
+        const int m = collect(get, p.n, T, need_eq, sh,
+                              [](int slot, int i, uint32_t key) { keys[slot] = pair_key(unfkey(key), (uint32_t)i); });
+        sort_desc<KNN_NT>(keys, m);
+        write_topk<KNN_NT>(keys, m, p.k, p.out_idx + (int64_t)s * p.k, p.out_val + (int64_t)s * p.k, 0.f);
         if (threadIdx.x == 0) p.out_cnt[s] = m;
         __syncthreads();
     }
@@ -264,9 +130,8 @@ template <bool DENSE>
 __global__ void __launch_bounds__(KNN_NT) knn_score_topk_kernel(const ScoreKnnParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     long long *acc = reinterpret_cast<long long *>(smem_raw);                       // [tile]
-    float *bv = reinterpret_cast<float *>(acc + p.tile);                             // [2 * KNN_KMAX]
-    int *bi = reinterpret_cast<int *>(bv + 2 * KNN_KMAX);                            // [2 * KNN_KMAX]
-    __shared__ SelShared sh;
+    uint64_t *keys = reinterpret_cast<uint64_t *>(acc + p.tile);                    // [2 * SELECT_KMAX]
+    __shared__ KnnShared sh;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const double up = ldexp(1.0, p.frac_bits), down = ldexp(1.0, -p.frac_bits);
     for (int64_t q = blockIdx.x; q < p.n_sel; q += gridDim.x) {
@@ -316,22 +181,21 @@ __global__ void __launch_bounds__(KNN_NT) knn_score_topk_kernel(const ScoreKnnPa
                 }
             }
             __syncthreads();
-            auto get = [acc, down](int i, float &v) {
+            auto get = [acc, down](int i, uint32_t &key) {
                 const long long x = acc[i];
-                v = (float)((double)x * down);
+                key = fkey((float)((double)x * down));
                 return x != KNN_MASKED;
             };
             uint32_t T;
             int need_eq;
             radix_threshold(get, tn, p.k, sh, T, need_eq);
-            const int m = collect(get, tn, T, need_eq, bv, bi, cur, c0, sh);
-            sort_pairs(bv, bi, cur + m);
+            const int m = collect(get, tn, T, need_eq, sh, [keys, cur, c0](int slot, int i, uint32_t key) {
+                keys[cur + slot] = pair_key(unfkey(key), (uint32_t)(i + c0));
+            });
+            sort_desc<KNN_NT>(keys, cur + m);
             cur = min(cur + m, p.k);
         }
-        for (int j = threadIdx.x; j < p.k; j += KNN_NT) {
-            p.out_idx[q * p.k + j] = j < cur ? bi[j] : -1;
-            p.out_val[q * p.k + j] = j < cur ? bv[j] : -CUDART_INF_F;
-        }
+        write_topk<KNN_NT>(keys, cur, p.k, p.out_idx + q * p.k, p.out_val + q * p.k, -CUDART_INF_F);
         __syncthreads();
     }
 }
@@ -343,7 +207,7 @@ static int knn_tile(int32_t n_cols) {
 
 template <bool DENSE>
 static int launch_score_topk(const ScoreKnnParams &p, void *stream) {
-    const size_t smem = (size_t)p.tile * 8 + (size_t)2 * KNN_KMAX * 8;
+    const size_t smem = (size_t)p.tile * 8 + (size_t)2 * SELECT_KMAX * 8;
     EB_CUDA(cudaFuncSetAttribute(knn_score_topk_kernel<DENSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
     EB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, knn_score_topk_kernel<DENSE>, KNN_NT, smem));
@@ -384,7 +248,7 @@ extern "C" int eb_knn_neighbors_f32(float *slab, int64_t ld, int32_t n_rows, int
                                     void *stream) {
     EB_ARG(slab && diag && out_idx && out_val && out_cnt, "null pointer");
     EB_ARG(n >= 1 && ld >= n && n_rows >= 0 && row0 >= 0, "bad shape n=%d ld=%lld n_rows=%d", n, (long long)ld, n_rows);
-    EB_ARG(k >= 1 && k <= KNN_KMAX, "k=%d outside [1, %d]", k, KNN_KMAX);
+    EB_ARG(k >= 1 && k <= SELECT_KMAX, "k=%d outside [1, %d]", k, SELECT_KMAX);
     if (n_rows == 0) return EB_OK;
     NbrParams p{slab, ld, n_rows, n, row0, diag, cosine ? 1 : 0, dot_scale, k, out_idx, out_val, out_cnt};
     int64_t grid = (int64_t)sm_count() * 4;
@@ -403,7 +267,7 @@ extern "C" int eb_knn_score_topk_f32(const int64_t *a_indptr, const int32_t *a_i
                                      float *out_val, void *stream) {
     EB_ARG(a_indptr && a_indices && a_values && b_indptr && b_indices && b_values && out_idx && out_val, "null pointer");
     EB_ARG(n_cols >= 1 && n_sel >= 0 && user_begin >= 0, "bad shape n_cols=%d n_sel=%lld", n_cols, (long long)n_sel);
-    EB_ARG(k >= 1 && k <= KNN_KMAX, "k=%d outside [1, %d]", k, KNN_KMAX);
+    EB_ARG(k >= 1 && k <= SELECT_KMAX, "k=%d outside [1, %d]", k, SELECT_KMAX);
     EB_ARG(frac_bits >= -1000 && frac_bits <= 1000, "frac_bits=%d out of range", frac_bits);
     EB_ARG((mask_indptr == nullptr) == (mask_indices == nullptr), "mask CSR: both or neither");
     if (n_sel == 0) return EB_OK;
@@ -419,7 +283,7 @@ extern "C" int eb_dense_score_topk_f32(const int64_t *a_indptr, const int32_t *a
     EB_ARG(a_indptr && a_indices && a_values && b && out_idx && out_val, "null pointer");
     EB_ARG(n_cols >= 1 && ldb >= n_cols && n_sel >= 0 && user_begin >= 0, "bad shape n_cols=%d ldb=%lld n_sel=%lld", n_cols,
            (long long)ldb, (long long)n_sel);
-    EB_ARG(k >= 1 && k <= KNN_KMAX, "k=%d outside [1, %d]", k, KNN_KMAX);
+    EB_ARG(k >= 1 && k <= SELECT_KMAX, "k=%d outside [1, %d]", k, SELECT_KMAX);
     EB_ARG(frac_bits >= -1000 && frac_bits <= 1000, "frac_bits=%d out of range", frac_bits);
     EB_ARG((mask_indptr == nullptr) == (mask_indices == nullptr), "mask CSR: both or neither");
     if (n_sel == 0) return EB_OK;

@@ -7,8 +7,11 @@
 //   rp3_rows_kernel<false>  : score row u = R[u] . W, train items masked, the k best (score desc, column asc);
 //   rp3_l1_rows_kernel      : W rows <- fp32(v / sum |v|), the sum in fp64 in stored (column) order;
 //   prune kernels           : per column of W the k largest nonzero values (value desc, row asc), W rebuilt as a CSR.
+// The three selects run block_select.cuh on 64-bit keys with 8-bit digits: fp64 bit patterns (similarity) or
+// (value, index) pair keys (scores, prune).
 #include <math_constants.h>
 
+#include "block_select.cuh"
 #include "common.cuh"
 
 namespace eb {
@@ -16,117 +19,9 @@ namespace eb {
 constexpr int RP3_NT = 512;                  // threads per CTA
 constexpr int RP3_NW = RP3_NT / 32;
 constexpr int RP3_TILE = 49152;              // fp32 accumulators per column tile (192 KB of shared memory)
-constexpr int RP3_KMAX = 1024;               // scoring: largest k
+constexpr int RP3_BITS = 8;                  // radix digit: 8 x 8 bits of the 64-bit keys
 
-// order-preserving map of a float onto uint32 (larger value -> larger key) and back
-__device__ __forceinline__ uint32_t fkey32(float v) {
-    const uint32_t u = __float_as_uint(v);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float unfkey32(uint32_t k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-// (value desc, index asc) as one distinct 64-bit key: larger key first
-__device__ __forceinline__ uint64_t pair_key(float v, uint32_t i) { return ((uint64_t)fkey32(v) << 32) | (0xffffffffu - i); }
-
-struct Rp3Sel {
-    uint32_t hist[256];
-    int warp_sum[RP3_NW];
-    int bin, above, total;
-};
-
-// exclusive prefix of x over the block in thread order; every thread gets the block total
-__device__ __forceinline__ int rp3_excl_scan(int x, Rp3Sel &sh, int &total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int v = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += y;
-    }
-    if (lane == 31) sh.warp_sum[warp] = v;
-    __syncthreads();
-    int before_w = 0, t = 0;
-#pragma unroll
-    for (int w = 0; w < RP3_NW; w++) {
-        const int s = sh.warp_sum[w];
-        if (w < warp) before_w += s;
-        t += s;
-    }
-    __syncthreads();
-    total = t;
-    return before_w + v - x;
-}
-
-// Key T of the k-th largest candidate key (get(i, key) over i in [0, n)) by an 8 x 8-bit radix select, and how many
-// candidates with key == T to take (the first ones by index).  At most k candidates: T = 0, need_eq = 0, and every
-// candidate is taken (candidate keys are never 0).
-template <class Get>
-__device__ void rp3_threshold(const Get &get, int n, int k, Rp3Sel &sh, uint64_t &T, int &need_eq) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint64_t prefix = 0, hi_mask = 0;
-    int need = k;
-    for (int pass = 0; pass < 8; pass++) {
-        const int sft = 56 - 8 * pass;
-        for (int b = threadIdx.x; b < 256; b += RP3_NT) sh.hist[b] = 0;
-        __syncthreads();
-        for (int i = threadIdx.x; i < n; i += RP3_NT) {
-            uint64_t key;
-            if (get(i, key) && (key & hi_mask) == prefix) atomicAdd(&sh.hist[(key >> sft) & 255u], 1u);
-        }
-        __syncthreads();
-        if (warp == 0) {                                   // lane l owns bins 255 - 8l .. 248 - 8l, counted from the top
-            int c[8], s = 0;
-#pragma unroll
-            for (int j = 0; j < 8; j++) { c[j] = (int)sh.hist[255 - 8 * lane - j]; s += c[j]; }
-            int incl = s;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int y = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += y;
-            }
-            const int pre = incl - s;
-            if (lane == 31) sh.total = incl;
-            if (pre < need && need <= incl) {
-                int cc = pre;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    if (cc + c[j] >= need) { sh.bin = 255 - 8 * lane - j; sh.above = cc; break; }
-                    cc += c[j];
-                }
-            }
-        }
-        __syncthreads();
-        if (pass == 0 && sh.total <= k) { T = 0; need_eq = 0; return; }   // uniform
-        prefix |= (uint64_t)sh.bin << sft;
-        hi_mask |= (uint64_t)255u << sft;
-        need -= sh.above;
-    }
-    T = prefix;
-    need_eq = need;
-}
-
-// Calls emit(slot, i, key) for the selected candidates (key > T, then the first need_eq with key == T) with slots
-// 0, 1, ... in index order.  Returns how many were selected.
-template <class Get, class Emit>
-__device__ int rp3_collect(const Get &get, int n, uint64_t T, int need_eq, Rp3Sel &sh, const Emit &emit) {
-    int base = 0, eq_seen = 0;
-    for (int i0 = 0; i0 < n; i0 += RP3_NT) {
-        const int i = i0 + (int)threadIdx.x;
-        uint64_t key = 0;
-        const bool c = i < n && get(i, key);
-        const bool eq = c && need_eq > 0 && key == T;
-        int eq_total = 0, er = 0;
-        if (need_eq > 0) er = rp3_excl_scan(eq ? 1 : 0, sh, eq_total);      // uniform condition
-        const bool take = (c && key > T) || (eq && eq_seen + er < need_eq);
-        int total;
-        const int slot = rp3_excl_scan(take ? 1 : 0, sh, total);
-        if (take) emit(base + slot, i, key);
-        base += total;
-        eq_seen += eq_total;
-    }
-    return base;
-}
+using Rp3Sel = SelectShared<RP3_NT, RP3_BITS>;
 
 // first index in [lo, hi) of the sorted a[] with a[idx] >= key; every lane of the warp gets it (<= 2 probe rounds for
 // rows of up to 1 024 entries)
@@ -187,29 +82,12 @@ __device__ __forceinline__ void rp3_accumulate(const Rp3Params &p, float *acc, i
     }
 }
 
-__device__ void rp3_sort_desc(uint64_t *kk, int m) {        // bitonic, slots [m, pow2) padded with 0 (sorts last)
-    int P = 1;
-    while (P < m) P <<= 1;
-    for (int i = m + (int)threadIdx.x; i < P; i += RP3_NT) kk[i] = 0;
-    __syncthreads();
-    for (int size = 2; size <= P; size <<= 1) {
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int t = threadIdx.x; t < P / 2; t += RP3_NT) {
-                const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-                const bool up = (lo & size) == 0;
-                const uint64_t a = kk[lo], b = kk[hi];
-                if ((b > a) == up) { kk[lo] = b; kk[hi] = a; }
-            }
-            __syncthreads();
-        }
-    }
-}
-
+// Three CTAs per SM (40 registers) whenever the accumulator row leaves room for them.
 template <bool SIM>
-__global__ void __launch_bounds__(RP3_NT) rp3_rows_kernel(const Rp3Params p) {
+__global__ void __launch_bounds__(RP3_NT, 3) rp3_rows_kernel(const Rp3Params p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *acc = reinterpret_cast<float *>(smem_raw);                                  // [tile]
-    uint64_t *keys = reinterpret_cast<uint64_t *>(acc + p.tile);                       // [RP3_KMAX], scoring only
+    uint64_t *keys = reinterpret_cast<uint64_t *>(acc + p.tile);                       // [SELECT_KMAX], scoring only
     __shared__ Rp3Sel sh;
     const bool tiled = p.n_cols > p.tile;
     float *grow = tiled ? p.row_ws + (int64_t)blockIdx.x * p.n_cols : nullptr;
@@ -246,10 +124,10 @@ __global__ void __launch_bounds__(RP3_NT) rp3_rows_kernel(const Rp3Params p) {
             };
             uint64_t T;
             int need_eq;
-            rp3_threshold(get, p.n_cols, p.k, sh, T, need_eq);
+            radix_threshold(get, p.n_cols, p.k, sh, T, need_eq);
             int32_t *oi = p.out_idx + q * p.stride;
             float *ov = p.out_val + q * p.stride;
-            const int m = rp3_collect(get, p.n_cols, T, need_eq, sh, [oi, ov](int slot, int i, uint64_t key) {
+            const int m = collect(get, p.n_cols, T, need_eq, sh, [oi, ov](int slot, int i, uint64_t key) {
                 oi[slot] = i;
                 ov[slot] = (float)__longlong_as_double((long long)key);
             });
@@ -262,14 +140,11 @@ __global__ void __launch_bounds__(RP3_NT) rp3_rows_kernel(const Rp3Params p) {
             };
             uint64_t T;
             int need_eq;
-            rp3_threshold(get, p.n_cols, p.k, sh, T, need_eq);
-            const int m = rp3_collect(get, p.n_cols, T, need_eq, sh, [keys](int slot, int, uint64_t key) { keys[slot] = key; });
-            rp3_sort_desc(keys, m);
-            for (int j = threadIdx.x; j < p.k; j += RP3_NT) {
-                const uint64_t key = j < m ? keys[j] : 0;
-                p.out_idx[q * p.stride + j] = j < m ? (int32_t)(0xffffffffu - (uint32_t)key) : -1;
-                p.out_val[q * p.stride + j] = j < m ? unfkey32((uint32_t)(key >> 32)) : -CUDART_INF_F;
-            }
+            radix_threshold(get, p.n_cols, p.k, sh, T, need_eq);
+            auto put = [keys](int slot, int, uint64_t key) { keys[slot] = key; };
+            const int m = collect(get, p.n_cols, T, need_eq, sh, put);
+            sort_desc<RP3_NT>(keys, m);
+            write_topk<RP3_NT>(keys, m, p.k, p.out_idx + q * p.stride, p.out_val + q * p.stride, -CUDART_INF_F);
         }
         __syncthreads();
     }
@@ -345,7 +220,7 @@ __global__ void __launch_bounds__(RP3_NT) rp3_select_cols_kernel(int32_t n, int6
         const uint64_t *ck = ckeys + col_ptr[c];
         const int len = (int)(col_ptr[c + 1] - col_ptr[c]);
         auto mark = [=](int, int, uint64_t key) {
-            const int64_t r = 0xffffffffu - (uint32_t)key;
+            const int64_t r = pair_index(key);
             const int32_t *row = idx + r * stride;
             int lo = 0, hi = cnt[r];
             while (lo < hi) {
@@ -361,8 +236,8 @@ __global__ void __launch_bounds__(RP3_NT) rp3_select_cols_kernel(int32_t n, int6
         auto get = [ck](int i, uint64_t &key) { key = ck[i]; return true; };
         uint64_t T;
         int need_eq;
-        rp3_threshold(get, len, k, sh, T, need_eq);
-        rp3_collect(get, len, T, need_eq, sh, mark);
+        radix_threshold(get, len, k, sh, T, need_eq);
+        collect(get, len, T, need_eq, sh, mark);
         __syncthreads();
     }
 }
@@ -424,7 +299,7 @@ static PruneWs prune_ws(void *base, int32_t n, int64_t stride, int64_t nnz) {
 }
 
 static size_t rows_smem(const Rp3Params &p, bool sim) {
-    return (size_t)p.tile * 4 + (sim ? 0 : (size_t)RP3_KMAX * 8);
+    return (size_t)p.tile * 4 + (sim ? 0 : (size_t)SELECT_KMAX * 8);
 }
 
 template <bool SIM>
@@ -530,7 +405,7 @@ extern "C" int eb_rp3_score_topk_f32(const int64_t *a_indptr, const int32_t *a_i
                                      float *out_val, void *workspace, size_t workspace_bytes, void *stream) {
     EB_ARG(a_indptr && a_indices && a_values && b_indptr && b_indices && b_values && out_idx && out_val, "null pointer");
     EB_ARG(n_cols >= 1 && n_sel >= 0 && user_begin >= 0, "bad shape n_cols=%d n_sel=%lld", n_cols, (long long)n_sel);
-    EB_ARG(k >= 1 && k <= RP3_KMAX, "k=%d outside [1, %d]", k, RP3_KMAX);
+    EB_ARG(k >= 1 && k <= SELECT_KMAX, "k=%d outside [1, %d]", k, SELECT_KMAX);
     EB_ARG((mask_indptr == nullptr) == (mask_indices == nullptr), "mask CSR: both or neither");
     if (n_sel == 0) return EB_OK;
     Rp3Params p{};
