@@ -155,6 +155,13 @@ SIGNATURES = {
                                       c_void]),
     "eb_rp3_score_topk_f32": (c_int, [c_void, c_void, c_void, c_void, c_void, c_void, c_i32, c_void, c_void, c_void, c_i32, c_i64,
                                       c_void, c_int, c_void, c_void, c_void, c_size, c_void]),
+    "eb_slim_shared_residual_fits": (c_int, [c_i32]),
+    "eb_slim_slots": (c_int, [c_i32, c_int]),
+    "eb_slim_workspace_bytes": (c_size, [c_i32, c_i32, c_i32, c_int]),
+    "eb_slim_fit_f32": (c_int, [c_void, c_void, c_void, c_void, c_void, c_i32, c_i32, c_i32, c_i32, c_f32, c_f32, c_f32,
+                                ctypes.c_uint32, c_int, c_int, c_int, c_i32, c_void, c_void, c_void, c_void, c_void, c_void,
+                                c_size, c_void]),
+    "eb_slim_drop_f32": (c_int, [c_i32, c_void, c_void, c_void]),
 }
 
 _lib = None

@@ -732,6 +732,75 @@ def dense_topk(scores, k, mask_indptr=None, mask_indices=None, rows=None, shift=
     return idx, val
 
 
+# ---------------------------------------------------------------- SLIM (slim.cu)
+def slim_slots(n_users, shared_residual):
+    return int(lib().eb_slim_slots(int(n_users), int(shared_residual)))
+
+
+def slim_shared_residual_fits(n_users):
+    return bool(lib().eb_slim_shared_residual_fits(int(n_users)))
+
+
+def slim_workspace_bytes(n_users, n_items, slots, shared_residual):
+    return int(lib().eb_slim_workspace_bytes(int(n_users), int(n_items), int(slots), int(shared_residual)))
+
+
+def slim_fit(csc, csr, n_users, n_items, l1, l2, seed, neighborhood, tol=1e-4, max_iter=100, shared_residual=None,
+             slots=None, items=None):
+    """Every item's SLIM elastic net (eb_slim_fit_f32).  csc = (colptr int64, rows int32, vals fp32) of X [users][items],
+    csr = (rowptr int64, cols int32) of X's pattern.  Returns (coef_t [n_items][n_items] fp32 with coef_t[i, p] the
+    coefficient of item i for item p, n_iter int32, gap fp32, nnz int32, drop int32), all indexed by item.  `items`
+    (begin, end) fits that range only (the other columns stay 0).  shared_residual None: shared memory when it fits."""
+    cp, ri, cv = csc
+    rp, ci = csr
+    _need_cuda(cp, ri, cv, rp, ci)
+    dev = cp.device
+    with torch.cuda.device(dev):
+        if shared_residual is None:
+            shared_residual = slim_shared_residual_fits(n_users)
+        cap = slim_slots(n_users, shared_residual)
+        if cap < 1:
+            raise RuntimeError(f"SLIM: no CTA fits for {n_users} users with shared_residual={shared_residual}")
+        slots = cap if slots is None else max(1, min(int(slots), cap))
+        coef_t = torch.zeros((n_items, n_items), dtype=torch.float32, device=dev)
+        n_iter = torch.zeros(n_items, dtype=torch.int32, device=dev)
+        gap = torch.zeros(n_items, dtype=torch.float32, device=dev)
+        nnz = torch.zeros(n_items, dtype=torch.int32, device=dev)
+        drop = torch.full((n_items,), -1, dtype=torch.int32, device=dev)
+        b, e = (0, n_items) if items is None else (int(items[0]), int(items[1]))
+        ws_bytes = slim_workspace_bytes(n_users, n_items, slots, shared_residual)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    _call("eb_slim_fit_f32", cp, _ptr(cp), _ptr(ri), _ptr(cv), _ptr(rp), _ptr(ci), int(n_users), int(n_items), b, e - b,
+          float(l1), float(l2), float(tol), int(seed) & 0xffffffff, int(max_iter), int(neighborhood), int(shared_residual),
+          int(slots), _ptr(coef_t), _ptr(n_iter), _ptr(gap), _ptr(nnz), _ptr(drop), _ptr(ws), ws_bytes)
+    return coef_t, n_iter, gap, nnz, drop
+
+
+def slim_weights(coef_t, drop, nnz, neighborhood):
+    """W as a CSR (indptr int64, indices int32, values fp32; rows list their columns ascending) from slim_fit's outputs:
+    per column p the min(nnz_p - 1, neighborhood) largest coefficients, ties to the lowest item.  The entry `drop`
+    names is removed first (eb_slim_drop_f32); the rest is eb_rp3_prune_cols_f32 with k = neighborhood over W's dense
+    rows.  coef_t is not modified."""
+    _need_cuda(coef_t, drop, nnz)
+    n = coef_t.shape[0]
+    dev = coef_t.device
+    with torch.cuda.device(dev):
+        vals = coef_t.clone()
+    _call("eb_slim_drop_f32", vals, n, _ptr(drop), _ptr(vals))
+    with torch.cuda.device(dev):
+        total = int(torch.clamp(nnz.to(torch.int64), min=0).sum().item())
+        idx = torch.arange(n, dtype=torch.int32, device=dev).repeat(n)
+        cnt = torch.full((n,), n, dtype=torch.int32, device=dev)
+        indptr = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        indices = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
+        values = torch.empty(max(total, 1), dtype=torch.float32, device=dev)
+        ws = torch.empty(int(lib().eb_rp3_prune_workspace_bytes(n, n, total)), dtype=torch.uint8, device=dev)
+    _call("eb_rp3_prune_cols_f32", vals, n, n, _ptr(cnt), _ptr(idx), _ptr(vals), total, int(neighborhood), _ptr(indptr),
+          _ptr(indices), _ptr(values), _ptr(ws), ws.numel())
+    m = int(indptr[-1].item())
+    return indptr, indices[:m], values[:m]
+
+
 # ---------------------------------------------------------------- NeuMF pieces (neumf.cu)
 def _call(name, dev_tensor, *args):
     with torch.cuda.device(dev_tensor.device):

@@ -11,3 +11,4 @@ from .knn import ItemKNN, UserKNN, KNNModel  # noqa: F401
 from .als import iALS, WRMF, ALSModel  # noqa: F401
 from .ease import EASER, EASEModel  # noqa: F401
 from .rp3beta import RP3beta, RP3Model  # noqa: F401
+from .slim import Slim, SlimModel  # noqa: F401

@@ -150,6 +150,35 @@ def rp3beta_yaml(tsv, out_dir, extra="", model_extra=""):
 {model_extra}"""
 
 
+def slim_yaml(tsv, out_dir, extra="", model_extra=""):
+    """config_files/recsys_config.yml's Slim block (l1_ratio 0.0000119, alpha 0.0788, neighborhood 544) with save_recs,
+    over the C1 layout above."""
+    return f"""experiment:
+  dataset: c1_synth
+  data_config:
+    strategy: dataset
+    dataset_path: {tsv}
+  splitting:
+    test_splitting:
+      strategy: random_subsampling
+      test_ratio: 0.2
+  top_k: 10
+  evaluation:
+    simple_metrics: [nDCG, HR, Precision, Recall]
+  path_output_rec_result: {out_dir}/recs
+  path_output_rec_weight: {out_dir}/weights
+  path_output_rec_performance: {out_dir}/performance
+  path_log_folder: {out_dir}/log
+{extra}  models:
+    Slim:
+      meta:
+        save_recs: True
+      l1_ratio: 0.0000119
+      alpha: 0.0788
+      neighborhood: 544
+{model_extra}"""
+
+
 def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra="", seed=42):
     """The reference's YAML layout (sample_hello_world.yml:1-19 with a `BPRMF:` block, BPRMF.py:43-56 keys)."""
     return f"""experiment:

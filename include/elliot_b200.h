@@ -601,6 +601,31 @@ int eb_rp3_score_topk_f32(const int64_t *a_indptr, const int32_t *a_indices, con
                           const int32_t *order, int k, int32_t *out_idx, float *out_val, void *workspace,
                           size_t workspace_bytes, void *stream);
 
+/* ------------------------------------------------------------------------
+ * SLIM (latent_factor_models/Slim/slim_model.py:44-113): per item p, sklearn's positive ElasticNet (fit_intercept=False,
+ * selection='random') by sparse coordinate descent on X (CSC colptr/rows/vals, users ascending in every column; the CSR
+ * pattern rowptr/cols gives user p's columns) with user row p read as zero and y = X[:, p].  l1 = fp32(alpha * l1_ratio *
+ * n_users), l2 = fp32(alpha * (1 - l1_ratio) * n_users), tol (1e-4), seed: the xorshift state every fit starts from.
+ * The coordinate updates reproduce the reference's float32 arithmetic; the gap's reductions run in fp64.
+ * eb_slim_fit_f32 fits items item_begin .. item_begin + n_problems - 1, `slots` at a time (each slot holds one problem's
+ * rows in the workspace, eb_slim_workspace_bytes(n_users, n_items, slots, shared_residual) bytes); the residual lives in
+ * shared memory when shared_residual is 1 (eb_slim_shared_residual_fits(n_users)), otherwise in the workspace.
+ * Outputs by item p: coef_t[i * n_items + p] = coefficient of item i, n_iter[p] (sklearn's n_iter_), gap[p] (sklearn's
+ * dual_gap_), nnz[p] (nonzero coefficients) and drop[p]: the coefficient the min(nnz - 1, neighborhood) rule removes
+ * when 1 <= nnz <= neighborhood (the smallest, ties: the highest item), else -1.  Requires n_items <= n_users.
+ * eb_slim_slots: how many problems run at once on this device.
+ * eb_slim_drop_f32: coef_t[drop[p] * n_items + p] = 0 wherever drop[p] >= 0.
+ * ------------------------------------------------------------------------ */
+int eb_slim_shared_residual_fits(int32_t n_users);
+int eb_slim_slots(int32_t n_users, int shared_residual);
+size_t eb_slim_workspace_bytes(int32_t n_users, int32_t n_items, int32_t slots, int shared_residual);
+int eb_slim_fit_f32(const int64_t *colptr, const int32_t *rows, const float *vals, const int64_t *rowptr, const int32_t *cols,
+                    int32_t n_users, int32_t n_items, int32_t item_begin, int32_t n_problems, float l1, float l2, float tol,
+                    uint32_t seed, int max_iter, int neighborhood, int shared_residual, int32_t slots, float *coef_t,
+                    int32_t *n_iter, float *gap, int32_t *nnz, int32_t *drop, void *workspace, size_t workspace_bytes,
+                    void *stream);
+int eb_slim_drop_f32(int32_t n_items, const int32_t *drop, float *coef_t, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
