@@ -27,6 +27,7 @@ from .. import ops
 from .._lib import EbError
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import TopKRecs, cuda_device, upload
 
 MAX_FACTORS = 200              # the top of the reference's own search range (config_files/recsys_config.yml, iALS block)
 
@@ -68,7 +69,7 @@ class ALSModel:
         else:
             w, c = wrmf_confidences(m, alpha)
         self.w_host, self.c_host = w, c
-        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(self.device, dt)
+        dev = self.device
         # item side: the transpose, its entries permuted along (users ascending within an item)
         nnz = m.nnz
         t = sp.csr_matrix((np.arange(nnz, dtype=np.int64), m.indices, m.indptr), shape=m.shape).tocsc()
@@ -78,11 +79,11 @@ class ALSModel:
         order_i = np.argsort(-lens_i, kind="stable")
         if kind == "iALS":
             order_i = order_i[lens_i[order_i] > 0]          # iALS_model.py:37-38: only warm items are solved
-        self.users = (to(m.indptr, torch.int64), to(m.indices, torch.int32), to(w, torch.float64), to(c, torch.float64),
-                      to(order_u, torch.int32))
-        self.items = (to(t.indptr, torch.int64), to(t.indices, torch.int32), to(w[perm], torch.float64),
-                      to(c[perm], torch.float64), to(order_i, torch.int32))
-        self.X, self.Y = to(X0, torch.float64), to(Y0, torch.float64)
+        self.users = (upload(m.indptr, dev, torch.int64), upload(m.indices, dev, torch.int32), upload(w, dev, torch.float64),
+                      upload(c, dev, torch.float64), upload(order_u, dev, torch.int32))
+        self.items = (upload(t.indptr, dev, torch.int64), upload(t.indices, dev, torch.int32), upload(w[perm], dev, torch.float64),
+                      upload(c[perm], dev, torch.float64), upload(order_i, dev, torch.int32))
+        self.X, self.Y = upload(X0, dev, torch.float64), upload(Y0, dev, torch.float64)
         self.G = torch.empty((self.d, self.d), dtype=torch.float64, device=self.device)
         self.G2 = torch.empty_like(self.G)
 
@@ -114,7 +115,7 @@ class ALSModel:
         return ops.score_topk(self.X, self.Y, None, self.d, k, mask_indptr, mask_indices, users=users)
 
 
-class _ALS(RecMixin, BaseRecommenderModel):
+class _ALS(TopKRecs, RecMixin, BaseRecommenderModel):
     _kind = None
 
     def _check(self):
@@ -124,32 +125,11 @@ class _ALS(RecMixin, BaseRecommenderModel):
         if self._save_weights or self._restore:
             raise NotImplementedError(f"meta.save_weights / meta.restore are not supported for {self._kind}: the "
                                       f"reference pickles the dense prediction matrix, which this build never forms")
-        if not torch.cuda.is_available():
-            raise RuntimeError(f"elliot_b200.{type(self).__name__} needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, type(self).__name__)
 
     @property
     def name(self):
         return f"{self._kind}_{self.get_base_params_shortcut()}_{self.get_params_shortcut()}"
-
-    def get_recommendations(self, k: int = 10):
-        recs_val, recs_test = self.process_protocol(k)
-        return dict(recs_val), dict(recs_test)
-
-    def get_recommendations_tensors(self, k: int = 10):
-        return self._model.topk(k, self._indptr, self._sorted_idx)
-
-    def get_single_recommendation(self, mask, k, *args):
-        if self._negative_sampling:
-            raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
-        idx, val = self.get_recommendations_tensors(k)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy()
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
-        return out
 
     def train(self):
         for it in self.iterate(self._epochs):

@@ -24,6 +24,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import TopKRecs, cuda_device
 
 
 class MFModel:
@@ -106,7 +107,7 @@ class MFModel:
             pickle.dump(self.get_model_state(), f)
 
 
-class BPRMF(RecMixin, BaseRecommenderModel):
+class BPRMF(TopKRecs, RecMixin, BaseRecommenderModel):
     r"""Bayesian Personalized Ranking MF (https://arxiv.org/abs/1205.2618) on the H100.
 
     YAML block identical to the reference's (BPRMF.py:37-56):
@@ -136,9 +137,7 @@ class BPRMF(RecMixin, BaseRecommenderModel):
         if self._mode == "hogwild" and not hasattr(self._params, "b200_eval"):
             self._params.b200_eval = "device"          # throughput mode: metrics straight from the top-k tensor
         self._batch_size = 1                                    # BPRMF.py:80 (YAML batch_size ignored)
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.BPRMF needs a CUDA device (there is no CPU fallback)")
+        self._device = cuda_device(self._params, "BPRMF")
         # construction order as in BPRMF.py:83-91: model (seeds np.random with the model seed),
         # then the sampler (reseeds the global stream with 42)
         self._model = MFModel(self._factors, self._data, self._learning_rate, self._user_regularization,
@@ -158,28 +157,6 @@ class BPRMF(RecMixin, BaseRecommenderModel):
     @property
     def name(self):
         return "BPRMF" + f"_{self.get_base_params_shortcut()}" + f"_{self.get_params_shortcut()}"
-
-    # ---- recommendation side (BPRMF.py:93-105) ---------------------------------------------
-    def get_recommendations(self, k: int = 10):
-        recs_val, recs_test = self.process_protocol(k)
-        return dict(recs_val), dict(recs_test)
-
-    def get_recommendations_tensors(self, k: int = 10):
-        """(idx, val) device tensors, rows = private users, -1 / -inf padded."""
-        return self._model.topk(k, self._indptr, self._sorted_idx)
-
-    def get_single_recommendation(self, mask, k, *args):
-        if self._negative_sampling:
-            raise NotImplementedError("evaluation-time negative sampling masks (negative_sampling.py) are outside "
-                                      "this build's hot-path scope")
-        idx, val = self.get_recommendations_tensors(k)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
-        return out
 
     # ---- training (BPRMF.py:113-129) -------------------------------------------------------
     def train(self):

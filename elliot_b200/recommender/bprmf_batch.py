@@ -12,12 +12,12 @@ checked against the fp64 restatement in oracle/tf_models.py (parity unpinned, se
 import math
 import pickle
 
-import numpy as np
 import torch
 
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import TopKRecs, cuda_device
 
 
 class BPRMFBatchModel:
@@ -85,7 +85,7 @@ class BPRMFBatchModel:
             self.set_model_state(pickle.load(f))
 
 
-class BPRMF_batch(RecMixin, BaseRecommenderModel):
+class BPRMF_batch(TopKRecs, RecMixin, BaseRecommenderModel):
     r"""Batch BPR-MF (Adam).  YAML keys as in the reference (BPRMF_batch.py:37-48):
     `epochs, batch_size, factors, lr, l_w, l_b`."""
 
@@ -100,9 +100,7 @@ class BPRMF_batch(RecMixin, BaseRecommenderModel):
         self.autoset_params()
         if self._batch_size < 1:
             self._batch_size = self._data.transactions                 # BPRMF_batch.py:74-75
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.BPRMF_batch needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, "BPRMF_batch")
         self._indptr, self._set_idx, self._sorted_idx = train_csr_of(self._data, self._device)
         self._sampler = ops.MtSampler(self._num_users, self._num_items, self._indptr, self._set_idx, self._sorted_idx, seed=42)
         self._model = BPRMFBatchModel(self._factors, self._learning_rate, self._l_w, self._l_b, self._num_users,
@@ -125,20 +123,4 @@ class BPRMF_batch(RecMixin, BaseRecommenderModel):
             self.evaluate(it, loss / (it + 1))
 
     def get_recommendations(self, k: int = 100):
-        recs_val, recs_test = self.process_protocol(k)
-        return dict(recs_val), dict(recs_test)
-
-    def get_recommendations_tensors(self, k):
-        return self._model.topk(k, self._indptr, self._sorted_idx)
-
-    def get_single_recommendation(self, mask, k, *args):
-        if self._negative_sampling:
-            raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
-        idx, val = self.get_recommendations_tensors(k)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
-        return out
+        return super().get_recommendations(k)

@@ -25,6 +25,7 @@ from .. import ops
 from .._lib import EbError
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import TopKRecs, check_free, cuda_device, upload, upload_csr
 from .knn import SLAB_BYTES, _bound, dense_operand, frac_bits, gram_slabs
 
 
@@ -37,11 +38,10 @@ class EASEModel:
         m = data.sp_i_train_ratings.tocsr()
         if not m.has_sorted_indices:
             m = m.sorted_indices()
-        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(self.device, dt)
-        self.urm = (to(m.indptr, torch.int64), to(m.indices, torch.int32), to(m.data, torch.float32))
+        self.urm = upload_csr(m.indptr, m.indices, m.data, self.device)
         self.n_users, self.n_items = m.shape
         # ease_r.py:86: np.ediff1d(X.tocsc().indptr), the number of stored ratings per item
-        self.count = to(np.bincount(m.indices, minlength=self.n_items), torch.int32)
+        self.count = upload(np.bincount(m.indices, minlength=self.n_items), self.device, torch.int32)
         self.B = None
 
     def working_set(self):
@@ -57,11 +57,7 @@ class EASEModel:
 
     def initialize(self):
         n = self.n_items
-        need, what = self.working_set()
-        free = torch.cuda.mem_get_info(self.device)[0]
-        if need > free:
-            raise MemoryError(f"EASER needs {need / 2**30:.1f} GiB on {self.device} at its peak ({what}) and "
-                              f"{free / 2**30:.1f} GiB are free")
+        check_free("EASER", self.device, *self.working_set())
         X, s, _ = dense_operand(self.urm, self.n_users, n, "items", who="EASER needs")
         A = torch.empty((n, n), dtype=torch.float64, device=self.device)
         for j0, C in gram_slabs(X, self.n_users, n, "items"):
@@ -84,7 +80,7 @@ class EASEModel:
                                     user_begin=user_begin, n_sel=n_sel)
 
 
-class EASER(RecMixin, BaseRecommenderModel):
+class EASER(TopKRecs, RecMixin, BaseRecommenderModel):
     r"""Embarrassingly shallow autoencoders for sparse data (https://dl.acm.org/doi/abs/10.1145/3308558.3313710), on the
     H100.  YAML block as the reference's: EASER: {meta: {...}, neighborhood, l2_norm}; optional keys `b200_eval` and
     `b200_device`."""
@@ -101,34 +97,13 @@ class EASER(RecMixin, BaseRecommenderModel):
         if self._save_weights or self._restore:
             raise NotImplementedError("meta.save_weights / meta.restore are not supported for EASER: the reference "
                                       "pickles the dense prediction matrix, which this build never forms")
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.EASER needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, "EASER")
         self._model = EASEModel(self._data, self._l2_norm, self._device)
         self._indptr, _, self._sorted_idx = train_csr_of(self._data, self._device, set_order=False)
 
     @property
     def name(self):
         return f"EASER_{self.get_params_shortcut()}"
-
-    def get_recommendations(self, k: int = 10):
-        recs_val, recs_test = self.process_protocol(k)
-        return dict(recs_val), dict(recs_test)
-
-    def get_recommendations_tensors(self, k: int = 10):
-        return self._model.topk(k, self._indptr, self._sorted_idx)
-
-    def get_single_recommendation(self, mask, k, *args):
-        if self._negative_sampling:
-            raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
-        idx, val = self.get_recommendations_tensors(k)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
-        return out
 
     def train(self):
         start = time.time()

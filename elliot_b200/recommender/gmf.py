@@ -15,12 +15,12 @@ oracle/tf_models.py::gmf_forward_backward).  mf_factors is padded to the kernels
 import math
 import pickle
 
-import numpy as np
 import torch
 
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import cuda_device, recs_dict
 
 
 class GeneralizedMatrixFactorizationModel:
@@ -100,9 +100,7 @@ class GMF(RecMixin, BaseRecommenderModel):
         self.autoset_params()
         if self._batch_size < 1:
             self._batch_size = self._data.transactions
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.GMF needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, "GMF")
         self._indptr, _, self._sorted_idx = train_csr_of(self._data, self._device, set_order=False)
         self._filter = ops.bloom_build(self._indptr, self._sorted_idx, self._num_users)
         self._model = GeneralizedMatrixFactorizationModel(self._num_users, self._num_items, int(self._mf_factors),
@@ -130,13 +128,7 @@ class GMF(RecMixin, BaseRecommenderModel):
     def get_recommendations(self, k: int = 100):
         if self._negative_sampling:
             raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
-        idx, val = self._model.get_recs_topk(k, self._indptr, self._sorted_idx)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
+        out = recs_dict(self._data, *self._model.get_recs_topk(k, self._indptr, self._sorted_idx))
         return out, out
 
     def get_recommendations_tensors(self, k: int = 10):

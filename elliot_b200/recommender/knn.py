@@ -22,6 +22,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import TopKRecs, cuda_device, upload_csr
 
 SIMILARITIES = ("cosine", "dot")
 SLAB_BYTES = 2 << 30            # fp32 Gram rows computed per GEMM call
@@ -138,8 +139,7 @@ class KNNModel:
         m = (data.sp_i_train if implicit else data.sp_i_train_ratings).tocsr()
         if not m.has_sorted_indices:
             m = m.sorted_indices()
-        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(self.device, dt)
-        self.urm = (to(m.indptr, torch.int64), to(m.indices, torch.int32), to(m.data, torch.float32))
+        self.urm = upload_csr(m.indptr, m.indices, m.data, self.device)
         self.n_users, self.n_items = m.shape
         self.A = self.B = None
 
@@ -158,7 +158,7 @@ class KNNModel:
                                   user_begin=user_begin, n_sel=n_sel)
 
 
-class _KNN(RecMixin, BaseRecommenderModel):
+class _KNN(TopKRecs, RecMixin, BaseRecommenderModel):
     _over = None
 
     def _setup(self):
@@ -187,34 +187,13 @@ class _KNN(RecMixin, BaseRecommenderModel):
                 self._row_weights or self._shrink:
             self.logger.info("Options normalize, asymmetric_alpha, tversky_alpha, tversky_beta, row_weights are ignored "
                              "with standard implementation. Try with implementation: aiolli")
-        if not torch.cuda.is_available():
-            raise RuntimeError(f"elliot_b200.{type(self).__name__} needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, type(self).__name__)
         self._model = KNNModel(self._data, self._num_neighbors, self._similarity, self._implicit, self._over, self._device)
         self._indptr, _, self._sorted_idx = train_csr_of(self._data, self._device, set_order=False)
 
     @property
     def name(self):
         return f"{type(self).__name__}_{self.get_params_shortcut()}"
-
-    def get_recommendations(self, k: int = 10):
-        recs_val, recs_test = self.process_protocol(k)
-        return dict(recs_val), dict(recs_test)
-
-    def get_recommendations_tensors(self, k: int = 10):
-        return self._model.topk(k, self._indptr, self._sorted_idx)
-
-    def get_single_recommendation(self, mask, k, *args):
-        if self._negative_sampling:
-            raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
-        idx, val = self.get_recommendations_tensors(k)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
-        return out
 
     def train(self):
         start = time.time()

@@ -21,6 +21,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import TopKRecs, cuda_device, upload
 
 
 class RendleSampler:
@@ -67,11 +68,10 @@ class MF2020Model:
         F = self._factors
         dt = torch.float64 if self._mode == "exact" else torch.float32
         self.ld = F if self._mode == "exact" else ops.padded_dim(F)
-        to = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float64)).to(self.device, dt)
-        nu, ni = s["_user_factors"].shape[0], s["_item_factors"].shape[0]
-        self.U = torch.zeros((nu, self.ld), dtype=dt, device=self.device); self.U[:, :F] = to(s["_user_factors"])
-        self.V = torch.zeros((ni, self.ld), dtype=dt, device=self.device); self.V[:, :F] = to(s["_item_factors"])
-        self.ub, self.ib = to(s["_user_bias"]).contiguous(), to(s["_item_bias"]).contiguous()
+        U, V, self.ub, self.ib = (upload(np.asarray(s[key], np.float64), self.device, dt)
+                                  for key in ("_user_factors", "_item_factors", "_user_bias", "_item_bias"))
+        self.U = torch.zeros((U.shape[0], self.ld), dtype=dt, device=self.device); self.U[:, :F] = U
+        self.V = torch.zeros((V.shape[0], self.ld), dtype=dt, device=self.device); self.V[:, :F] = V
         self.gb = torch.tensor([float(s["_global_bias"])], dtype=dt, device=self.device)
 
     def get_model_state(self):
@@ -104,7 +104,7 @@ class MF2020Model:
             pickle.dump(self.get_model_state(), f)
 
 
-class MF2020(RecMixin, BaseRecommenderModel):
+class MF2020(TopKRecs, RecMixin, BaseRecommenderModel):
     r"""Matrix Factorization as in "NCF vs. MF Revisited" (https://dl.acm.org/doi/pdf/10.1145/3383313.3412488) on the H100.
 
     YAML block identical to the reference's (MF.py:41-52): MF2020: {meta: {...}, epochs, factors, lr, reg, m};
@@ -127,9 +127,7 @@ class MF2020(RecMixin, BaseRecommenderModel):
         self._hog_batch = int(getattr(self._params, "b200_batch", 1 << 20))   # samples per Hogwild launch
         if self._mode == "hogwild" and not hasattr(self._params, "b200_eval"):
             self._params.b200_eval = "device"
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.MF2020 needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, "MF2020")
         self._batch_size = 100000                                     # MF.py:68-69 (progress-bar granularity only)
         # MF.py:65-76: the sampler is built first, the model second; both seed the global streams with the model
         # seed and only the model draws before training, so one numpy stream (init, then negatives) serves both
@@ -145,25 +143,6 @@ class MF2020(RecMixin, BaseRecommenderModel):
     @property
     def name(self):
         return "MF2020" + f"_{self.get_base_params_shortcut()}" + f"_{self.get_params_shortcut()}"
-
-    def get_recommendations(self, k: int = 10):
-        recs_val, recs_test = self.process_protocol(k)
-        return dict(recs_val), dict(recs_test)
-
-    def get_recommendations_tensors(self, k: int = 10):
-        return self._model.topk(k, self._indptr, self._sorted_idx)
-
-    def get_single_recommendation(self, mask, k, *args):
-        if self._negative_sampling:
-            raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
-        idx, val = self.get_recommendations_tensors(k)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
-        return out
 
     def predict(self, u: int, i: int):
         """Score of a (public user, public item) pair (MF.py:96-103 / MF_model.py:60-62)."""

@@ -10,12 +10,12 @@ is UNPINNED (TF cannot run here): tests check the gradients against the fp64 res
 """
 import random
 
-import numpy as np
 import torch
 
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import cuda_device, recs_dict
 from .multi_vae import VariationalAutoEncoder, epoch_user_order
 
 
@@ -76,9 +76,7 @@ class MultiDAE(RecMixin, BaseRecommenderModel):
         ]
         self.autoset_params()
         self._dropout_rate = 1. - self._dropout_rate
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.MultiDAE needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, "MultiDAE")
         self._indptr, _, self._sorted_idx = train_csr_of(self._data, self._device, set_order=False)
         self._model = DenoisingAutoEncoder(self._num_items, int(self._intermediate_dim), int(self._latent_dim), self._learning_rate,
                                            self._dropout_rate, self._lambda, self._seed, self._indptr, self._sorted_idx, self._device)
@@ -101,13 +99,8 @@ class MultiDAE(RecMixin, BaseRecommenderModel):
         if self._negative_sampling:
             raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
         out = {}
-        items = np.array(self._data.items, dtype=object)
         for offset in range(0, self._num_users, self._batch_size):              # recommender_utils_mixin.py:63-73
             stop = min(offset + self._batch_size, self._num_users)
             rows = torch.arange(offset, stop, dtype=torch.int32, device=self._device)
-            idx, val = self._model.predict_topk(rows, k, self._indptr, self._sorted_idx)
-            idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-            for r, pu in enumerate(range(offset, stop)):
-                ok = idx[r] >= 0
-                out[self._data.users[pu]] = list(zip(items[idx[r][ok]].tolist(), val[r][ok].tolist()))
+            recs_dict(self._data, *self._model.predict_topk(rows, k, self._indptr, self._sorted_idx), first=offset, out=out)
         return out, out

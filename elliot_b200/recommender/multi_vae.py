@@ -15,12 +15,12 @@ import os
 import pickle
 import random
 
-import numpy as np
 import torch
 
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import cuda_device, recs_dict
 
 
 def _pad4(n):
@@ -222,13 +222,11 @@ class MultiVAE(RecMixin, BaseRecommenderModel):
         if self._batch_size < 1:
             self._batch_size = self._num_users
         self._dropout_rate = 1. - self._dropout_rate
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.MultiVAE needs a CUDA device (there is no CPU fallback)")
         # b200_dp: true (under torchrun) -> data parallel: replicated weights, every batch split across the ranks,
         # gradients averaged by one all-reduce per step (SURVEY.md §8e); each rank drives the GPU of its LOCAL_RANK
         self._dp = bool(getattr(self._params, "b200_dp", False))
         default_dev = f"cuda:{os.environ.get('LOCAL_RANK', '0')}" if self._dp else "cuda:0"
-        self._device = torch.device(getattr(self._params, "b200_device", default_dev))
+        self._device = cuda_device(self._params, "MultiVAE", default_dev)
         self._indptr, _, self._sorted_idx = train_csr_of(self._data, self._device, set_order=False)
         self._model = VariationalAutoEncoder(self._num_items, self._intermediate_dim, self._latent_dim, self._learning_rate,
                                              self._dropout_rate, self._lambda, self._seed, self._indptr, self._sorted_idx,
@@ -271,13 +269,8 @@ class MultiVAE(RecMixin, BaseRecommenderModel):
         if self._negative_sampling:
             raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
         out = {}
-        items = np.array(self._data.items, dtype=object)
         for offset in range(0, self._num_users, self._batch_size):              # recommender_utils_mixin.py:63-73
             stop = min(offset + self._batch_size, self._num_users)
             rows = torch.arange(offset, stop, dtype=torch.int32, device=self._device)
-            idx, val = self._model.predict_topk(rows, k, self._indptr, self._sorted_idx)
-            idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-            for r, pu in enumerate(range(offset, stop)):
-                ok = idx[r] >= 0
-                out[self._data.users[pu]] = list(zip(items[idx[r][ok]].tolist(), val[r][ok].tolist()))
+            recs_dict(self._data, *self._model.predict_topk(rows, k, self._indptr, self._sorted_idx), first=offset, out=out)
         return out, out

@@ -22,6 +22,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import cuda_device, recs_dict
 
 
 class ReferenceSampler:
@@ -179,9 +180,7 @@ class NeuMF(RecMixin, BaseRecommenderModel):
             self._batch_size = self._data.transactions
         if self._dropout or not (self._is_mf_train and self._is_mlp_train):
             raise NotImplementedError("elliot_b200.NeuMF covers the default configuration: dropout 0, both branches trained")
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.NeuMF needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, "NeuMF")
         self._indptr, _, self._sorted_idx = train_csr_of(self._data, self._device, set_order=False)
         self._model = NeuralMatrixFactorizationModel(self._num_users, self._num_items, self._mf_factors, self._learning_rate,
                                                      self._seed, self._device)
@@ -220,14 +219,9 @@ class NeuMF(RecMixin, BaseRecommenderModel):
         if self._negative_sampling:
             raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
         out = {}
-        items = np.array(self._data.items, dtype=object)
         f = self._mf_factors
         block = max(1, min(self._batch_size, (256 << 20) // max(1, self._num_items * 4 * f * 2)))   # <= 256 MB of layer-1 operand
         for u0 in range(0, self._num_users, block):
             u1 = min(u0 + block, self._num_users)
-            idx, val = self._model.get_recs_topk(u0, u1, k, self._indptr, self._sorted_idx)
-            idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-            for r, pu in enumerate(range(u0, u1)):
-                ok = idx[r] >= 0
-                out[self._data.users[pu]] = list(zip(items[idx[r][ok]].tolist(), val[r][ok].tolist()))
+            recs_dict(self._data, *self._model.get_recs_topk(u0, u1, k, self._indptr, self._sorted_idx), first=u0, out=out)
         return out, out

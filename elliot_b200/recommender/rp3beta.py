@@ -24,6 +24,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import TopKRecs, check_free, cuda_device, upload, upload_csr
 
 
 def l1_rows(indptr, data):
@@ -60,9 +61,7 @@ class RP3Model:
         self.alpha, self.beta, self.normalize = float(alpha), float(beta), bool(normalize_similarity)
         if self.R.nnz and float(self.R.data.min()) < 0:
             raise ValueError("RP3beta needs nonnegative ratings: its transition probabilities are ratings over row sums")
-        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(self.device, dt)
-        self._to = to
-        self.urm = (to(self.R.indptr, torch.int64), to(self.R.indices, torch.int32), to(self.R.data, torch.float32))
+        self.urm = upload_csr(self.R.indptr, self.R.indices, self.R.data, self.device)
         self.W = None
 
     def host_operands(self):
@@ -95,40 +94,40 @@ class RP3Model:
                                                  f"column prune {prune / g:.1f} GiB, the operands {operands / g:.1f} GiB")
 
     def initialize(self):
-        need, what = self.working_set(self.R.nnz)
-        free = torch.cuda.mem_get_info(self.device)[0]
-        if need > free:
-            raise MemoryError(f"RP3beta needs {need / 2**30:.1f} GiB on {self.device} at its peak ({what}) and "
-                              f"{free / 2**30:.1f} GiB are free")
-        (pp, pi, pv), (qp, qi, qv), degree = self.host_operands()
-        to = self._to
-        Pui = (to(pp, torch.int64), to(pi, torch.int32), to(pv, torch.float32))
-        Piu = (to(qp, torch.int64), to(qi, torch.int32), to(qv, torch.float32))
+        check_free("RP3beta", self.device, *self.working_set(self.R.nnz))
+        pui, piu, degree = self.host_operands()
+        Pui, Piu = upload_csr(*pui, self.device), upload_csr(*piu, self.device)
         # longest rows first: row i costs sum over its users of their rating counts
         work = np.bincount(self.R.indices, weights=np.diff(self.R.indptr)[np.repeat(np.arange(self.n_users),
                                                                                     np.diff(self.R.indptr))],
                            minlength=self.n_items)
-        order = to(np.argsort(-work, kind="stable"), torch.int32)
-        idx, val, cnt = ops.rp3_similarity(Piu, Pui, to(degree, torch.float64), self.k, order=order)
+        order = upload(np.argsort(-work, kind="stable"), self.device, torch.int32)
+        idx, val, cnt = ops.rp3_similarity(Piu, Pui, upload(degree, self.device, torch.float64), self.k, order=order)
         del Pui, Piu
         if self.normalize:
             ops.rp3_l1_rows(val, cnt)
         self.W = ops.rp3_prune_cols(idx, val, cnt, self.k)
 
     def topk(self, k, mask_indptr, mask_indices, users=None, user_begin=0, n_sel=None):
-        ap, ai, _ = self.urm
-        rows = users.long() if users is not None else \
-            torch.arange(user_begin, user_begin + (ap.numel() - 1 - user_begin if n_sel is None else n_sel), device=ap.device)
-        # longest rows first: row u costs the lengths of the W rows its ratings select
-        wl = torch.diff(self.W[0])
-        cs = torch.cat([torch.zeros(1, dtype=torch.int64, device=ap.device), torch.cumsum(wl[ai.long()], 0)])
-        work = cs[ap[rows + 1]] - cs[ap[rows]]
-        order = torch.argsort(work, descending=True, stable=True).to(torch.int32)
-        return ops.rp3_score_topk(self.urm, self.W, self.n_items, k, mask_indptr, mask_indices, users=users,
-                                  user_begin=user_begin, n_sel=n_sel, order=order)
+        return sparse_score_topk(self.urm, self.W, self.n_items, k, mask_indptr, mask_indices, users, user_begin, n_sel)
 
 
-class RP3beta(RecMixin, BaseRecommenderModel):
+def sparse_score_topk(urm, W, n_items, k, mask_indptr, mask_indices, users=None, user_begin=0, n_sel=None):
+    """The masked top k of urm . W (both CSRs on the device) in SciPy's float32 csr * csr order, the selected rows
+    visited longest first."""
+    ap, ai, _ = urm
+    rows = users.long() if users is not None else \
+        torch.arange(user_begin, user_begin + (ap.numel() - 1 - user_begin if n_sel is None else n_sel), device=ap.device)
+    # longest rows first: row u costs the lengths of the W rows its ratings select
+    wl = torch.diff(W[0])
+    cs = torch.cat([torch.zeros(1, dtype=torch.int64, device=ap.device), torch.cumsum(wl[ai.long()], 0)])
+    work = cs[ap[rows + 1]] - cs[ap[rows]]
+    order = torch.argsort(work, descending=True, stable=True).to(torch.int32)
+    return ops.rp3_score_topk(urm, W, n_items, k, mask_indptr, mask_indices, users=users, user_begin=user_begin,
+                              n_sel=n_sel, order=order)
+
+
+class RP3beta(TopKRecs, RecMixin, BaseRecommenderModel):
     r"""Updatable, accurate, diverse, and scalable recommendations for interactive applications
     (https://dl.acm.org/doi/10.1145/2955101), on the H100.  YAML block as the reference's: RP3beta: {meta: {...},
     neighborhood, alpha, beta, normalize_similarity}; optional keys `b200_eval` and `b200_device`."""
@@ -147,9 +146,7 @@ class RP3beta(RecMixin, BaseRecommenderModel):
         if self._save_weights or self._restore:
             raise NotImplementedError("meta.save_weights / meta.restore are not supported for RP3beta: the reference "
                                       "pickles the dense prediction matrix, which this build never forms")
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.RP3beta needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, "RP3beta")
         self._model = RP3Model(self._data, self._neighborhood, self._alpha, self._beta, self._normalize_similarity,
                                self._device)
         self._indptr, _, self._sorted_idx = train_csr_of(self._data, self._device, set_order=False)
@@ -157,25 +154,6 @@ class RP3beta(RecMixin, BaseRecommenderModel):
     @property
     def name(self):
         return f"RP3beta_{self.get_params_shortcut()}"
-
-    def get_recommendations(self, k: int = 10):
-        recs_val, recs_test = self.process_protocol(k)
-        return dict(recs_val), dict(recs_test)
-
-    def get_recommendations_tensors(self, k: int = 10):
-        return self._model.topk(k, self._indptr, self._sorted_idx)
-
-    def get_single_recommendation(self, mask, k, *args):
-        if self._negative_sampling:
-            raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
-        idx, val = self.get_recommendations_tensors(k)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
-        return out
 
     def train(self):
         start = time.time()

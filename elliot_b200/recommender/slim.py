@@ -23,6 +23,8 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
+from ._device import TopKRecs, check_free, cuda_device, upload_csr
+from .rp3beta import sparse_score_topk
 
 
 def seed_state(seed):
@@ -50,9 +52,7 @@ class SlimModel:
         # the ElasticNet's penalties, formed in double and passed to the float32 solver
         self.l1 = float(np.float32(self.alpha * self.l1_ratio * self.n_users))
         self.l2 = float(np.float32(self.alpha * (1.0 - self.l1_ratio) * self.n_users))
-        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(self.device, dt)
-        self._to = to
-        self.urm = (to(self.R.indptr, torch.int64), to(self.R.indices, torch.int32), to(self.R.data, torch.float32))
+        self.urm = upload_csr(self.R.indptr, self.R.indices, self.R.data, self.device)
         self.W = None
         self.coef_t = self.n_iter = self.gap = self.nnz = None
 
@@ -72,15 +72,10 @@ class SlimModel:
         shared = ops.slim_shared_residual_fits(self.n_users) if shared_residual is None else bool(shared_residual)
         cap = ops.slim_slots(self.n_users, shared)
         slots = cap if slots is None else max(1, min(int(slots), cap))
-        need, what = self.working_set(slots, shared)
-        free = torch.cuda.mem_get_info(self.device)[0]
-        if need > free:
-            raise MemoryError(f"SLIM needs {need / 2**30:.1f} GiB on {self.device} at its peak ({what}) and "
-                              f"{free / 2**30:.1f} GiB are free")
+        check_free("SLIM", self.device, *self.working_set(slots, shared))
         C = self.R.tocsc()
         C.sort_indices()
-        to = self._to
-        csc = (to(C.indptr, torch.int64), to(C.indices, torch.int32), to(C.data, torch.float32))
+        csc = upload_csr(C.indptr, C.indices, C.data, self.device)
         csr = (self.urm[0], self.urm[1])
         self.coef_t, self.n_iter, self.gap, self.nnz, drop = ops.slim_fit(
             csc, csr, self.n_users, self.n_items, self.l1, self.l2, seed_state(self.seed), self.k,
@@ -88,19 +83,10 @@ class SlimModel:
         self.W = ops.slim_weights(self.coef_t, drop, self.nnz, self.k)
 
     def topk(self, k, mask_indptr, mask_indices, users=None, user_begin=0, n_sel=None):
-        ap, ai, _ = self.urm
-        rows = users.long() if users is not None else \
-            torch.arange(user_begin, user_begin + (ap.numel() - 1 - user_begin if n_sel is None else n_sel), device=ap.device)
-        # longest rows first: row u costs the lengths of the W rows its ratings select
-        wl = torch.diff(self.W[0])
-        cs = torch.cat([torch.zeros(1, dtype=torch.int64, device=ap.device), torch.cumsum(wl[ai.long()], 0)])
-        work = cs[ap[rows + 1]] - cs[ap[rows]]
-        order = torch.argsort(work, descending=True, stable=True).to(torch.int32)
-        return ops.rp3_score_topk(self.urm, self.W, self.n_items, k, mask_indptr, mask_indices, users=users,
-                                  user_begin=user_begin, n_sel=n_sel, order=order)
+        return sparse_score_topk(self.urm, self.W, self.n_items, k, mask_indptr, mask_indices, users, user_begin, n_sel)
 
 
-class Slim(RecMixin, BaseRecommenderModel):
+class Slim(TopKRecs, RecMixin, BaseRecommenderModel):
     r"""Sparse Linear Methods (SLIM) item model, one elastic net per item
     (http://glaros.dtc.umn.edu/gkhome/fetch/papers/SLIM2011icdm.pdf), on the H100.  YAML block as the reference's:
     Slim: {meta: {...}, l1_ratio, alpha, neighborhood}; optional keys `b200_eval` and `b200_device`."""
@@ -116,34 +102,13 @@ class Slim(RecMixin, BaseRecommenderModel):
         if self._save_weights or self._restore:
             raise NotImplementedError("meta.save_weights / meta.restore are not supported for Slim: the reference's "
                                       "model state reads an `_A_tilde` it never sets")
-        if not torch.cuda.is_available():
-            raise RuntimeError("elliot_b200.Slim needs a CUDA device (there is no CPU fallback)")
-        self._device = torch.device(getattr(self._params, "b200_device", "cuda:0"))
+        self._device = cuda_device(self._params, "Slim")
         self._model = SlimModel(self._data, self._l1_ratio, self._alpha, self._neighborhood, self._seed, self._device)
         self._indptr, _, self._sorted_idx = train_csr_of(self._data, self._device, set_order=False)
 
     @property
     def name(self):
         return f"Slim_{self.get_base_params_shortcut()}_{self.get_params_shortcut()}"
-
-    def get_recommendations(self, k: int = 10):
-        recs_val, recs_test = self.process_protocol(k)
-        return dict(recs_val), dict(recs_test)
-
-    def get_recommendations_tensors(self, k: int = 10):
-        return self._model.topk(k, self._indptr, self._sorted_idx)
-
-    def get_single_recommendation(self, mask, k, *args):
-        if self._negative_sampling:
-            raise NotImplementedError("evaluation-time negative sampling masks are outside this build's hot-path scope")
-        idx, val = self.get_recommendations_tensors(k)
-        idx, val = idx.cpu().numpy(), val.cpu().numpy().astype(np.float64)
-        items = np.array(self._data.items, dtype=object)
-        out = {}
-        for pu, u in enumerate(self._data.users):
-            ok = idx[pu] >= 0
-            out[u] = list(zip(items[idx[pu][ok]].tolist(), val[pu][ok].tolist()))
-        return out
 
     def train(self):
         start = time.time()

@@ -40,36 +40,11 @@ def write_tsv(path, seed=SEED):
     return checksum(u, i, r)
 
 
-def hello_world_yaml(tsv, out_dir, extra="", model_extra=""):
-    """config_files/sample_hello_world.yml's ItemKNN block (neighbors 50, cosine, save_recs) over the C1 layout above."""
-    return f"""experiment:
-  dataset: c1_synth
-  data_config:
-    strategy: dataset
-    dataset_path: {tsv}
-  splitting:
-    test_splitting:
-      strategy: random_subsampling
-      test_ratio: 0.2
-  top_k: 10
-  evaluation:
-    simple_metrics: [nDCG, HR, Precision, Recall]
-  path_output_rec_result: {out_dir}/recs
-  path_output_rec_weight: {out_dir}/weights
-  path_output_rec_performance: {out_dir}/performance
-  path_log_folder: {out_dir}/log
-{extra}  models:
-    ItemKNN:
-      meta:
-        save_recs: True
-      neighbors: 50
-      similarity: cosine
-{model_extra}"""
-
-
-def als_yaml(tsv, out_dir, model_key, epochs, block, extra="", model_extra=""):
-    """An iALS or WRMF block (`block`: its parameter lines, e.g. factors / alpha / reg) with save_recs, over the C1
-    layout above."""
+def experiment_yaml(tsv, out_dir, model_key, block, meta=("save_recs: True",), extra="", model_extra=""):
+    """The reference's YAML layout (sample_hello_world.yml:1-19) over the C1 file above: one `model_key` block with the
+    given `meta` lines (without indentation) and parameter lines (`block`, indented, newline-ended).
+    `extra` goes into the experiment section, `model_extra` after the model's parameters."""
+    meta = "".join(f"        {m}\n" for m in meta)
     return f"""experiment:
   dataset: c1_synth
   data_config:
@@ -89,120 +64,43 @@ def als_yaml(tsv, out_dir, model_key, epochs, block, extra="", model_extra=""):
 {extra}  models:
     {model_key}:
       meta:
-        save_recs: True
-      epochs: {epochs}
-{block}{model_extra}"""
+{meta}{block}{model_extra}"""
+
+
+def hello_world_yaml(tsv, out_dir, extra="", model_extra=""):
+    """config_files/sample_hello_world.yml's ItemKNN block (neighbors 50, cosine, save_recs)."""
+    return experiment_yaml(tsv, out_dir, "ItemKNN", "      neighbors: 50\n      similarity: cosine\n", extra=extra,
+                           model_extra=model_extra)
+
+
+def als_yaml(tsv, out_dir, model_key, epochs, block, extra="", model_extra=""):
+    """An iALS or WRMF block (`block`: its parameter lines, e.g. factors / alpha / reg) with save_recs."""
+    return experiment_yaml(tsv, out_dir, model_key, f"      epochs: {epochs}\n{block}", extra=extra,
+                           model_extra=model_extra)
 
 
 def ease_yaml(tsv, out_dir, extra="", model_extra=""):
-    """An EASER block with the reference's defaults (neighborhood -1, l2_norm 1e3) and save_recs, over the C1 layout
-    above."""
-    return f"""experiment:
-  dataset: c1_synth
-  data_config:
-    strategy: dataset
-    dataset_path: {tsv}
-  splitting:
-    test_splitting:
-      strategy: random_subsampling
-      test_ratio: 0.2
-  top_k: 10
-  evaluation:
-    simple_metrics: [nDCG, HR, Precision, Recall]
-  path_output_rec_result: {out_dir}/recs
-  path_output_rec_weight: {out_dir}/weights
-  path_output_rec_performance: {out_dir}/performance
-  path_log_folder: {out_dir}/log
-{extra}  models:
-    EASER:
-      meta:
-        save_recs: True
-{model_extra}"""
+    """An EASER block with the reference's defaults (neighborhood -1, l2_norm 1e3) and save_recs."""
+    return experiment_yaml(tsv, out_dir, "EASER", "", extra=extra, model_extra=model_extra)
 
 
 def rp3beta_yaml(tsv, out_dir, extra="", model_extra=""):
     """config_files/recsys_config.yml's RP3beta block (neighborhood 546, alpha 1.0807, beta 0.7029, normalize_similarity
-    True) with save_recs, over the C1 layout above."""
-    return f"""experiment:
-  dataset: c1_synth
-  data_config:
-    strategy: dataset
-    dataset_path: {tsv}
-  splitting:
-    test_splitting:
-      strategy: random_subsampling
-      test_ratio: 0.2
-  top_k: 10
-  evaluation:
-    simple_metrics: [nDCG, HR, Precision, Recall]
-  path_output_rec_result: {out_dir}/recs
-  path_output_rec_weight: {out_dir}/weights
-  path_output_rec_performance: {out_dir}/performance
-  path_log_folder: {out_dir}/log
-{extra}  models:
-    RP3beta:
-      meta:
-        save_recs: True
-      neighborhood: 546
-      alpha: 1.0807
-      beta: 0.7029
-      normalize_similarity: True
-{model_extra}"""
+    True) with save_recs."""
+    return experiment_yaml(tsv, out_dir, "RP3beta", "      neighborhood: 546\n      alpha: 1.0807\n      beta: 0.7029\n"
+                           "      normalize_similarity: True\n", extra=extra, model_extra=model_extra)
 
 
 def slim_yaml(tsv, out_dir, extra="", model_extra=""):
-    """config_files/recsys_config.yml's Slim block (l1_ratio 0.0000119, alpha 0.0788, neighborhood 544) with save_recs,
-    over the C1 layout above."""
-    return f"""experiment:
-  dataset: c1_synth
-  data_config:
-    strategy: dataset
-    dataset_path: {tsv}
-  splitting:
-    test_splitting:
-      strategy: random_subsampling
-      test_ratio: 0.2
-  top_k: 10
-  evaluation:
-    simple_metrics: [nDCG, HR, Precision, Recall]
-  path_output_rec_result: {out_dir}/recs
-  path_output_rec_weight: {out_dir}/weights
-  path_output_rec_performance: {out_dir}/performance
-  path_log_folder: {out_dir}/log
-{extra}  models:
-    Slim:
-      meta:
-        save_recs: True
-      l1_ratio: 0.0000119
-      alpha: 0.0788
-      neighborhood: 544
-{model_extra}"""
+    """config_files/recsys_config.yml's Slim block (l1_ratio 0.0000119, alpha 0.0788, neighborhood 544) with
+    save_recs."""
+    return experiment_yaml(tsv, out_dir, "Slim", "      l1_ratio: 0.0000119\n      alpha: 0.0788\n      neighborhood: 544\n",
+                           extra=extra, model_extra=model_extra)
 
 
 def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra="", seed=42):
-    """The reference's YAML layout (sample_hello_world.yml:1-19 with a `BPRMF:` block, BPRMF.py:43-56 keys)."""
-    return f"""experiment:
-  dataset: c1_synth
-  data_config:
-    strategy: dataset
-    dataset_path: {tsv}
-  splitting:
-    test_splitting:
-      strategy: random_subsampling
-      test_ratio: 0.2
-  top_k: 10
-  evaluation:
-    simple_metrics: [nDCG, HR, Precision, Recall]
-  path_output_rec_result: {out_dir}/recs
-  path_output_rec_weight: {out_dir}/weights
-  path_output_rec_performance: {out_dir}/performance
-  path_log_folder: {out_dir}/log
-{extra}  models:
-    {model_key}:
-      meta:
-        save_recs: True
-        verbose: False
-      epochs: {epochs}
+    """A `BPRMF:` block with BPRMF.py:43-56 keys, the reference's default hyper-parameters, save_recs and verbose off."""
+    return experiment_yaml(tsv, out_dir, model_key, f"""      epochs: {epochs}
       factors: {factors}
       lr: 0.05
       bias_regularization: 0
@@ -210,4 +108,4 @@ def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra=""
       positive_item_regularization: 0.0025
       negative_item_regularization: 0.00025
       seed: {seed}
-{model_extra}"""
+""", meta=("save_recs: True", "verbose: False"), extra=extra, model_extra=model_extra)

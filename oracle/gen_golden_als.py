@@ -18,12 +18,9 @@ Every synthetic case is also checked against the fp64 restatement oracle/als.py 
     python oracle/gen_golden_als.py [--skip-c1]
 """
 import argparse
-import glob
-import importlib.util
+import importlib
 import os
-import shutil
 import sys
-import tempfile
 import time
 
 import numpy as np
@@ -35,7 +32,6 @@ from oracle import als as oals, ref_stubs  # noqa: E402
 from elliot_b200 import synth_c1  # noqa: E402
 
 GOLD = os.path.join(HERE, "..", "tests", "golden")
-METRICS = ["nDCG", "HR", "Precision", "Recall"]
 TOPK = 5
 EPOCHS = 3
 SEED = 42
@@ -59,13 +55,6 @@ def _scipy_dense_alias():
     `toarray()`, what it always was) so the unmodified reference runs on a current SciPy."""
     if not hasattr(sp.spmatrix, "A"):
         sp.spmatrix.A = property(lambda self: self.toarray())
-
-
-def _load(path, name):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 class _Data:
@@ -94,8 +83,8 @@ def _matrix(seed, U=70, I=50):
 
 def synthetic(ref_root):
     base = os.path.join(ref_root, "elliot/recommender/latent_factor_models")
-    mods = {"iALS": _load(os.path.join(base, "iALS/iALS_model.py"), "ref_ials_model"),
-            "WRMF": _load(os.path.join(base, "WRMF/wrmf_model.py"), "ref_wrmf_model")}
+    mods = {"iALS": ref_stubs.load(os.path.join(base, "iALS/iALS_model.py"), "ref_ials_model"),
+            "WRMF": ref_stubs.load(os.path.join(base, "WRMF/wrmf_model.py"), "ref_wrmf_model")}
     out = {"cases": np.array(list(CASES)), "topk": TOPK, "epochs": EPOCHS}
     for n, (name, (model, d, alpha, eps, reg, scaling)) in enumerate(CASES.items()):
         R = _matrix(100 + n)
@@ -139,58 +128,35 @@ def synthetic(ref_root):
     np.savez_compressed(os.path.join(GOLD, "als_cases.npz"), **out)
 
 
-def c1_runs(ref_root):
+def c1_runs():
     ref_stubs.install()
-    tmp = tempfile.mkdtemp(prefix="als_c1_golden_")
-    tsv = os.path.join(tmp, "dataset.tsv")
-    checksum = synth_c1.write_tsv(tsv)
-    logcfg = ref_stubs.write_logger_config(os.path.join(tmp, "logger_config.yml"))
-    from elliot.evaluation.evaluator import Evaluator
-    from elliot.run import run_experiment
-    orig_eval = Evaluator.eval
-    out = {"metrics": np.array(METRICS), "checksum": np.uint64(checksum)}
+    out = {"metrics": np.array(ref_stubs.METRICS)}
     for model, (epochs, block) in C1_BLOCKS.items():
-        got, steps = [], []
-
-        def recording_eval(self, recommendations):       # pass-through: records what the reference computed
-            res = orig_eval(self, recommendations)
-            k = list(res.keys())[0]
-            got.append([float(res[k]["test_results"][m]) for m in METRICS])
-            return res
-        Evaluator.eval = recording_eval
         mod = importlib.import_module("elliot.recommender.latent_factor_models.iALS.iALS_model" if model == "iALS" else
                                       "elliot.recommender.latent_factor_models.WRMF.wrmf_model")
         cls = mod.iALSModel if model == "iALS" else mod.WRMFModel
-        orig_step = cls.train_step
+        orig_step, steps = cls.train_step, []
 
         def timed_step(self):                              # pass-through: times the reference's own step
             t0 = time.time()
             orig_step(self)
             steps.append(time.time() - t0)
         cls.train_step = timed_step
-        run_dir = os.path.join(tmp, model)
-        os.makedirs(run_dir)
-        cfg = os.path.join(run_dir, "cfg.yml")
-        with open(cfg, "w") as fh:
-            fh.write(synth_c1.als_yaml(tsv, run_dir, model, epochs, block, extra=f"  path_logger_config: {logcfg}\n"))
-        t0 = time.time()
-        run_experiment(cfg)
-        dt = time.time() - t0
-        Evaluator.eval, cls.train_step = orig_eval, orig_step
-        rec_files = sorted(glob.glob(os.path.join(run_dir, "recs", "*.tsv")))
-        assert len(rec_files) == epochs, rec_files      # one file per evaluated epoch, `_it=<epoch>`
-        rec = np.loadtxt(rec_files[-1], delimiter="\t")
-        users = np.unique(rec[:, 0].astype(np.int64))
-        sel = np.isin(rec[:, 0].astype(np.int64), users[:400])
+        try:
+            got, recs, checksum, dt = ref_stubs.run_c1(
+                lambda tsv, d, extra: synth_c1.als_yaml(tsv, d, model, epochs, block, extra=extra))
+        finally:
+            cls.train_step = orig_step
+        assert len(recs) == epochs, list(recs)            # one file per evaluated epoch, `_it=<epoch>`
+        name, rec = list(recs.items())[-1]
         p = model.lower()
-        out.update({f"{p}_epochs": epochs, f"{p}_test_metrics": np.array(got), f"{p}_rec_file": os.path.basename(rec_files[-1]),
-                    f"{p}_rec_files": np.array([os.path.basename(f) for f in rec_files]),
-                    f"{p}_rec_users": rec[sel, 0].astype(np.int64), f"{p}_rec_items": rec[sel, 1].astype(np.int64),
-                    f"{p}_rec_scores": rec[sel, 2], f"{p}_n_rec_users": len(users), f"{p}_reference_seconds": dt,
+        out["checksum"] = np.uint64(checksum)
+        out.update({f"{p}_epochs": epochs, f"{p}_test_metrics": np.array(got), f"{p}_rec_file": name,
+                    f"{p}_rec_files": np.array(list(recs)), f"{p}_reference_seconds": dt,
                     f"{p}_reference_step_seconds": np.array(steps)})
-        print(f"{model} c1: per-epoch metrics {got}, train_step {steps} s, run {dt:.0f} s, {rec_files[-1]}", flush=True)
+        out.update({f"{p}_{k}": v for k, v in ref_stubs.first_users(rec).items()})
+        print(f"{model} c1: per-epoch metrics {got}, train_step {steps} s, run {dt:.0f} s, {name}", flush=True)
     np.savez_compressed(os.path.join(GOLD, "als_c1.npz"), **out)
-    shutil.rmtree(tmp, ignore_errors=True)
 
 
 def main():
@@ -200,7 +166,7 @@ def main():
     _scipy_dense_alias()
     synthetic(ref_stubs.REF)
     if not args.skip_c1:
-        c1_runs(ref_stubs.REF)
+        c1_runs()
 
 
 if __name__ == "__main__":

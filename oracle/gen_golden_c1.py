@@ -14,12 +14,8 @@ around Evaluator.eval records them — the reference only logs them), the recomm
     python oracle/gen_golden_c1.py [--epochs 10]
 """
 import argparse
-import glob
 import os
-import shutil
 import sys
-import tempfile
-import time
 
 import numpy as np
 
@@ -29,7 +25,6 @@ from oracle import ref_stubs  # noqa: E402
 from elliot_b200 import synth_c1  # noqa: E402
 
 OUT = os.path.join(HERE, "..", "tests", "golden", "bprmf_c1.npz")
-METRICS = ["nDCG", "HR", "Precision", "Recall"]
 
 
 def main():
@@ -37,43 +32,14 @@ def main():
     ap.add_argument("--epochs", type=int, default=10)
     ap.add_argument("--factors", type=int, default=64)
     args = ap.parse_args()
-    ref_stubs.install()
-    tmp = tempfile.mkdtemp(prefix="c1_golden_")
-    tsv = os.path.join(tmp, "dataset.tsv")
-    checksum = synth_c1.write_tsv(tsv)
-    logcfg = ref_stubs.write_logger_config(os.path.join(tmp, "logger_config.yml"))
-    cfg = os.path.join(tmp, "cfg.yml")
-    with open(cfg, "w") as fh:
-        fh.write(synth_c1.yaml_text(tsv, tmp, "BPRMF", args.epochs, args.factors, extra=f"  path_logger_config: {logcfg}\n"))
-
-    from elliot.evaluation.evaluator import Evaluator
-    per_epoch = []
-    orig_eval = Evaluator.eval
-
-    def recording_eval(self, recommendations):                      # pass-through: records what the reference computed
-        res = orig_eval(self, recommendations)
-        k = list(res.keys())[0]
-        per_epoch.append([float(res[k]["test_results"][m]) for m in METRICS])
-        print(f"epoch {len(per_epoch)}: " + " ".join(f"{m}={v:.6f}" for m, v in zip(METRICS, per_epoch[-1])), flush=True)
-        return res
-    Evaluator.eval = recording_eval
-    from elliot.run import run_experiment
-    t0 = time.time()
-    run_experiment(cfg)
-    dt = time.time() - t0
-    Evaluator.eval = orig_eval
-    rec_files = sorted(glob.glob(os.path.join(tmp, "recs", "*.tsv")))
-    assert rec_files, "the reference stored no recommendation file"
-    rec = np.loadtxt(rec_files[-1], delimiter="\t")
-    users, first = np.unique(rec[:, 0].astype(np.int64), return_index=True)
-    keep = 400                                                      # lists of the first 400 users (by public id)
-    sel = np.isin(rec[:, 0].astype(np.int64), users[:keep])
-    np.savez_compressed(OUT, metrics=np.array(METRICS), per_epoch=np.array(per_epoch), epochs=args.epochs, factors=args.factors,
-                        rec_users=rec[sel, 0].astype(np.int64), rec_items=rec[sel, 1].astype(np.int64), rec_scores=rec[sel, 2],
-                        rec_file=os.path.basename(rec_files[-1]), checksum=np.uint64(checksum), n_rec_users=len(users),
-                        reference_seconds=dt)
-    print(f"wrote {OUT}: {len(per_epoch)} epochs, {int(sel.sum())} rec rows, reference run {dt:.0f} s")
-    shutil.rmtree(tmp, ignore_errors=True)
+    per_epoch, recs, checksum, dt = ref_stubs.run_c1(
+        lambda tsv, d, extra: synth_c1.yaml_text(tsv, d, "BPRMF", args.epochs, args.factors, extra=extra))
+    assert recs, "the reference stored no recommendation file"
+    name, rec = list(recs.items())[-1]
+    kept = ref_stubs.first_users(rec)                               # lists of the first 400 users (by public id)
+    np.savez_compressed(OUT, metrics=np.array(ref_stubs.METRICS), per_epoch=np.array(per_epoch), epochs=args.epochs,
+                        factors=args.factors, rec_file=name, checksum=np.uint64(checksum), reference_seconds=dt, **kept)
+    print(f"wrote {OUT}: {len(per_epoch)} epochs, {len(kept['rec_users'])} rec rows, reference run {dt:.0f} s")
 
 
 if __name__ == "__main__":

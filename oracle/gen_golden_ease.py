@@ -20,14 +20,9 @@ and the top-k lists equal at every isolated rank.
     python oracle/gen_golden_ease.py [--skip-c1]
 """
 import argparse
-import glob
-import importlib.util
 import logging
 import os
-import shutil
 import sys
-import tempfile
-import time
 
 import numpy as np
 import scipy.sparse as sp
@@ -39,7 +34,6 @@ from oracle.knn import isolated  # noqa: E402
 from elliot_b200 import synth_c1  # noqa: E402
 
 GOLD = os.path.join(HERE, "..", "tests", "golden")
-METRICS = ["nDCG", "HR", "Precision", "Recall"]
 TOPK = 10
 # name: (users, items, rating kind, l2_norm, seed)
 CASES = {
@@ -51,13 +45,6 @@ CASES = {
     "half_l0.3": (60, 40, "half", 0.3, 6),
     "int_l0.3_tiny": (40, 25, "int", 0.3, 7),
 }
-
-
-def _load(path, name):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 class _Data:
@@ -110,7 +97,7 @@ def _reference_case(mod, R, l2_norm):
 
 def synthetic(ref_root):
     ref_stubs.install()
-    mod = _load(os.path.join(ref_root, "elliot/recommender/autoencoders/EASE_R/ease_r.py"), "ref_ease_r")
+    mod = ref_stubs.load(os.path.join(ref_root, "elliot/recommender/autoencoders/EASE_R/ease_r.py"), "ref_ease_r")
     out = {"cases": np.array(list(CASES)), "topk": TOPK}
     for name, (U, I, kind, lam, seed) in CASES.items():
         R = _matrix(U, I, kind, seed)
@@ -129,40 +116,13 @@ def synthetic(ref_root):
 
 
 def c1_run():
-    ref_stubs.install()
-    tmp = tempfile.mkdtemp(prefix="ease_c1_golden_")
-    tsv = os.path.join(tmp, "dataset.tsv")
-    checksum = synth_c1.write_tsv(tsv)
-    logcfg = ref_stubs.write_logger_config(os.path.join(tmp, "logger_config.yml"))
-    cfg = os.path.join(tmp, "cfg.yml")
-    with open(cfg, "w") as fh:
-        fh.write(synth_c1.ease_yaml(tsv, tmp, extra=f"  path_logger_config: {logcfg}\n"))
-    from elliot.evaluation.evaluator import Evaluator
-    got = []
-    orig_eval = Evaluator.eval
-
-    def recording_eval(self, recommendations):           # pass-through: records what the reference computed
-        res = orig_eval(self, recommendations)
-        k = list(res.keys())[0]
-        got.append([float(res[k]["test_results"][m]) for m in METRICS])
-        return res
-    Evaluator.eval = recording_eval
-    from elliot.run import run_experiment
-    t0 = time.time()
-    run_experiment(cfg)
-    dt = time.time() - t0
-    Evaluator.eval = orig_eval
-    rec_files = sorted(glob.glob(os.path.join(tmp, "recs", "*.tsv")))
-    assert len(rec_files) == 1, rec_files
-    rec = np.loadtxt(rec_files[0], delimiter="\t")
-    users = np.unique(rec[:, 0].astype(np.int64))
-    sel = np.isin(rec[:, 0].astype(np.int64), users[:400])
-    np.savez_compressed(os.path.join(GOLD, "ease_c1.npz"), metrics=np.array(METRICS), test_metrics=np.array(got[-1]),
-                        rec_users=rec[sel, 0].astype(np.int64), rec_items=rec[sel, 1].astype(np.int64), rec_scores=rec[sel, 2],
-                        rec_file=os.path.basename(rec_files[0]), checksum=np.uint64(checksum), n_rec_users=len(users),
-                        reference_seconds=dt)
-    print(f"ease_c1: metrics {dict(zip(METRICS, got[-1]))}, reference run {dt:.0f} s, {rec_files[0]}")
-    shutil.rmtree(tmp, ignore_errors=True)
+    got, recs, checksum, dt = ref_stubs.run_c1(synth_c1.ease_yaml)
+    assert len(recs) == 1, list(recs)
+    (name, rec), = recs.items()
+    np.savez_compressed(os.path.join(GOLD, "ease_c1.npz"), metrics=np.array(ref_stubs.METRICS),
+                        test_metrics=np.array(got[-1]), rec_file=name, checksum=np.uint64(checksum), reference_seconds=dt,
+                        **ref_stubs.first_users(rec))
+    print(f"ease_c1: metrics {dict(zip(ref_stubs.METRICS, got[-1]))}, reference run {dt:.0f} s, {name}")
 
 
 def main():

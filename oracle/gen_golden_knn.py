@@ -18,13 +18,8 @@ neighbour lists are within 1e-5 relative of the reference's.
     python oracle/gen_golden_knn.py [--skip-c1]
 """
 import argparse
-import glob
-import importlib.util
 import os
-import shutil
 import sys
-import tempfile
-import time
 
 import numpy as np
 import scipy.sparse as sp
@@ -35,15 +30,7 @@ from oracle import knn as oknn, ref_stubs  # noqa: E402
 from elliot_b200 import synth_c1  # noqa: E402
 
 GOLD = os.path.join(HERE, "..", "tests", "golden")
-METRICS = ["nDCG", "HR", "Precision", "Recall"]
 TOPK = 10
-
-
-def _load(path, name):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 class _Data:
@@ -117,8 +104,8 @@ def _reference_case(mod, R, over, k_nn, sim, implicit):
 
 
 def synthetic(ref_root):
-    mods = {"items": _load(os.path.join(ref_root, "elliot/recommender/knn/item_knn/item_knn_similarity.py"), "ref_item_knn"),
-            "users": _load(os.path.join(ref_root, "elliot/recommender/knn/user_knn/user_knn_similarity.py"), "ref_user_knn")}
+    mods = {"items": ref_stubs.load(os.path.join(ref_root, "elliot/recommender/knn/item_knn/item_knn_similarity.py"), "ref_item_knn"),
+            "users": ref_stubs.load(os.path.join(ref_root, "elliot/recommender/knn/user_knn/user_knn_similarity.py"), "ref_user_knn")}
     sizes = {"tiny": (12, 9, 3, False), "small": (150, 80, 10, True)}
     for over, model in (("items", "itemknn"), ("users", "userknn")):
         for size, (U, I, k_nn, dup) in sizes.items():
@@ -142,40 +129,13 @@ def synthetic(ref_root):
 
 
 def hello_world_c1():
-    ref_stubs.install()
-    tmp = tempfile.mkdtemp(prefix="knn_c1_golden_")
-    tsv = os.path.join(tmp, "dataset.tsv")
-    checksum = synth_c1.write_tsv(tsv)
-    logcfg = ref_stubs.write_logger_config(os.path.join(tmp, "logger_config.yml"))
-    cfg = os.path.join(tmp, "cfg.yml")
-    with open(cfg, "w") as fh:
-        fh.write(synth_c1.hello_world_yaml(tsv, tmp, extra=f"  path_logger_config: {logcfg}\n"))
-    from elliot.evaluation.evaluator import Evaluator
-    got = []
-    orig_eval = Evaluator.eval
-
-    def recording_eval(self, recommendations):           # pass-through: records what the reference computed
-        res = orig_eval(self, recommendations)
-        k = list(res.keys())[0]
-        got.append([float(res[k]["test_results"][m]) for m in METRICS])
-        return res
-    Evaluator.eval = recording_eval
-    from elliot.run import run_experiment
-    t0 = time.time()
-    run_experiment(cfg)
-    dt = time.time() - t0
-    Evaluator.eval = orig_eval
-    rec_files = sorted(glob.glob(os.path.join(tmp, "recs", "*.tsv")))
-    assert len(rec_files) == 1, rec_files
-    rec = np.loadtxt(rec_files[0], delimiter="\t")
-    users = np.unique(rec[:, 0].astype(np.int64))
-    sel = np.isin(rec[:, 0].astype(np.int64), users[:400])
-    np.savez_compressed(os.path.join(GOLD, "itemknn_c1.npz"), metrics=np.array(METRICS), test_metrics=np.array(got[-1]),
-                        rec_users=rec[sel, 0].astype(np.int64), rec_items=rec[sel, 1].astype(np.int64), rec_scores=rec[sel, 2],
-                        rec_file=os.path.basename(rec_files[0]), checksum=np.uint64(checksum), n_rec_users=len(users),
-                        reference_seconds=dt)
-    print(f"itemknn_c1: metrics {dict(zip(METRICS, got[-1]))}, reference run {dt:.0f} s, {rec_files[0]}")
-    shutil.rmtree(tmp, ignore_errors=True)
+    got, recs, checksum, dt = ref_stubs.run_c1(synth_c1.hello_world_yaml)
+    assert len(recs) == 1, list(recs)
+    (name, rec), = recs.items()
+    np.savez_compressed(os.path.join(GOLD, "itemknn_c1.npz"), metrics=np.array(ref_stubs.METRICS),
+                        test_metrics=np.array(got[-1]), rec_file=name, checksum=np.uint64(checksum), reference_seconds=dt,
+                        **ref_stubs.first_users(rec))
+    print(f"itemknn_c1: metrics {dict(zip(ref_stubs.METRICS, got[-1]))}, reference run {dt:.0f} s, {name}")
 
 
 def main():

@@ -22,14 +22,9 @@ Every synthetic case is also checked against oracle/rp3beta.py here (the same ch
     python oracle/gen_golden_rp3beta.py [--skip-c1]
 """
 import argparse
-import glob
-import importlib.util
 import logging
 import os
-import shutil
 import sys
-import tempfile
-import time
 
 import numpy as np
 import scipy.sparse as sp
@@ -41,7 +36,6 @@ from oracle.rp3beta import preds_digest  # noqa: E402
 from elliot_b200 import synth_c1  # noqa: E402
 
 GOLD = os.path.join(HERE, "..", "tests", "golden")
-METRICS = ["nDCG", "HR", "Precision", "Recall"]
 TOPK = 10
 # name: (users, items, rating kind, alpha, beta, normalize_similarity, neighborhood, seed)
 CASES = {
@@ -54,13 +48,6 @@ CASES = {
     "int_a0.5_b0_norm_nb400": (60, 40, "int", 0.5, 0.0, True, 400, 7),
     "implicit_a1_b0_nb10": (80, 60, "implicit", 1.0, 0.0, False, 10, 8),
 }
-
-
-def _load(path, name):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 class _Data:
@@ -138,7 +125,7 @@ def reference_case(mod, R, alpha, beta, normalize, nbh):
 def synthetic(ref_root):
     from oracle.rp3beta import check_case
     ref_stubs.install()
-    mod = _load(os.path.join(ref_root, "elliot/recommender/graph_based/RP3beta/rp3beta.py"), "ref_rp3beta")
+    mod = ref_stubs.load(os.path.join(ref_root, "elliot/recommender/graph_based/RP3beta/rp3beta.py"), "ref_rp3beta")
     out = {"cases": np.array(list(CASES)), "topk": TOPK}
     for name, (U, I, kind, alpha, beta, norm, nbh, seed) in CASES.items():
         R = matrix(U, I, kind, seed)
@@ -151,40 +138,13 @@ def synthetic(ref_root):
 
 
 def c1_run():
-    ref_stubs.install()
-    tmp = tempfile.mkdtemp(prefix="rp3beta_c1_golden_")
-    tsv = os.path.join(tmp, "dataset.tsv")
-    checksum = synth_c1.write_tsv(tsv)
-    logcfg = ref_stubs.write_logger_config(os.path.join(tmp, "logger_config.yml"))
-    cfg = os.path.join(tmp, "cfg.yml")
-    with open(cfg, "w") as fh:
-        fh.write(synth_c1.rp3beta_yaml(tsv, tmp, extra=f"  path_logger_config: {logcfg}\n"))
-    from elliot.evaluation.evaluator import Evaluator
-    got = []
-    orig_eval = Evaluator.eval
-
-    def recording_eval(self, recommendations):           # pass-through: records what the reference computed
-        res = orig_eval(self, recommendations)
-        k = list(res.keys())[0]
-        got.append([float(res[k]["test_results"][m]) for m in METRICS])
-        return res
-    Evaluator.eval = recording_eval
-    from elliot.run import run_experiment
-    t0 = time.time()
-    run_experiment(cfg)
-    dt = time.time() - t0
-    Evaluator.eval = orig_eval
-    rec_files = sorted(glob.glob(os.path.join(tmp, "recs", "*.tsv")))
-    assert len(rec_files) == 1, rec_files
-    rec = np.loadtxt(rec_files[0], delimiter="\t")
-    users = np.unique(rec[:, 0].astype(np.int64))
-    sel = np.isin(rec[:, 0].astype(np.int64), users[:400])
-    np.savez_compressed(os.path.join(GOLD, "rp3beta_c1.npz"), metrics=np.array(METRICS), test_metrics=np.array(got[-1]),
-                        rec_users=rec[sel, 0].astype(np.int64), rec_items=rec[sel, 1].astype(np.int64), rec_scores=rec[sel, 2],
-                        rec_file=os.path.basename(rec_files[0]), checksum=np.uint64(checksum), n_rec_users=len(users),
-                        reference_seconds=dt)
-    print(f"rp3beta_c1: metrics {dict(zip(METRICS, got[-1]))}, reference run {dt:.0f} s, {rec_files[0]}")
-    shutil.rmtree(tmp, ignore_errors=True)
+    got, recs, checksum, dt = ref_stubs.run_c1(synth_c1.rp3beta_yaml)
+    assert len(recs) == 1, list(recs)
+    (name, rec), = recs.items()
+    np.savez_compressed(os.path.join(GOLD, "rp3beta_c1.npz"), metrics=np.array(ref_stubs.METRICS),
+                        test_metrics=np.array(got[-1]), rec_file=name, checksum=np.uint64(checksum), reference_seconds=dt,
+                        **ref_stubs.first_users(rec))
+    print(f"rp3beta_c1: metrics {dict(zip(ref_stubs.METRICS, got[-1]))}, reference run {dt:.0f} s, {name}")
 
 
 def main():

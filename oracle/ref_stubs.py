@@ -8,16 +8,25 @@ attribute is a subclassable, callable dummy) and puts the original project (REF)
 or modified; code paths that would really call TensorFlow/hyperopt (the TF models, hyper-parameter search) stay out of
 reach and are never used by the generators/tests that call this.
 
+`run_c1()` runs the reference's `run_experiment` on the C1 synthetic file and returns what the goldens record.
+
 Also provides a logging config equivalent to elliot/config/logger_config.yml without its `queue: cfg://objects.queue`
 handler, which Python >= 3.12's logging.config rejects (the reference targets Python 3.6-3.8); the reference reads it
 through its own `path_logger_config` key.
 """
 import abc
+import glob
 import importlib.abc
 import importlib.machinery
+import importlib.util
 import os
+import shutil
 import sys
+import tempfile
+import time
 import types
+
+import numpy as np
 
 # a checkout of the original Elliot project: $ELLIOT_REFERENCE, or a directory named `reference` beside this repository
 REF = os.environ.get("ELLIOT_REFERENCE") or os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "reference")
@@ -94,3 +103,63 @@ def write_logger_config(path):
     with open(path, "w") as fh:
         fh.write(body)
     return path
+
+
+METRICS = ["nDCG", "HR", "Precision", "Recall"]
+
+
+def load(path, name):
+    """Import one reference file by its path, as module `name`."""
+    spec = importlib.util.spec_from_file_location(name, path)
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+def run_c1(make_yaml):
+    """elliot.run.run_experiment on `make_yaml(tsv, out_dir, extra=...)` over the C1 synthetic file of
+    elliot_b200/synth_c1.py, in a temporary directory.  Returns (the test METRICS of every evaluation in order, {rec file
+    name: its rows} sorted by name, the file's checksum, the wall time of the run).  A pass-through wrapper around
+    Evaluator.eval records the metrics, which the reference only logs."""
+    from elliot_b200 import synth_c1
+    install()
+    tmp = tempfile.mkdtemp(prefix="c1_golden_")
+    try:
+        tsv = os.path.join(tmp, "dataset.tsv")
+        checksum = synth_c1.write_tsv(tsv)
+        logcfg = write_logger_config(os.path.join(tmp, "logger_config.yml"))
+        cfg = os.path.join(tmp, "cfg.yml")
+        with open(cfg, "w") as fh:
+            fh.write(make_yaml(tsv, tmp, extra=f"  path_logger_config: {logcfg}\n"))
+        from elliot.evaluation.evaluator import Evaluator
+        from elliot.run import run_experiment
+        evals = []
+        orig_eval = Evaluator.eval
+
+        def recording_eval(self, recommendations):       # pass-through: records what the reference computed
+            res = orig_eval(self, recommendations)
+            k = list(res.keys())[0]
+            evals.append([float(res[k]["test_results"][m]) for m in METRICS])
+            print(f"evaluation {len(evals)}: " + " ".join(f"{m}={v:.6f}" for m, v in zip(METRICS, evals[-1])), flush=True)
+            return res
+        Evaluator.eval = recording_eval
+        try:
+            t0 = time.time()
+            run_experiment(cfg)
+            dt = time.time() - t0
+        finally:
+            Evaluator.eval = orig_eval
+        recs = {os.path.basename(f): np.loadtxt(f, delimiter="\t")
+                for f in sorted(glob.glob(os.path.join(tmp, "recs", "*.tsv")))}
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+    return evals, recs, checksum, dt
+
+
+def first_users(rec, keep=400):
+    """The rows of the first `keep` users (by public id) of a rec file: rec_users, rec_items, rec_scores, and
+    n_rec_users, the number of users in the file."""
+    users = np.unique(rec[:, 0].astype(np.int64))
+    sel = np.isin(rec[:, 0].astype(np.int64), users[:keep])
+    return {"rec_users": rec[sel, 0].astype(np.int64), "rec_items": rec[sel, 1].astype(np.int64),
+            "rec_scores": rec[sel, 2], "n_rec_users": len(users)}

@@ -7,17 +7,12 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+import c1_harness as c1h
+from c1_harness import DEV, GOLD, to_dev
 from elliot_b200 import ops
 from elliot_b200._lib import EbError
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-
-
-def _t(a, dt=None):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
 
 
 # ---------------------------------------------------------------- 1. Gram
@@ -27,7 +22,7 @@ def test_gram_matches_numpy_and_reruns_bit_identical(n, d):
     g = np.random.default_rng(n * 1000 + d)
     ld = d + 3
     Y = g.standard_normal((n, ld))
-    Yd = _t(Y)
+    Yd = to_dev(Y)
     G1 = ops.gram_f64(Yd, d).cpu().numpy()
     G2 = ops.gram_f64(Yd.clone(), d).cpu().numpy()
     want = Y[:, :d].T @ Y[:, :d]
@@ -76,7 +71,7 @@ def _gpu_solve(Y, G, indptr, indices, w, c, reg, order, ld_x=None):
     d = Y.shape[1]
     ld_x = ld_x or d
     X = torch.full((len(indptr) - 1, ld_x), 7.0, dtype=torch.float64, device=DEV)
-    ops.als_solve_f64(_t(G), _t(Y), d, _t(indptr), _t(indices), _t(w), _t(c), _t(order.astype(np.int32)), reg, X)
+    ops.als_solve_f64(to_dev(G), to_dev(Y), d, to_dev(indptr), to_dev(indices), to_dev(w), to_dev(c), to_dev(order.astype(np.int32)), reg, X)
     return X.cpu().numpy()
 
 
@@ -188,7 +183,7 @@ def test_model_matches_reference_every_epoch(name):
     print(f"\n{name}: tables within {worst:.2e} (max abs diff / max abs value) of the reference over every epoch")
     mask = sp.csr_matrix(R != 0)
     mask.sort_indices()
-    idx, val = m.topk(int(g["topk"]), _t(mask.indptr, torch.int64), _t(mask.indices, torch.int32))
+    idx, val = m.topk(int(g["topk"]), to_dev(mask.indptr, torch.int64), to_dev(mask.indices, torch.int32))
     assert np.array_equal(idx.cpu().numpy(), g[f"{name}_topk_idx"]), name
     tv = g[f"{name}_topk_val"]
     assert np.abs(val.cpu().numpy() - tv).max() <= GOLDEN_TOL * np.abs(tv).max()
@@ -218,14 +213,7 @@ def test_negative_alpha_is_refused_with_its_name():
 
 
 # ---------------------------------------------------------------- 4. run_experiment at C1 scale
-@pytest.fixture(scope="module")
-def c1(tmp_path_factory):
-    from elliot_b200 import synth_c1
-    g = dict(np.load(os.path.join(GOLD, "als_c1.npz")))
-    d = tmp_path_factory.mktemp("als_c1")
-    tsv = str(d / "dataset.tsv")
-    assert synth_c1.write_tsv(tsv) == int(g["checksum"]), "this numpy draws a different synthetic file than the golden's"
-    return g, d, tsv
+c1 = c1h.c1_fixture("als_c1.npz")
 
 
 BLOCKS = {
@@ -234,32 +222,20 @@ BLOCKS = {
 }
 
 
-def _run(d, tsv, model, epochs, tag, model_extra=""):
-    from elliot_b200 import run_experiment, synth_c1
-    out = d / f"{model}_{tag}"
-    os.makedirs(out, exist_ok=True)
-    txt = synth_c1.als_yaml(tsv, str(out), model, epochs, BLOCKS[model], model_extra=model_extra)
-    if tag == "device":                      # metrics straight from the top-k tensor: no rec dicts, no rec files
-        txt = txt.replace("save_recs: True", "save_recs: False")
-    (out / "cfg.yml").write_text(txt)
-    return run_experiment(str(out / "cfg.yml"))[0], out
-
-
 @pytest.mark.parametrize("ev", ["host", "device"])
 @pytest.mark.parametrize("model", ["iALS", "WRMF"])
 def test_run_experiment_matches_the_reference_run(c1, model, ev):
+    from elliot_b200 import synth_c1
     g, d, tsv = c1
     p = model.lower()
     epochs = int(g[f"{p}_epochs"])
-    res, out = _run(d, tsv, model, epochs, ev, model_extra=f"      b200_eval: {ev}\n")
-    want = g[f"{p}_test_metrics"]
-    assert len(res["history"]) == epochs == len(want)
-    for e in range(epochs):
-        for j, m in enumerate(g["metrics"].tolist()):
-            got = res["history"][e][10][m]
-            assert abs(got - want[e][j]) <= 1e-4, (model, ev, e, m, got, want[e][j])
+    out = d / f"{model}_{ev}"
+    res = c1h.run(out, synth_c1.als_yaml(tsv, str(out), model, epochs, BLOCKS[model], model_extra=f"      b200_eval: {ev}\n"),
+                  ev == "device")
+    assert len(res["history"]) == epochs
+    c1h.assert_metrics(res, g["metrics"].tolist(), g[f"{p}_test_metrics"], model, ev)
     if ev == "device":
-        assert not os.path.exists(out / "recs") or not os.listdir(out / "recs")
+        c1h.assert_no_rec_files(out)
         return
     files = sorted(os.listdir(out / "recs"))
     assert files == g[f"{p}_rec_files"].tolist(), (files, g[f"{p}_rec_files"])      # same model `name` as the reference's

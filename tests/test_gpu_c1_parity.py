@@ -16,31 +16,21 @@ import os
 import numpy as np
 import pytest
 
+import c1_harness as c1h
 from elliot_b200 import synth_c1
 
 pytestmark = pytest.mark.gpu
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "bprmf_c1.npz")
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HOGWILD_TOL = 0.005          # |mean_seeds nDCG@10(hogwild) - nDCG@10(reference)|, absolute (H100: 0.0006; single seeds <= 0.0031)
 OUT = {}
 
 
-@pytest.fixture(scope="module")
-def c1(tmp_path_factory):
-    g = dict(np.load(GOLDEN))
-    d = tmp_path_factory.mktemp("c1")
-    tsv = str(d / "dataset.tsv")
-    assert synth_c1.write_tsv(tsv) == int(g["checksum"]), "this numpy draws a different synthetic file than the golden's"
-    return g, d, tsv
+c1 = c1h.c1_fixture("bprmf_c1.npz")
 
 
 def _run(d, tsv, g, tag, model_extra="", seed=42):
-    from elliot_b200 import run_experiment
     out = d / tag
-    os.makedirs(out, exist_ok=True)
-    cfg = out / "cfg.yml"
-    cfg.write_text(synth_c1.yaml_text(tsv, str(out), "BPRMF", int(g["epochs"]), int(g["factors"]), model_extra=model_extra, seed=seed))
-    return run_experiment(str(cfg))[0], out
+    text = synth_c1.yaml_text(tsv, str(out), "BPRMF", int(g["epochs"]), int(g["factors"]), model_extra=model_extra, seed=seed)
+    return c1h.run(out, text), out
 
 
 def _dump():
@@ -63,7 +53,7 @@ def test_c1_exact_mode_reproduces_the_reference_run(c1):
     OUT["exact"] = {"max_abs_metric_diff_over_epochs": worst, "ndcg_per_epoch": [r[10]["nDCG"] for r in hist],
                     "reference_ndcg_per_epoch": g["per_epoch"][:, 0].tolist()}
     _dump()
-    assert worst <= 1e-4, worst                                  # north_star tolerance
+    c1h.assert_metrics(res, names, g["per_epoch"])               # north_star tolerance
     assert worst <= 1e-9, worst                                  # what exact mode actually delivers
     # the recommendation file of the same epoch as the golden's, item for item
     suffix = str(g["rec_file"]).rsplit("_it=", 1)[1]

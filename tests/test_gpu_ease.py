@@ -8,6 +8,8 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+import c1_harness as c1h
+from c1_harness import DEV, GOLD, dev_csr, to_dev
 from elliot_b200 import ops
 from elliot_b200._lib import EbError
 from elliot_b200.recommender import knn
@@ -15,15 +17,8 @@ from oracle import ease as oease
 from oracle.knn import isolated, topk as oracle_topk
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
 EPS = np.finfo(np.float64).eps
 RESIDUAL_C = 1.0       # max |A P - I| <= RESIDUAL_C * n * eps * ||A||_inf * ||P||_inf
-
-
-def _t(a, dt=None):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
 
 
 def _matrix(kind, n, seed):
@@ -41,7 +36,7 @@ def _gpu_inverse(A, ld=None):
     n = A.shape[0]
     ld = ld or n
     T = torch.full((n, ld), 7.0, dtype=torch.float64, device=DEV)
-    T[:, :n] = _t(A)
+    T[:, :n] = to_dev(A)
     ops.inverse_f64(T, n)
     out = T.cpu().numpy()
     assert np.all(out[:, n:] == 7.0), "padding columns must stay untouched"
@@ -123,7 +118,7 @@ def test_normal_matrix_rows_from_slabs():
     slab = (g.integers(-300, 300, (S, n + 5)) * 4).astype(np.float32)
     count = g.integers(0, 50, n).astype(np.int32)
     A = torch.full((n, n + 2), 9.0, dtype=torch.float64, device=DEV)
-    ops.ease_normal_f64(_t(slab)[:, :n + 5], row0, _t(count), 0.3, 0.25, A)
+    ops.ease_normal_f64(to_dev(slab)[:, :n + 5], row0, to_dev(count), 0.3, 0.25, A)
     got = A.cpu().numpy()
     want = slab[:, :n].astype(np.float64) * 0.25
     for r in range(S):
@@ -136,23 +131,17 @@ def test_weights_bit_equal_to_numpy():
     g = np.random.default_rng(4)
     n = 333
     P = g.standard_normal((n, n)) * 10.0 ** g.integers(-3, 3, (n, n))
-    B = ops.ease_weights_f32(_t(P)).cpu().numpy()
+    B = ops.ease_weights_f32(to_dev(P)).cpu().numpy()
     want = (-P / np.diag(P)[None, :]).astype(np.float32)
     want[np.diag_indices(n)] = 0.0
     assert np.array_equal(B.view(np.int32), want.view(np.int32))
     P[40, 40] = 0.0
     P[7, 7] = 0.0
     with pytest.raises(EbError, match="column 7:"):
-        ops.ease_weights_f32(_t(P))
+        ops.ease_weights_f32(to_dev(P))
 
 
 # ---------------------------------------------------------------- 3. dense scorer
-def _dev_csr(M):
-    M = sp.csr_matrix(M, dtype=np.float32)
-    M.sort_indices()
-    return _t(M.indptr, torch.int64), _t(M.indices, torch.int32), _t(M.data, torch.float32)
-
-
 def _score_case(n_rows, n_mid, n_cols, seed):
     g = np.random.default_rng(seed)
     A = sp.random(n_rows, n_mid, density=0.08, random_state=seed, format="csr")
@@ -176,19 +165,19 @@ def test_dense_scorer_bit_equal_to_sparse(n_cols, k, select):
     T = ops.knn_score_tile_cols()
     n_cols = T + 77 if n_cols == "tile+77" else n_cols
     A, B, mask = _score_case(96, 70, n_cols, 13 + k)
-    dA, dM = _dev_csr(A), _dev_csr(mask)
+    dA, dM = dev_csr(A), dev_csr(mask)
     Bcsr = sp.csr_matrix(B)
     Bcsr.sort_indices()
-    dBs = _dev_csr(Bcsr)
+    dBs = dev_csr(Bcsr)
     ldb = n_cols + 5
     dB = torch.zeros((70, ldb), dtype=torch.float32, device=DEV)
-    dB[:, :n_cols] = _t(B)
+    dB[:, :n_cols] = to_dev(B)
     f = knn.frac_bits(knn._bound(dA, dBs))
     kw = {}
     rows = np.arange(96)
     if select == "users":
         rows = np.array([95, 3, 5, 40, 40, 0], np.int32)
-        kw = {"users": _t(rows)}
+        kw = {"users": to_dev(rows)}
     elif select == "begin":
         rows = np.arange(17, 96)
         kw = {"user_begin": 17, "n_sel": len(rows)}
@@ -237,7 +226,7 @@ def test_model_matches_reference_goldens(name):
     B_or = oease.weights(np.linalg.inv(oease.normal_matrix(R, lam)))
     # both round an fp64 quotient to fp32 once; the two fp64 inverses differ in the last bits only, so at most 1 ulp apart
     assert np.all(np.abs(m.B.cpu().numpy() - B_or) <= np.spacing(np.abs(B_or))), name
-    mask = _dev_csr(R != 0)
+    mask = dev_csr(R != 0)
     ti, tv = m.topk(k, mask[0], mask[1])
     gi, gv = ti.cpu().numpy(), tv.cpu().numpy().astype(np.float64)
     ri, rv = g[f"{name}_topk_idx"], g[f"{name}_topk_val"]
@@ -280,32 +269,18 @@ def test_ratings_without_an_exact_scale_are_refused():
 
 
 # ---------------------------------------------------------------- 5. run_experiment at C1 scale
-@pytest.fixture(scope="module")
-def c1(tmp_path_factory):
-    from elliot_b200 import synth_c1
-    g = dict(np.load(os.path.join(GOLD, "ease_c1.npz")))
-    d = tmp_path_factory.mktemp("ease_c1")
-    tsv = str(d / "dataset.tsv")
-    assert synth_c1.write_tsv(tsv) == int(g["checksum"]), "this numpy draws a different synthetic file than the golden's"
-    return g, d, tsv
+c1 = c1h.c1_fixture("ease_c1.npz")
 
 
 @pytest.mark.parametrize("ev", ["host", "device"])
 def test_run_experiment_matches_the_reference_run(c1, ev):
-    from elliot_b200 import run_experiment, synth_c1
+    from elliot_b200 import synth_c1
     g, d, tsv = c1
     out = d / ev
-    os.makedirs(out, exist_ok=True)
-    txt = synth_c1.ease_yaml(tsv, str(out), model_extra=f"      b200_eval: {ev}\n")
-    if ev == "device":                      # metrics straight from the top-k tensor: no rec dicts, no rec files
-        txt = txt.replace("save_recs: True", "save_recs: False")
-    (out / "cfg.yml").write_text(txt)
-    res = run_experiment(str(out / "cfg.yml"))[0]
-    for m, want in zip(g["metrics"].tolist(), g["test_metrics"]):
-        got = res["test_results"][10][m]
-        assert abs(got - float(want)) <= 1e-4, (ev, m, got, float(want))
+    res = c1h.run(out, synth_c1.ease_yaml(tsv, str(out), model_extra=f"      b200_eval: {ev}\n"), ev == "device")
+    c1h.assert_metrics(res, g["metrics"].tolist(), g["test_metrics"], ev)
     if ev == "device":
-        assert not os.path.exists(out / "recs") or not os.listdir(out / "recs")
+        c1h.assert_no_rec_files(out)
         return
     files = os.listdir(out / "recs")
     assert files == [str(g["rec_file"])], (files, str(g["rec_file"]))          # the same model `name` as the reference's

@@ -10,22 +10,15 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+import c1_harness as c1h
+from c1_harness import DEV, GOLD, dev_csr
 from elliot_b200 import ops, synth_c1
 from elliot_b200.recommender import knn
 from oracle import knn as oknn
 from oracle.knn import isolated
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-
-
-def _dev_csr(M):
-    M = sp.csr_matrix(M, dtype=np.float32)
-    M.sort_indices()
-    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
-    return t(M.indptr, torch.int64), t(M.indices, torch.int32), t(M.data, torch.float32)
 
 
 def _int_matrix(U, I, dens, hi, seed):
@@ -49,7 +42,7 @@ def _gram_check(name):
         R[:, 0] = 63; R[:, 2] = 63                  # diagonal and off-diagonal 63^2 * 4096 = 16 257 024, just under 2^24
     else:
         R[0, :] = 63; R[2, :] = 63
-    urm = _dev_csr(R)
+    urm = dev_csr(R)
     X, rs, cs = ops.csr_to_dense_bf16(*urm, I, row_sq=True, col_sq=True)
     Ri = R.astype(np.int64)
     if over == "items":
@@ -100,7 +93,7 @@ def test_neighbours_equal_the_oracle_bitwise(over, cosine, k, dens, kind):
     U, I = (300, 1203) if over == "items" else (1203, 300)       # n not a multiple of 8, k above the nonzeros at 1 %
     R = _nbr_matrix(U, I, dens, kind, 5 + k)
     n = I if over == "items" else U
-    idx, val = knn.neighbours(_dev_csr(R), U, I, over, k, cosine, slab_rows=64)         # 19 slabs
+    idx, val = knn.neighbours(dev_csr(R), U, I, over, k, cosine, slab_rows=64)         # 19 slabs
     S = oknn.similarity(oknn.gram(R, over), cosine)
     oi, ov, oc = oknn.neighbours(S, k)
     assert np.array_equal(idx.cpu().numpy(), oi)
@@ -112,7 +105,7 @@ def test_neighbours_equal_the_oracle_bitwise(over, cosine, k, dens, kind):
 
 def test_neighbour_counts_and_slab_offset():
     R = _nbr_matrix(200, 131, 0.05, "int", 3)
-    urm = _dev_csr(R)
+    urm = dev_csr(R)
     X, _, cs = ops.csr_to_dense_bf16(*urm, 131, col_sq=True)
     j0, S = 40, 48
     C = ops.gemm_bf16(X[:, j0:], X, S, 131, 200, a_rows_are_k=True, b_rows_are_k=True)
@@ -152,7 +145,7 @@ def test_score_topk_integer_data_is_exact(n_cols, k):
     T = ops.knn_score_tile_cols()
     n_cols = {"tile": T, "tile+1": T + 1}.get(n_cols, n_cols)
     A, B, mask = _score_case(64, 50, n_cols, n_cols + k, integer=True)
-    dA, dB, dM = _dev_csr(A), _dev_csr(B), _dev_csr(mask)
+    dA, dB, dM = dev_csr(A), dev_csr(B), dev_csr(mask)
     f = knn.frac_bits(knn._bound(dA, dB))
     idx, val = ops.knn_score_topk(dA, dB, n_cols, k, f, dM[0], dM[1])
     oi, ov = _oracle_topk(A, B, mask, k, np.arange(64))
@@ -169,7 +162,7 @@ def test_score_topk_integer_data_is_exact(n_cols, k):
 def test_score_topk_real_values_within_bound(select, k):
     n_cols = ops.knn_score_tile_cols() + 77
     A, B, mask = _score_case(96, 80, n_cols, 9 + k, integer=False)
-    dA, dB, dM = _dev_csr(A), _dev_csr(B), _dev_csr(mask)
+    dA, dB, dM = dev_csr(A), dev_csr(B), dev_csr(mask)
     f = knn.frac_bits(knn._bound(dA, dB))
     if select == "users":
         rows = np.array([95, 3, 5, 40, 40, 0], np.int32)
@@ -240,7 +233,7 @@ def test_models_match_reference_goldens(model, size):
             W = knn.transpose_lists(torch.from_numpy(g[f"{tag}_nbr_idx"]).to(DEV), torch.from_numpy(g[f"{tag}_nbr_val"]).to(DEV))
             m.A, m.B = (m.urm, W) if over == "items" else (W, m.urm)
             m.frac_bits = knn.frac_bits(knn._bound(m.A, m.B))
-            mask = _dev_csr(R != 0)
+            mask = dev_csr(R != 0)
             ti, tv = m.topk(k, mask[0], mask[1])
             gi, gv = ti.cpu().numpy(), tv.cpu().numpy()
             ri, rv = g[f"{tag}_topk_idx"], g[f"{tag}_topk_val"]
@@ -253,31 +246,14 @@ def test_models_match_reference_goldens(model, size):
 
 
 # ---------------------------------------------------------------- 5. the reference's hello world at C1 scale
-@pytest.fixture(scope="module")
-def c1(tmp_path_factory):
-    g = dict(np.load(os.path.join(GOLD, "itemknn_c1.npz")))
-    d = tmp_path_factory.mktemp("knn_c1")
-    tsv = str(d / "dataset.tsv")
-    assert synth_c1.write_tsv(tsv) == int(g["checksum"]), "this numpy draws a different synthetic file than the golden's"
-    return g, d, tsv
-
-
-def _hello(d, tsv, tag, model_extra="", save_recs=True):
-    from elliot_b200 import run_experiment
-    out = d / tag
-    os.makedirs(out, exist_ok=True)
-    txt = synth_c1.hello_world_yaml(tsv, str(out), model_extra=model_extra)
-    if not save_recs:
-        txt = txt.replace("save_recs: True", "save_recs: False")
-    (out / "cfg.yml").write_text(txt)
-    return run_experiment(str(out / "cfg.yml"))[0], out
+c1 = c1h.c1_fixture("itemknn_c1.npz")
 
 
 def test_hello_world_itemknn_matches_the_reference_run(c1):
     g, d, tsv = c1
-    res, out = _hello(d, tsv, "host")
-    for m, want in zip(g["metrics"].tolist(), g["test_metrics"]):
-        assert abs(res["test_results"][10][m] - float(want)) <= 1e-4, (m, res["test_results"][10][m], float(want))
+    out = d / "host"
+    res = c1h.run(out, synth_c1.hello_world_yaml(tsv, str(out)))
+    c1h.assert_metrics(res, g["metrics"].tolist(), g["test_metrics"])
     files = os.listdir(out / "recs")
     assert files == [str(g["rec_file"])], (files, str(g["rec_file"]))
     rec = np.loadtxt(out / "recs" / files[0], delimiter="\t")
@@ -294,7 +270,7 @@ def test_hello_world_itemknn_matches_the_reference_run(c1):
 
 def test_hello_world_itemknn_device_eval_without_recs(c1):
     g, d, tsv = c1
-    res, out = _hello(d, tsv, "device", model_extra="      b200_eval: device\n", save_recs=False)
-    for m, want in zip(g["metrics"].tolist(), g["test_metrics"]):
-        assert abs(res["test_results"][10][m] - float(want)) <= 1e-4, m
-    assert not os.path.exists(out / "recs") or not os.listdir(out / "recs")
+    out = d / "device"
+    res = c1h.run(out, synth_c1.hello_world_yaml(tsv, str(out), model_extra="      b200_eval: device\n"), device_eval=True)
+    c1h.assert_metrics(res, g["metrics"].tolist(), g["test_metrics"])
+    c1h.assert_no_rec_files(out)

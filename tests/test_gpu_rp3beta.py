@@ -8,25 +8,19 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+import c1_harness as c1h
+from c1_harness import DEV, GOLD, all_scores, to_dev, w_host
 from elliot_b200 import ops
 from elliot_b200._lib import EbError
 from oracle import rp3beta as orp3
 from oracle.knn import isolated, topk as oracle_topk
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
 _G = dict(np.load(os.path.join(GOLD, "rp3beta_cases.npz")))
 
 
-def _t(a, dt=None):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
-
-
 def _dev_csr(M):
-    M = sp.csr_matrix(M, dtype=np.float32)
-    return _t(M.indptr, torch.int64), _t(M.indices, torch.int32), _t(M.data, torch.float32)
+    return c1h.dev_csr(M, sort=False)
 
 
 class _Data:
@@ -43,25 +37,10 @@ def _case(name):
 
 def _device_lists(m):
     (pp, pi, pv), (qp, qi, qv), degree = m.host_operands()
-    idx, val, cnt = ops.rp3_similarity((_t(qp, torch.int64), _t(qi, torch.int32), _t(qv)),
-                                       (_t(pp, torch.int64), _t(pi, torch.int32), _t(pv)), _t(degree, torch.float64), m.k)
+    idx, val, cnt = ops.rp3_similarity((to_dev(qp, torch.int64), to_dev(qi, torch.int32), to_dev(qv)),
+                                       (to_dev(pp, torch.int64), to_dev(pi, torch.int32), to_dev(pv)), to_dev(degree, torch.float64), m.k)
     idx, val, cnt = idx.cpu().numpy(), val.cpu().numpy(), cnt.cpu().numpy()
     return {i: (idx[i, :cnt[i]].astype(np.int64), val[i, :cnt[i]]) for i in range(len(cnt))}
-
-
-def _w_host(W, n):
-    p, i, v = (a.cpu().numpy() for a in W)
-    return sp.csr_matrix((v, i, p), shape=(n, n))
-
-
-def _all_scores(A, W, n):
-    """Every column's score of every row, read back from a top-n call without a mask."""
-    idx, val = ops.rp3_score_topk(A, W, n, n)
-    idx, val = idx.cpu().numpy(), val.cpu().numpy()
-    P = np.zeros((idx.shape[0], n), np.float32)
-    np.put_along_axis(P, idx.astype(np.int64), val, 1)
-    assert np.all(np.sort(idx, 1) == np.arange(n)[None, :])
-    return P
 
 
 # ---------------------------------------------------------------- 1. the model against the oracle and the goldens
@@ -81,7 +60,7 @@ def test_similarity_w_and_scores_match(name):
         assert np.array_equal(mine[i][0], lists_or[i][0]), (name, i)
         assert np.array_equal(mine[i][1].view(np.int32), lists_or[i][1].view(np.int32)), (name, i)
     m.initialize()
-    W = _w_host(m.W, n)
+    W = w_host(m.W, n)
     assert np.array_equal(W.indptr, W_or.indptr) and np.array_equal(W.indices, W_or.indices), name
     assert np.array_equal(W.data.view(np.int32), W_or.data.view(np.int32)), name
     ref_lists = orp3.reference_lists(_G[f"{name}_s_row"], _G[f"{name}_s_col"], _G[f"{name}_s_val"], n)
@@ -89,7 +68,7 @@ def test_similarity_w_and_scores_match(name):
     orp3.w_equal_but_ties(W, W_ref, lists_or, ref_lists, k)
     # scores from the golden's own W: bit-equal to the reference's preds
     W_ref.sort_indices()
-    P = _all_scores(m.urm, _dev_csr(W_ref), n)
+    P = all_scores(m.urm, _dev_csr(W_ref), n)
     assert orp3.preds_digest(P) == str(_G[f"{name}_preds_sha256"]), name
     # the model's lists equal the oracle's (same W, same tie rule), and with the golden's W the reference's lists
     # wherever the k-th and (k+1)-th scores differ
@@ -117,7 +96,7 @@ def test_neighborhood_minus_one_keeps_every_nonzero():
     assert m.k == R.shape[1]
     m.initialize()
     W_or, _ = orp3.weights(sp.csr_matrix(R.astype(np.float32)), alpha, beta, k, norm)
-    W = _w_host(m.W, R.shape[1])
+    W = w_host(m.W, R.shape[1])
     assert W.nnz == W_or.nnz == int(_G[f"{name}_w_data"].size)
 
 
@@ -163,7 +142,7 @@ def test_column_tiled_path_matches_the_oracle():
     W.sort_indices()
     users = np.array([0, 7, 14, 350, 699, 3], np.int32)
     mask = _dev_csr(R != 0)
-    ti, tv = ops.rp3_score_topk(m.urm, _dev_csr(W), n, 100, mask[0], mask[1], users=_t(users))
+    ti, tv = ops.rp3_score_topk(m.urm, _dev_csr(W), n, 100, mask[0], mask[1], users=to_dev(users))
     P = orp3.preds(R, W, rows=users).astype(np.float64)
     oi, ov = oracle_topk(P, (R != 0).toarray()[users], 100)
     assert np.array_equal(ti.cpu().numpy(), oi)
@@ -177,32 +156,18 @@ def test_bad_arguments_are_refused():
 
 
 # ---------------------------------------------------------------- 3. run_experiment at C1 scale
-@pytest.fixture(scope="module")
-def c1(tmp_path_factory):
-    from elliot_b200 import synth_c1
-    g = dict(np.load(os.path.join(GOLD, "rp3beta_c1.npz")))
-    d = tmp_path_factory.mktemp("rp3beta_c1")
-    tsv = str(d / "dataset.tsv")
-    assert synth_c1.write_tsv(tsv) == int(g["checksum"]), "this numpy draws a different synthetic file than the golden's"
-    return g, d, tsv
+c1 = c1h.c1_fixture("rp3beta_c1.npz")
 
 
 @pytest.mark.parametrize("ev", ["host", "device"])
 def test_run_experiment_matches_the_reference_run(c1, ev):
-    from elliot_b200 import run_experiment, synth_c1
+    from elliot_b200 import synth_c1
     g, d, tsv = c1
     out = d / ev
-    os.makedirs(out, exist_ok=True)
-    txt = synth_c1.rp3beta_yaml(tsv, str(out), model_extra=f"      b200_eval: {ev}\n")
-    if ev == "device":                      # metrics straight from the top-k tensor: no rec dicts, no rec files
-        txt = txt.replace("save_recs: True", "save_recs: False")
-    (out / "cfg.yml").write_text(txt)
-    res = run_experiment(str(out / "cfg.yml"))[0]
-    for m, want in zip(g["metrics"].tolist(), g["test_metrics"]):
-        got = res["test_results"][10][m]
-        assert abs(got - float(want)) <= 1e-4, (ev, m, got, float(want))
+    res = c1h.run(out, synth_c1.rp3beta_yaml(tsv, str(out), model_extra=f"      b200_eval: {ev}\n"), ev == "device")
+    c1h.assert_metrics(res, g["metrics"].tolist(), g["test_metrics"], ev)
     if ev == "device":
-        assert not os.path.exists(out / "recs") or not os.listdir(out / "recs")
+        c1h.assert_no_rec_files(out)
         return
     files = os.listdir(out / "recs")
     assert files == [str(g["rec_file"])], (files, str(g["rec_file"]))          # the same model `name` as the reference's

@@ -7,28 +7,15 @@ import os
 import numpy as np
 import pytest
 import scipy.sparse as sp
-import torch
 
-from elliot_b200 import ops
+import c1_harness as c1h
+from c1_harness import DEV, GOLD, all_scores, dev_csr, w_host
 from oracle import slim as oslim
 from oracle.knn import isolated, topk as oracle_topk
 from oracle.rp3beta import preds_digest
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
 _G = dict(np.load(os.path.join(GOLD, "slim_cases.npz")))
-
-
-def _t(a, dt=None):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
-
-
-def _dev_csr(M):
-    M = sp.csr_matrix(M, dtype=np.float32)
-    M.sort_indices()
-    return _t(M.indptr, torch.int64), _t(M.indices, torch.int32), _t(M.data, torch.float32)
 
 
 class _Data:
@@ -43,19 +30,6 @@ def _model(name, **kw):
                   int(_G["seed"]), DEV)
     m.initialize(**kw)
     return R, m
-
-
-def _w_host(W, n):
-    p, i, v = (a.cpu().numpy() for a in W)
-    return sp.csr_matrix((v, i, p), shape=(n, n))
-
-
-def _all_scores(A, W, n):
-    idx, val = ops.rp3_score_topk(A, W, n, n)
-    idx, val = idx.cpu().numpy(), val.cpu().numpy()
-    P = np.zeros((idx.shape[0], n), np.float32)
-    np.put_along_axis(P, idx.astype(np.int64), val, 1)
-    return P
 
 
 # ---------------------------------------------------------------- 1. the model against the oracle and the goldens
@@ -73,7 +47,7 @@ def test_coefficients_w_and_scores_match(name):
     assert np.array_equal(n_iter, oi), name
     assert np.allclose(m.gap.cpu().numpy(), og, rtol=1e-3, atol=1e-12), name
     assert np.array_equal(m.nnz.cpu().numpy(), (oc != 0).sum(1)), name
-    W = _w_host(m.W, n)
+    W = w_host(m.W, n)
     W_or = oslim.select(oc, int(_G[f"{name}_neighborhood"]))
     assert np.array_equal(W.indptr, W_or.indptr) and np.array_equal(W.indices, W_or.indices), name
     assert np.array_equal(W.data.view(np.int32), W_or.data.view(np.int32)), name
@@ -81,11 +55,11 @@ def test_coefficients_w_and_scores_match(name):
     oslim.w_equal_except_ties(W, Wg, _G[f"{name}_coef"])
     # scores from the golden's own W: bit-equal to the reference's preds
     Wg.sort_indices()
-    P = _all_scores(m.urm, _dev_csr(Wg), n)
+    P = all_scores(m.urm, dev_csr(Wg), n)
     assert preds_digest(P) == str(_G[f"{name}_preds_sha256"]), name
     # the model's lists: the oracle's, and the reference's at isolated ranks
     K = int(_G["topk"])
-    mask = _dev_csr(R != 0)
+    mask = dev_csr(R != 0)
     ti, tv = m.topk(K, mask[0], mask[1])
     gi = ti.cpu().numpy()
     oi_, ov_ = oracle_topk(oslim.preds(R, W_or).astype(np.float64), R != 0, K + 1)
@@ -109,7 +83,7 @@ def test_reruns_are_bit_identical():
     outs = []
     for _ in range(2):
         R, m = _model("implicit_default")
-        mask = _dev_csr(R != 0)
+        mask = dev_csr(R != 0)
         ti, tv = m.topk(50, mask[0], mask[1])
         outs.append([a.cpu().numpy().view(np.int32) for a in (m.coef_t, m.n_iter, *m.W[1:], ti, tv)])
     for a, b in zip(*outs):
@@ -123,31 +97,18 @@ def test_more_items_than_users_is_refused():
 
 
 # ---------------------------------------------------------------- 2. run_experiment at C1 scale
-@pytest.fixture(scope="module")
-def c1(tmp_path_factory):
-    from elliot_b200 import synth_c1
-    g = dict(np.load(os.path.join(GOLD, "slim_c1.npz")))
-    d = tmp_path_factory.mktemp("slim_c1")
-    tsv = str(d / "dataset.tsv")
-    assert synth_c1.write_tsv(tsv) == int(g["checksum"]), "this numpy draws a different synthetic file than the golden's"
-    return g, d, tsv
+c1 = c1h.c1_fixture("slim_c1.npz")
 
 
 @pytest.mark.parametrize("ev", ["host", "device"])
 def test_run_experiment_matches_the_reference_run(c1, ev):
-    from elliot_b200 import run_experiment, synth_c1
+    from elliot_b200 import synth_c1
     g, d, tsv = c1
     out = d / ev
-    os.makedirs(out, exist_ok=True)
-    txt = synth_c1.slim_yaml(tsv, str(out), model_extra=f"      b200_eval: {ev}\n")
-    if ev == "device":                      # metrics straight from the top-k tensor: no rec dicts, no rec files
-        txt = txt.replace("save_recs: True", "save_recs: False")
-    (out / "cfg.yml").write_text(txt)
-    res = run_experiment(str(out / "cfg.yml"))[0]
-    for m, want in zip(g["metrics"].tolist(), g["test_metrics"]):
-        got = res["test_results"][10][m]
-        assert abs(got - float(want)) <= 1e-4, (ev, m, got, float(want))
+    res = c1h.run(out, synth_c1.slim_yaml(tsv, str(out), model_extra=f"      b200_eval: {ev}\n"), ev == "device")
+    c1h.assert_metrics(res, g["metrics"].tolist(), g["test_metrics"], ev)
     if ev == "device":
+        c1h.assert_no_rec_files(out)
         return
     files = os.listdir(out / "recs")
     assert files == [str(g["rec_file"])], (files, str(g["rec_file"]))          # the same model `name` as the reference's

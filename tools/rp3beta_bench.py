@@ -31,6 +31,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 from elliot_b200 import ops  # noqa: E402
+from elliot_b200.recommender._device import upload, upload_csr  # noqa: E402
 from elliot_b200.recommender.rp3beta import RP3Model  # noqa: E402
 from knn_bench import c1_matrix, ml20m_matrix  # noqa: E402
 
@@ -48,18 +49,16 @@ def run_once(m):
     ev = {n: (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for n in names}
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    (pp, pi, pv), (qp, qi, qv), degree = m.host_operands()
+    pui, piu, degree = m.host_operands()
     R = m.R
     work = np.bincount(R.indices, weights=np.diff(R.indptr)[np.repeat(np.arange(m.n_users), np.diff(R.indptr))],
                        minlength=m.n_items)
     order_np = np.argsort(-work, kind="stable")
     host = time.perf_counter() - t0
-    to = m._to
     a, b = ev["upload"]
     a.record()
-    Pui = (to(pp, torch.int64), to(pi, torch.int32), to(pv, torch.float32))
-    Piu = (to(qp, torch.int64), to(qi, torch.int32), to(qv, torch.float32))
-    deg, order = to(degree, torch.float64), to(order_np, torch.int32)
+    Pui, Piu = upload_csr(*pui, m.device), upload_csr(*piu, m.device)
+    deg, order = upload(degree, m.device, torch.float64), upload(order_np, m.device, torch.int32)
     b.record()
     a, b = ev["similarity"]
     a.record(); idx, val, cnt = ops.rp3_similarity(Piu, Pui, deg, m.k, order=order); b.record()

@@ -30,6 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 from elliot_b200 import ops  # noqa: E402
+from elliot_b200.recommender._device import upload_csr  # noqa: E402
 from elliot_b200.recommender.slim import SlimModel, seed_state  # noqa: E402
 from knn_bench import c1_matrix, ml20m_matrix  # noqa: E402
 
@@ -45,8 +46,7 @@ class _Data:
 def _operands(m):
     C = m.R.tocsc()
     C.sort_indices()
-    to = m._to
-    return (to(C.indptr, torch.int64), to(C.indices, torch.int32), to(C.data, torch.float32)), (m.urm[0], m.urm[1])
+    return upload_csr(C.indptr, C.indices, C.data, m.device), (m.urm[0], m.urm[1])
 
 
 def run_once(m):
