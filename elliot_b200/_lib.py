@@ -27,6 +27,11 @@ SIGNATURES = {
     "eb_bpr_step_sampled_filter_f32": (c_int, [c_void, c_void, c_void, c_int, c_int, c_i32, c_i32, c_void, c_void, c_void, c_int,
                                                c_i64, c_u64, c_u64, c_f32, c_f32, c_f32, c_f32, c_f32,
                                                c_void, c_void, c_void, c_void, c_void, c_size, c_int, c_void]),
+    "eb_bpr_schedule_sampled": (c_int, [c_i32, c_i32, c_void, c_i64, c_u64, c_u64, c_void, c_size, ctypes.POINTER(c_size), c_int,
+                                        c_void]),
+    "eb_bpr_apply_sampled_filter_f32": (c_int, [c_void, c_void, c_void, c_int, c_int, c_i32, c_i32, c_void, c_void, c_void, c_int,
+                                                c_i64, c_u64, c_u64, c_f32, c_f32, c_f32, c_f32, c_f32,
+                                                c_void, c_void, c_void, c_void, c_void, c_int, c_void]),
     "eb_bpr_sample_philox_filter": (c_int, [c_i32, c_i32, c_void, c_void, c_void, c_int, c_i64, c_u64, c_u64, c_void, c_void, c_void,
                                             c_void]),
     "eb_bpr_sample_philox": (c_int, [c_i32, c_i32, c_void, c_void, c_i64, c_u64, c_u64, c_void, c_void, c_void,

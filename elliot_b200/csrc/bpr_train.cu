@@ -720,29 +720,38 @@ static GroupLayout group_layout(int64_t n, int32_t n_users) {
     return L;
 }
 
-// Sampled step on local tables, free-running: per sub-step, the user keys, the stable sort of the triple indices by user,
-// then the grouped update.  The key pass and the update leave `reserve` SMs free; cub's sort kernels size their own grids.
+// The schedule of one sub-step (p.n <= GROUP_MAX): the user keys and the stable sort of the triple indices by user.  Reads
+// only seed, first, n, n_users, n_items and indptr, never the tables.  The ordered indices end up in one of the workspace's two
+// index buffers (cub's double buffer decides which): `order` points at it.  The key pass leaves `reserve` SMs free; cub's
+// sort kernels size their own grids.
+static int schedule_grouped(const HogwildParams &p, int reserve, char *ws, const GroupLayout &L, cudaStream_t st,
+                            const int32_t *&order) {
+    int sms = sm_count() - reserve;
+    if (sms < 1) sms = 1;
+    cub::DoubleBuffer<uint32_t> keys((uint32_t *)(ws + L.key_a), (uint32_t *)(ws + L.key_b));
+    cub::DoubleBuffer<int32_t> vals((int32_t *)(ws + L.val_a), (int32_t *)(ws + L.val_b));
+    int64_t grid = (p.n + 255) / 256;
+    if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
+    user_key_kernel<<<(unsigned)grid, 256, 0, st>>>(p, keys.Current(), vals.Current());
+    EB_CUDA(cudaGetLastError());
+    size_t cb = L.cub_bytes;
+    EB_CUDA(cub::DeviceRadixSort::SortPairs(ws + L.cub, cb, keys, vals, (int)p.n, 0, bits_for((uint64_t)p.n_users), st));
+    order = vals.Current();
+    return EB_OK;
+}
+
+// Sampled step on local tables, free-running: per sub-step, the schedule above, then the grouped update (which leaves
+// `reserve` SMs free).
 template <int DP, bool ATOMIC>
 static int launch_grouped(HogwildParams p, int reserve, char *ws, const GroupLayout &L, cudaStream_t st) {
-    const int ubits = bits_for((uint64_t)p.n_users);
     const int64_t n = p.n;
     const uint64_t first = p.first;
     int32_t *out_u = p.out_u, *out_i = p.out_i, *out_j = p.out_j;
-    int sms = sm_count() - reserve;
-    if (sms < 1) sms = 1;
     for (int64_t c0 = 0; c0 < n; c0 += GROUP_MAX) {
         p.n = n - c0 < GROUP_MAX ? n - c0 : GROUP_MAX;
         p.first = first + (uint64_t)c0;
         if (out_u) { p.out_u = out_u + c0; p.out_i = out_i + c0; p.out_j = out_j + c0; }
-        cub::DoubleBuffer<uint32_t> keys((uint32_t *)(ws + L.key_a), (uint32_t *)(ws + L.key_b));
-        cub::DoubleBuffer<int32_t> vals((int32_t *)(ws + L.val_a), (int32_t *)(ws + L.val_b));
-        int64_t grid = (p.n + 255) / 256;
-        if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
-        user_key_kernel<<<(unsigned)grid, 256, 0, st>>>(p, keys.Current(), vals.Current());
-        EB_CUDA(cudaGetLastError());
-        size_t cb = L.cub_bytes;
-        EB_CUDA(cub::DeviceRadixSort::SortPairs(ws + L.cub, cb, keys, vals, (int)p.n, 0, ubits, st));
-        p.order = vals.Current();
+        if (int rc = schedule_grouped(p, reserve, ws, L, st, p.order)) return rc;
         if (int rc = launch_grouped_t<DP, ATOMIC>(p, reserve, st)) return rc;
     }
     return EB_OK;
@@ -777,6 +786,18 @@ static int launch_hogwild(const HogwildParams &p, int dp, int flags, cudaStream_
                                        : launch_hogwild_t<DP, false, false, false, false>(p, reserve, st);
         }
         return launch_hogwild_t<DP, SAMPLE, true, false, true>(p, reserve, st);   // deterministic rounds
+    });
+}
+
+// The grouped update alone, on an order the caller scheduled (p.order, p.n <= GROUP_MAX)
+static int launch_apply(const HogwildParams &p, int dp, int flags, cudaStream_t st) {
+    const bool atomic = !(flags & 1);
+    const int reserve = (flags >> 8) & 0xff;
+    EB_ARG(!(flags & (32 | 64)), "the grouped update runs free-running on local tables (no rounds, no staged kernel)");
+    return with_stride<8, 16, 32, 64, 128, 256>(dp, "8,16,32,64,128,256 floats", [&](auto dpc) {
+        constexpr int DP = decltype(dpc)::value;
+        item_table_l2_window(p, st);
+        return atomic ? launch_grouped_t<DP, true>(p, reserve, st) : launch_grouped_t<DP, false>(p, reserve, st);
     });
 }
 
@@ -1041,6 +1062,44 @@ extern "C" int eb_bpr_step_sampled_filter_f32(float *U, float *V, float *item_bi
     p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
     if (int rc = set_filter(p, filter, filter_words)) return rc;
     return launch_hogwild<true>(p, ld, flags, (cudaStream_t)stream, workspace, workspace_bytes);
+}
+
+extern "C" int eb_bpr_schedule_sampled(int32_t n_users, int32_t n_items, const int64_t *csr_indptr, int64_t n, uint64_t seed,
+                                       uint64_t first_triple, void *workspace, size_t workspace_bytes, size_t *order_offset,
+                                       int flags, void *stream) {
+    EB_ARG(n >= 1 && n <= GROUP_MAX && n_users > 0 && n_items > 1, "bad sizes (a schedule covers 1..%lld triples)",
+           (long long)GROUP_MAX);
+    EB_ARG(csr_indptr && order_offset, "null pointer");
+    const GroupLayout L = group_layout(n, n_users);
+    if (!workspace || workspace_bytes < L.total)
+        return set_err(EB_ERR_WORKSPACE, "workspace %zu < required %zu", workspace ? workspace_bytes : 0, L.total);
+    HogwildParams p{};
+    p.n = n; p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.seed = seed; p.first = first_triple;
+    const int32_t *order = nullptr;
+    if (int rc = schedule_grouped(p, (flags >> 8) & 0xff, (char *)workspace, L, (cudaStream_t)stream, order)) return rc;
+    *order_offset = (size_t)((const char *)order - (const char *)workspace);
+    return EB_OK;
+}
+
+extern "C" int eb_bpr_apply_sampled_filter_f32(float *U, float *V, float *item_bias, int d, int ld, int32_t n_users,
+                                               int32_t n_items, const int64_t *csr_indptr, const int32_t *csr_indices,
+                                               const uint32_t *filter, int filter_words, int64_t n, uint64_t seed,
+                                               uint64_t first_triple, float lr, float reg_u, float reg_b, float reg_pos,
+                                               float reg_neg, double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
+                                               const int32_t *order, int flags, void *stream) {
+    if (int rc = check_tables(U, V, item_bias, d, ld)) return rc;
+    EB_ARG(n >= 1 && n <= GROUP_MAX && n_users > 0 && n_items > 1, "bad sizes (an apply covers 1..%lld triples)",
+           (long long)GROUP_MAX);
+    EB_ARG(csr_indptr && csr_indices && order, "null CSR or order");
+    EB_ARG((!out_u && !out_i && !out_j) || (out_u && out_i && out_j), "out_u/out_i/out_j: all or none");
+    HogwildParams p{};
+    p.U = U; p.V = V; p.b = item_bias; p.ld = ld; p.n = n;
+    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
+    p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
+    p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
+    p.order = order;
+    if (int rc = set_filter(p, filter, filter_words)) return rc;
+    return launch_apply(p, ld, flags, (cudaStream_t)stream);
 }
 
 extern "C" int eb_bpr_step_peer_f32(float *U, float *const *V_shards, float *const *b_shards, int n_shards, int32_t shard_rows,

@@ -7,6 +7,7 @@ wrappers keep a grow-only scratch buffer per device (scoring, evaluation, the na
 global-bias accumulator): those ops must not run concurrently on two streams of the same device from one process.
 """
 import ctypes
+import os
 
 import torch
 
@@ -76,7 +77,10 @@ def bpr_step_sampled_f32(U, V, b, d, n_users, n_items, indptr, indices, n, seed,
                          reg_neg, loss=None, out=None, racy=False, reserve_sms=0, filter=None, deterministic=False, _variant=0):
     """Fused sample+update step (custom_sampler.py:24-46 distribution, Philox stream).  filter: bloom_build() output.
     The default free-running Hogwild step applies the triples grouped by user (key pass, stable sort, update; see
-    eb_bpr_step_sampled_f32) with a grow-only device workspace of this module.
+    eb_bpr_step_sampled_f32) with device workspace of this module.  Once two calls in a row have advanced `first` by
+    exactly `n`, each call also schedules the next one (key pass and sort) on a side stream while its own update runs;
+    the next call uses that schedule only if it asks for exactly those triples on the same, unmodified CSR
+    (set_bpr_prefetch).  Which triples are drawn and how they are applied does not depend on it.
     deterministic: run the launch in rounds (reads, grid barrier, atomic adds, grid barrier) so the same inputs give the same
     tables on every run up to fp32 summation order; slower than the default free-running Hogwild.
     _variant (profiling): one table always runs the register-staged kernel (16 or 0); 32, the shared-memory-staged kernel,
@@ -87,16 +91,118 @@ def bpr_step_sampled_f32(U, V, b, d, n_users, n_items, indptr, indices, n, seed,
     if out is not None:
         ou, oi, oj = out
         _need_cuda(ou, oi, oj); _chk_idx(ou, oi, oj)
+    flags = (1 if racy else 0) | (64 if deterministic else 0) | ((int(reserve_sms) & 0xff) << 8) | int(_variant)
+    fw = 0 if filter is None else filter.shape[1]
+    if _prefetch_on and not deterministic and not _variant and 1 <= n <= _SCHEDULE_MAX:
+        with torch.cuda.device(U.device):
+            _schedules_of(U.device).step(U, V, b, d, n_users, n_items, indptr, indices, filter, fw, n, seed, first,
+                                         (lr, reg_u, reg_b, reg_pos, reg_neg), loss, (ou, oi, oj), flags)
+        return
     ws = None
     if not deterministic:
         ws = _ws_grouped.get(lib().eb_bpr_step_sampled_workspace_bytes(n, n_users), U.device)
     with torch.cuda.device(U.device):
         check(lib().eb_bpr_step_sampled_filter_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), n_users, n_items, _ptr(indptr),
-                                                   _ptr(indices), _ptr(filter), 0 if filter is None else filter.shape[1], n, seed,
+                                                   _ptr(indices), _ptr(filter), fw, n, seed,
                                                    first, lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), _ptr(ou), _ptr(oi),
-                                                   _ptr(oj), _ptr(ws), 0 if ws is None else ws.numel(),
-                                                   (1 if racy else 0) | (64 if deterministic else 0) | ((int(reserve_sms) & 0xff) << 8) | int(_variant),
-                                                   _stream(U)))
+                                                   _ptr(oj), _ptr(ws), 0 if ws is None else ws.numel(), flags, _stream(U)))
+
+
+# ---- schedule prefetch of the grouped sampled step
+_SCHEDULE_MAX = 2**31 - 1                     # longer calls run as sub-steps inside eb_bpr_step_sampled_f32
+_prefetch_on = os.environ.get("EB_BPR_PREFETCH", "1") != "0"
+_schedules = {}
+
+
+def set_bpr_prefetch(enabled):
+    """Schedule prefetch of bpr_step_sampled_f32 on (the default; EB_BPR_PREFETCH=0 starts with it off) or off.  Off, every
+    call schedules and applies on the caller's stream as eb_bpr_step_sampled_f32 does, and the schedule slots are freed.
+    Returns the previous setting."""
+    global _prefetch_on
+    was, _prefetch_on = _prefetch_on, bool(enabled)
+    if not enabled:
+        for s in _schedules.values():
+            s.release()
+        _schedules.clear()
+    return was
+
+
+def _schedules_of(device):
+    i = device.index if device.index is not None else torch.cuda.current_device()
+    if i not in _schedules:
+        _schedules[i] = _Schedules(torch.device("cuda", i))
+    return _schedules[i]
+
+
+class _Schedules:
+    """Two schedule slots of one device (workspace of eb_bpr_schedule_sampled each: user keys and triple indices,
+    double-buffered for the sort, 16 B per triple + cub's storage) and the side stream that fills them ahead of time.
+
+    A call applies the order in one slot.  When it continues the previous call (first advanced by exactly n), it then
+    enqueues the schedule of first + n into the other slot on the side stream: after an event recorded on the caller's
+    stream just before the apply (everything the caller enqueued earlier, CSR edits included, is visible) and after the
+    last apply that read that slot.  The next call takes the slot if its key matches, waiting on the slot's event;
+    otherwise it schedules inline.  The key holds the CSR tensors' version counters, so an in-place edit of indptr or
+    indices invalidates a prefetched order."""
+
+    def __init__(self, device):
+        self.device = device
+        self.side = torch.cuda.Stream(device)
+        self.buf = [None, None]
+        self.off = [0, 0]
+        self.key = [None, None]            # call a slot's pending prefetched order was made for
+        self.built = [torch.cuda.Event(), torch.cuda.Event()]   # the slot's last schedule has been written
+        self.read = [torch.cuda.Event(), torch.cuda.Event()]    # the last apply that read the slot has finished
+        self.ready = torch.cuda.Event()
+        self.cur = 0                       # slot of the last call
+        self.last = None                   # (first, n) of the last call
+
+    def release(self):
+        for e in self.built + self.read:
+            e.synchronize()
+        self.buf = [None, None]
+        self.key = [None, None]
+
+    def _schedule(self, s, n_users, n_items, indptr, n, seed, first, flags, stream):
+        need = int(lib().eb_bpr_step_sampled_workspace_bytes(n, n_users))
+        if self.buf[s] is None or self.buf[s].numel() < need:
+            self.built[s].synchronize(); self.read[s].synchronize()
+            self.buf[s] = None
+            self.buf[s] = torch.empty(need, dtype=torch.uint8, device=self.device)
+            self.buf[s].record_stream(self.side)
+        off = ctypes.c_size_t(0)
+        check(lib().eb_bpr_schedule_sampled(n_users, n_items, _ptr(indptr), n, seed, first, _ptr(self.buf[s]), self.buf[s].numel(),
+                                            ctypes.byref(off), flags & 0xff00, stream.cuda_stream))
+        self.off[s] = off.value
+
+    def step(self, U, V, b, d, n_users, n_items, indptr, indices, filt, fw, n, seed, first, hp, loss, out, flags):
+        st = torch.cuda.current_stream(self.device)
+        csr = (n_users, n_items, indptr.data_ptr(), indices.data_ptr(), _ptr(filt), indptr._version, indices._version)
+        key = (seed, first, n) + csr
+        s = 0 if self.key[0] == key else 1 if self.key[1] == key else None
+        if s is None:
+            s = self.cur
+            st.wait_event(self.built[s]); st.wait_event(self.read[s])
+            self._schedule(s, n_users, n_items, indptr, n, seed, first, flags, st)
+        else:
+            st.wait_event(self.built[s])
+        self.key[s] = None
+        ahead = self.last == (first - n, n)
+        if ahead:
+            self.ready.record(st)
+        order = self.buf[s].data_ptr() + self.off[s]
+        check(lib().eb_bpr_apply_sampled_filter_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), n_users, n_items, _ptr(indptr),
+                                                    _ptr(indices), _ptr(filt), fw, n, seed, first, *hp, _ptr(loss),
+                                                    *(_ptr(x) for x in out), order, flags, st.cuda_stream))
+        self.read[s].record(st)
+        self.cur, self.last = s, (first, n)
+        if ahead:
+            o = 1 - s
+            self.side.wait_event(self.ready); self.side.wait_event(self.read[o])
+            self._schedule(o, n_users, n_items, indptr, n, seed, first + n, flags, self.side)
+            self.built[o].record(self.side)
+            indptr.record_stream(self.side)
+            self.key[o] = (seed, first + n, n) + csr
 
 
 def bpr_sample_philox(n_users, n_items, indptr, indices, n, seed, first=0, filter=None):

@@ -104,6 +104,25 @@ int eb_bpr_step_sampled_filter_f32(float *U, float *V, float *item_bias, int d, 
                                    float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
                                    double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
                                    void *workspace, size_t workspace_bytes, int flags, void *stream);
+/* The two halves of the free-running sampled step above, for one call of at most INT32_MAX triples; the step is the
+ * schedule followed by the apply.  The schedule is the key pass and the stable sort: it reads only csr_indptr (never the
+ * tables), so the schedule of the next call can run on another stream while this call's apply runs.  workspace: at least
+ * eb_bpr_step_sampled_workspace_bytes(n, n_users) bytes; the ordered triple indices (n int32) are left at byte
+ * *order_offset of it.  Flags bits 8..15: the key pass leaves that many SMs free.
+ * The apply samples triple order[k] for k = 0..n-1 (triple t draws the same as in the step, whatever the order, and is
+ * emitted at index t) and applies it grouped as in the step.  Any permutation of [0, n) gives the step's triples; one
+ * sorted by user (the schedule's) gives long user runs.  Flags as for the step, without deterministic rounds (bit 6). */
+int eb_bpr_schedule_sampled(int32_t n_users, int32_t n_items, const int64_t *csr_indptr, int64_t n, uint64_t seed,
+                            uint64_t first_triple, void *workspace, size_t workspace_bytes, size_t *order_offset, int flags,
+                            void *stream);
+int eb_bpr_apply_sampled_filter_f32(float *U, float *V, float *item_bias, int d, int ld,
+                                    int32_t n_users, int32_t n_items,
+                                    const int64_t *csr_indptr, const int32_t *csr_indices,
+                                    const uint32_t *filter, int filter_words,
+                                    int64_t n, uint64_t seed, uint64_t first_triple,
+                                    float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
+                                    double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
+                                    const int32_t *order, int flags, void *stream);
 int eb_bpr_sample_philox_filter(int32_t n_users, int32_t n_items, const int64_t *csr_indptr,
                                 const int32_t *csr_indices, const uint32_t *filter, int filter_words, int64_t n,
                                 uint64_t seed, uint64_t first_triple, int32_t *out_u, int32_t *out_i, int32_t *out_j,
