@@ -167,6 +167,13 @@ SIGNATURES = {
                                 ctypes.c_uint32, c_int, c_int, c_int, c_i32, c_void, c_void, c_void, c_void, c_void, c_void,
                                 c_size, c_void]),
     "eb_slim_drop_f32": (c_int, [c_i32, c_void, c_void, c_void]),
+    "eb_svd_max_width": (c_int, []),
+    "eb_csr_spmm_f64": (c_int, [c_void, c_void, c_void, c_i64, c_void, c_int, c_i64, c_void, c_i64, c_void]),
+    "eb_chol_pivoted_f64": (c_int, [c_void, c_int, c_void, c_void, c_void]),
+    "eb_tall_times_small_f64": (c_int, [c_void, c_i64, c_int, c_i64, c_void, c_int, c_void, c_i64, c_void]),
+    "eb_sym_eig_f64_workspace_bytes": (c_size, [c_int]),
+    "eb_sym_eig_f64": (c_int, [c_void, c_int, c_void, c_void, c_void, c_size, c_void]),
+    "eb_svd_finish_f64": (c_int, [c_void, c_int, c_int, c_void, c_i64, c_i64, c_void, c_i64, c_i64, c_int, c_void, c_void]),
 }
 
 _lib = None

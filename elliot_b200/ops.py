@@ -907,6 +907,96 @@ def slim_weights(coef_t, drop, nnz, neighborhood):
     return indptr, indices[:m], values[:m]
 
 
+# ---------------------------------------------------------------- randomized SVD pieces (pure_svd.cu)
+def svd_max_width():
+    """Largest block width the SVD pieces take (the limit of gram_f64)."""
+    return int(lib().eb_svd_max_width())
+
+
+def _chk_f64(*ts):
+    for t in ts:
+        if t.dtype != torch.float64 or t.dim() != 2 or t.stride(1) != 1:
+            raise TypeError("fp64 blocks must be 2-D with unit column stride")
+
+
+def csr_spmm_f64(csr, X, out=None):
+    """A X (eb_csr_spmm_f64) for csr = (indptr int64, indices int32, data fp32) of A and an fp64 X with one row per column
+    of A; every output element summed over its row's entries in stored order.  Returns out [rows of A][X.shape[1]]."""
+    indptr, indices, data = csr
+    _need_cuda(indptr, indices, data, X, out)
+    _chk_f64(X)
+    _chk_idx(indices)
+    assert indptr.dtype == torch.int64 and data.dtype == torch.float32 and indptr.is_contiguous() and data.is_contiguous()
+    n, w = indptr.numel() - 1, X.shape[1]
+    if out is None:
+        with torch.cuda.device(X.device):
+            out = torch.empty((n, w), dtype=torch.float64, device=X.device)
+    _chk_f64(out)
+    assert out.shape[0] == n and out.shape[1] >= w
+    indices, data = _nonempty(indices), _nonempty(data)
+    _call("eb_csr_spmm_f64", X, _ptr(indptr), _ptr(indices), _ptr(data), n, _ptr(X), w, X.stride(0), _ptr(out), out.stride(0))
+    return out
+
+
+def chol_pivoted_f64(G, M=None, rank=None):
+    """M = P L^-T from the pivoted Cholesky factorisation P^T G P = L L^T (eb_chol_pivoted_f64), columns past the
+    numerical rank zero.  `rank`: an optional int32 device tensor of one element that receives the rank."""
+    _need_cuda(G, M, rank)
+    w = G.shape[0]
+    assert G.dtype == torch.float64 and G.is_contiguous() and G.shape == (w, w)
+    if M is None:
+        with torch.cuda.device(G.device):
+            M = torch.empty((w, w), dtype=torch.float64, device=G.device)
+    assert M.dtype == torch.float64 and M.is_contiguous() and M.shape == (w, w)
+    assert rank is None or (rank.dtype == torch.int32 and rank.numel() >= 1)
+    _call("eb_chol_pivoted_f64", G, _ptr(G), w, _ptr(M), _ptr(rank))
+    return M
+
+
+def tall_times_small_f64(X, M, out=None):
+    """X M (eb_tall_times_small_f64) for a tall fp64 X [n][w] and a contiguous M [w][d]; `out` may be X itself when
+    d == w."""
+    _need_cuda(X, M, out)
+    _chk_f64(X)
+    n, w = X.shape
+    assert M.dtype == torch.float64 and M.is_contiguous() and M.shape[0] == w
+    d = M.shape[1]
+    if out is None:
+        with torch.cuda.device(X.device):
+            out = torch.empty((n, d), dtype=torch.float64, device=X.device)
+    _chk_f64(out)
+    assert out.shape[0] == n and out.shape[1] >= d
+    _call("eb_tall_times_small_f64", X, _ptr(X), n, w, X.stride(0), _ptr(M), d, _ptr(out), out.stride(0))
+    return out
+
+
+def sym_eig_f64(A):
+    """(eigenvalues descending [w], eigenvectors [w][w] by column) of a symmetric fp64 A (eb_sym_eig_f64, Jacobi)."""
+    _need_cuda(A)
+    w = A.shape[0]
+    assert A.dtype == torch.float64 and A.is_contiguous() and A.shape == (w, w)
+    with torch.cuda.device(A.device):
+        evals = torch.empty(w, dtype=torch.float64, device=A.device)
+        evecs = torch.empty((w, w), dtype=torch.float64, device=A.device)
+        ws = torch.empty(max(1, int(lib().eb_sym_eig_f64_workspace_bytes(w))), dtype=torch.uint8, device=A.device)
+    _call("eb_sym_eig_f64", A, _ptr(A), w, _ptr(evals), _ptr(evecs), _ptr(ws), ws.numel())
+    return evals, evecs
+
+
+def svd_finish_f64(evals, user, item, scale_user_by_inv_s):
+    """In place on the first d = user.shape[1] columns (eb_svd_finish_f64): the optional 1/s and s column scaling and
+    the sign of each user column's largest entry; returns s [d]."""
+    _need_cuda(evals, user, item)
+    _chk_f64(user, item)
+    d = user.shape[1]
+    assert evals.dtype == torch.float64 and evals.is_contiguous() and item.shape[1] == d
+    with torch.cuda.device(user.device):
+        s = torch.empty(d, dtype=torch.float64, device=user.device)
+    _call("eb_svd_finish_f64", user, _ptr(evals), evals.numel(), d, _ptr(user), user.shape[0], user.stride(0), _ptr(item),
+          item.shape[0], item.stride(0), int(bool(scale_user_by_inv_s)), _ptr(s))
+    return s
+
+
 # ---------------------------------------------------------------- NeuMF pieces (neumf.cu)
 def _call(name, dev_tensor, *args):
     with torch.cuda.device(dev_tensor.device):

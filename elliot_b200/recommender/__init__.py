@@ -12,3 +12,4 @@ from .als import iALS, WRMF, ALSModel  # noqa: F401
 from .ease import EASER, EASEModel  # noqa: F401
 from .rp3beta import RP3beta, RP3Model  # noqa: F401
 from .slim import Slim, SlimModel  # noqa: F401
+from .pure_svd import PureSVD, PureSVDModel  # noqa: F401

@@ -98,6 +98,12 @@ def slim_yaml(tsv, out_dir, extra="", model_extra=""):
                            extra=extra, model_extra=model_extra)
 
 
+def pure_svd_yaml(tsv, out_dir, extra="", model_extra=""):
+    """The PureSVD block of the reference's docstring (factors 10, seed 42) with save_recs."""
+    return experiment_yaml(tsv, out_dir, "PureSVD", "      factors: 10\n      seed: 42\n", extra=extra,
+                           model_extra=model_extra)
+
+
 def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra="", seed=42):
     """A `BPRMF:` block with BPRMF.py:43-56 keys, the reference's default hyper-parameters, save_recs and verbose off."""
     return experiment_yaml(tsv, out_dir, model_key, f"""      epochs: {epochs}

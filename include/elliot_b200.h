@@ -645,6 +645,39 @@ int eb_slim_fit_f32(const int64_t *colptr, const int32_t *rows, const float *val
                     void *stream);
 int eb_slim_drop_f32(int32_t n_items, const int32_t *drop, float *coef_t, void *stream);
 
+/* ------------------------------------------------------------------------
+ * PureSVD (latent_factor_models/PureSVD/pure_svd_model.py:36-43: sklearn's randomized_svd), fp64.  Widths w and d are at
+ * most eb_svd_max_width() (200, the limit of eb_gram_f64).
+ * eb_csr_spmm_f64: Y[n_rows][w] (row stride ldy) = A X for a CSR A (int64 indptr, int32 indices, fp32 data) and X (row
+ * stride ldx); element Y[r][c] is fma-summed over row r's entries in stored order from 0, so reruns are bit-identical.
+ * Y must not be X.
+ * eb_chol_pivoted_f64: for a symmetric positive semi-definite G[w][w] (G = X^T X), the Cholesky factorisation
+ * P^T G P = L L^T with diagonal pivoting (the largest remaining diagonal entry; ties: the lowest index), stopped at the
+ * first pivot <= w * 2^-52 * trace(G); writes M[w][w] = P L^-T with its columns past the numerical rank zero, and the rank
+ * to *rank when rank is not NULL.  X M then has orthonormal columns spanning X's column space, followed by zero columns.
+ * eb_tall_times_small_f64: Y[n][d] = X[n][w] M[w][d] (M row-major, row stride d), each element fma-summed over k in order.
+ * Y may be X when d == w and ldy == ldx; otherwise they must not overlap.
+ * eb_sym_eig_f64: eigenvalues (descending; ties: the lower diagonal index first) and eigenvectors (evecs[w][w], column k
+ * for evals[k]) of a symmetric A[w][w], by cyclic Jacobi rotations in the parallel order; a pair is rotated while
+ * |a_pq| > 2^-52 sqrt(|a_pp a_qq|) and |a_pq| > w 2^-52 sum_i |a_ii|.  workspace: at least
+ * eb_sym_eig_f64_workspace_bytes(w) bytes, else EB_ERR_WORKSPACE.  The call synchronises `stream`; EB_ERR_DATA when it
+ * does not converge.  Calls must not run concurrently on one device (they share the status word).
+ * eb_svd_finish_f64: for k < d: s_out[k] = sqrt(max(evals[k], 0)); when scale_user_by_inv_s, user column k is
+ * multiplied by 1 / s_out[k] (by 0 when evals[k] <= w * 2^-52 * sum_j max(evals[j], 0)) and item column k by s_out[k].
+ * Then both columns are multiplied by the sign of the user column's largest-|.| entry (the first such row; +1 when the
+ * column is zero), as sklearn's svd_flip does.
+ * ------------------------------------------------------------------------ */
+int eb_svd_max_width(void);
+int eb_csr_spmm_f64(const int64_t *indptr, const int32_t *indices, const float *data, int64_t n_rows, const double *X, int w,
+                    int64_t ldx, double *Y, int64_t ldy, void *stream);
+int eb_chol_pivoted_f64(const double *G, int w, double *M, int32_t *rank, void *stream);
+int eb_tall_times_small_f64(const double *X, int64_t n, int w, int64_t ldx, const double *M, int d, double *Y, int64_t ldy,
+                            void *stream);
+size_t eb_sym_eig_f64_workspace_bytes(int w);
+int eb_sym_eig_f64(const double *A, int w, double *evals, double *evecs, void *workspace, size_t workspace_bytes, void *stream);
+int eb_svd_finish_f64(const double *evals, int w, int d, double *user, int64_t n_user, int64_t ld_user, double *item,
+                      int64_t n_item, int64_t ld_item, int scale_user_by_inv_s, double *s_out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
