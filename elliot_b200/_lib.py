@@ -174,6 +174,9 @@ SIGNATURES = {
     "eb_sym_eig_f64_workspace_bytes": (c_size, [c_int]),
     "eb_sym_eig_f64": (c_int, [c_void, c_int, c_void, c_void, c_void, c_size, c_void]),
     "eb_svd_finish_f64": (c_int, [c_void, c_int, c_int, c_void, c_i64, c_i64, c_void, c_i64, c_i64, c_int, c_void, c_void]),
+    "eb_slope_one_dev_f64": (c_int, [c_void, c_void, c_void, c_i64, c_i32, c_i32, c_int, c_void, c_i64, c_void]),
+    "eb_slope_one_score_topk_f64": (c_int, [c_void, c_i64, c_i32, c_void, c_void, c_void, c_void, c_void, c_void, c_i32, c_i64,
+                                            c_int, c_void, c_void, c_void]),
 }
 
 _lib = None

@@ -997,6 +997,48 @@ def svd_finish_f64(evals, user, item, scale_user_by_inv_s):
     return s
 
 
+# ---------------------------------------------------------------- SlopeOne (slope_one.cu)
+def slope_one_dev_f64(F, M1, M2, n, s, out=None):
+    """E rows = ((M1 - M2) 2^-s) / F in fp64, NaN where F = 0 (eb_slope_one_dev_f64), for fp32 slabs F, M1, M2 [rows][>= n]
+    of one layout.  `out`: fp64 [rows][>= n] with unit column stride, e.g. a row range of the full E."""
+    _need_cuda(F, M1, M2, out)
+    for t in (F, M1, M2):
+        assert t.dtype == torch.float32 and t.stride(1) == 1 and t.stride(0) == F.stride(0) and t.shape[0] == F.shape[0]
+    rows = F.shape[0]
+    if out is None:
+        with torch.cuda.device(F.device):
+            out = torch.empty((rows, n), dtype=torch.float64, device=F.device)
+    assert out.dtype == torch.float64 and out.stride(1) == 1 and out.shape[0] == rows and out.shape[1] >= n
+    _call("eb_slope_one_dev_f64", F, _ptr(F), _ptr(M1), _ptr(M2), F.stride(0), rows, n, int(s), _ptr(out), out.stride(0))
+    return out
+
+
+def slope_one_score_topk(E, train, k, mask_indptr=None, mask_indices=None, users=None, user_begin=0, n_sel=None):
+    """Top k of the SlopeOne scores (eb_slope_one_score_topk_f64): E fp64 [n_items][>= n_items], train = (indptr int64,
+    items int32, ratings fp32) with each user's items in summation order.  Returns (idx int32 [n_sel][k], val fp64
+    [n_sel][k]), (score desc, item asc), -1 / -inf padded."""
+    indptr, items, ratings = train
+    _need_cuda(E, indptr, items, ratings, mask_indptr, mask_indices, users)
+    assert E.dtype == torch.float64 and E.stride(1) == 1
+    assert indptr.dtype == torch.int64 and ratings.dtype == torch.float32 and ratings.is_contiguous()
+    _chk_idx(items)
+    if users is not None:
+        _chk_idx(users)
+        n_sel = users.numel()
+    elif n_sel is None:
+        n_sel = indptr.numel() - 1 - user_begin
+    with torch.cuda.device(E.device):
+        idx = torch.empty((n_sel, k), dtype=torch.int32, device=E.device)
+        val = torch.empty((n_sel, k), dtype=torch.float64, device=E.device)
+    items, ratings = _nonempty(items), _nonempty(ratings)
+    if mask_indices is not None:
+        _chk_idx(mask_indices)
+        mask_indices = _nonempty(mask_indices)
+    _call("eb_slope_one_score_topk_f64", E, _ptr(E), E.stride(0), E.shape[0], _ptr(indptr), _ptr(items), _ptr(ratings),
+          _ptr(mask_indptr), _ptr(mask_indices), _ptr(users), user_begin, n_sel, k, _ptr(idx), _ptr(val))
+    return idx, val
+
+
 # ---------------------------------------------------------------- NeuMF pieces (neumf.cu)
 def _call(name, dev_tensor, *args):
     with torch.cuda.device(dev_tensor.device):

@@ -104,6 +104,11 @@ def pure_svd_yaml(tsv, out_dir, extra="", model_extra=""):
                            model_extra=model_extra)
 
 
+def slope_one_yaml(tsv, out_dir, extra="", model_extra=""):
+    """The SlopeOne block of the reference's docstring (no parameters) with save_recs."""
+    return experiment_yaml(tsv, out_dir, "SlopeOne", "", extra=extra, model_extra=model_extra)
+
+
 def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra="", seed=42):
     """A `BPRMF:` block with BPRMF.py:43-56 keys, the reference's default hyper-parameters, save_recs and verbose off."""
     return experiment_yaml(tsv, out_dir, model_key, f"""      epochs: {epochs}

@@ -678,6 +678,26 @@ int eb_sym_eig_f64(const double *A, int w, double *evals, double *evecs, void *w
 int eb_svd_finish_f64(const double *evals, int w, int d, double *user, int64_t n_user, int64_t ld_user, double *item,
                       int64_t n_item, int64_t ld_item, int scale_user_by_inv_s, double *s_out, void *stream);
 
+/* ------------------------------------------------------------------------
+ * SlopeOne (algebric/slope_one/slope_one_model.py:19-64), fp64.
+ * eb_slope_one_dev_f64: for a row slab of the exact fp32 products F = B^T B, M1 = X^T B and M2 = B^T X (row stride
+ * ld_in; X the ratings times 2^s, B the entry pattern, every entry an integer below 2^24), E[r][c] (row stride lde) =
+ * ((double)M1 - (double)M2) * 2^-s / (double)F, divided with round-to-nearest, and NaN where F = 0.  0 <= s <= 30.
+ * eb_slope_one_score_topk_f64: for output row q (user users[q], or user_begin + q when users is NULL), with the user's
+ * train items j and ratings taken from the CSR indptr / items / ratings in stored order: mean = (sum of the ratings) / n
+ * (the sum must be exact in fp64, as it is for ratings times 2^s that are integers), and for every item c the sum of
+ * -E[j][c] over the j in stored order (sequential fp64 additions from 0, NaN entries skipped), divided by the number of
+ * terms summed, plus the mean (the mean alone when there are none).  Items of the mask CSR (any order) are excluded; the
+ * k best by (score desc, item asc) go to out_idx/out_val [n_sel][k], padded with -1 / -inf when fewer than k items are
+ * left.  1 <= k <= 1024.  No workspace: the scores of one column tile live in shared memory.
+ * ------------------------------------------------------------------------ */
+int eb_slope_one_dev_f64(const float *F, const float *M1, const float *M2, int64_t ld_in, int32_t n_rows, int32_t n, int s,
+                         double *E, int64_t lde, void *stream);
+int eb_slope_one_score_topk_f64(const double *E, int64_t lde, int32_t n_items, const int64_t *indptr, const int32_t *items,
+                                const float *ratings, const int64_t *mask_indptr, const int32_t *mask_indices,
+                                const int32_t *users, int32_t user_begin, int64_t n_sel, int k, int32_t *out_idx,
+                                double *out_val, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
