@@ -177,6 +177,11 @@ SIGNATURES = {
     "eb_slope_one_dev_f64": (c_int, [c_void, c_void, c_void, c_i64, c_i32, c_i32, c_int, c_void, c_i64, c_void]),
     "eb_slope_one_score_topk_f64": (c_int, [c_void, c_i64, c_i32, c_void, c_void, c_void, c_void, c_void, c_void, c_i32, c_i64,
                                             c_int, c_void, c_void, c_void]),
+    "eb_nnmf_dots_f64": (c_int, [c_void, c_void, c_int, c_void, c_void, c_i32, c_void, c_void]),
+    "eb_nnmf_bias_chain_f64": (c_int, [c_void, c_void, c_void, c_void, c_i32, c_i32, c_f64, c_f64, c_f64, c_void, c_void,
+                                       c_void, c_void]),
+    "eb_nnmf_row_update_f64": (c_int, [c_void, c_void, c_void, c_i32, c_void, c_void, c_void, c_void, c_void, c_int, c_f64,
+                                       c_void]),
 }
 
 _lib = None

@@ -1039,6 +1039,60 @@ def slope_one_score_topk(E, train, k, mask_indptr=None, mask_indices=None, users
     return idx, val
 
 
+# ---------------------------------------------------------------- NonNegMF (nonneg_mf.cu)
+def _chk_f64(*ts):
+    for t in ts:
+        assert t.dtype == torch.float64 and t.is_contiguous()
+
+
+def nnmf_dots_f64(P, Q, indptr, items, out=None):
+    """dot_k = Q[i_k] . P[u_k] for every rating k of the CSR (indptr int64, items int32), summed in f order from +0.0
+    (eb_nnmf_dots_f64).  P [n_users][F] and Q [n_items][F] fp64, contiguous."""
+    _need_cuda(P, Q, indptr, items, out)
+    _chk_f64(P, Q)
+    _chk_idx(items)
+    assert indptr.dtype == torch.int64 and P.shape[1] == Q.shape[1] and indptr.numel() == P.shape[0] + 1
+    if out is None:
+        with torch.cuda.device(P.device):
+            out = torch.empty(items.numel(), dtype=torch.float64, device=P.device)
+    _chk_f64(out)
+    _call("eb_nnmf_dots_f64", P, _ptr(P), _ptr(Q), P.shape[1], _ptr(indptr), _ptr(items), P.shape[0], _ptr(out))
+    return out
+
+
+def nnmf_bias_chain_f64(indptr, items, ratings, dots, mu, lr, reg, bu, bi, out=None):
+    """est_k for every rating k in order, updating bu and bi in place as the reference's loop does
+    (eb_nnmf_bias_chain_f64).  ratings, dots, bu, bi: fp64 contiguous."""
+    _need_cuda(indptr, items, ratings, dots, bu, bi, out)
+    _chk_f64(ratings, dots, bu, bi)
+    _chk_idx(items)
+    assert indptr.dtype == torch.int64 and indptr.numel() == bu.numel() + 1
+    if out is None:
+        with torch.cuda.device(bu.device):
+            out = torch.empty(items.numel(), dtype=torch.float64, device=bu.device)
+    _chk_f64(out)
+    _call("eb_nnmf_bias_chain_f64", bu, _ptr(indptr), _ptr(items), _ptr(ratings), _ptr(dots), bu.numel(), bi.numel(),
+          float(mu), float(lr), float(reg), _ptr(bu), _ptr(bi), _ptr(out))
+    return out
+
+
+def nnmf_row_update_f64(indptr, cols, pos, ratings, est, T, S, reg, out=None):
+    """S * (num / den) row by row (eb_nnmf_row_update_f64): num and den the ordered sums of T[col] * r_k and
+    T[col] * est_k over each row's entries (k = pos[e], or e when pos is None), den + (n reg) S.  `out` may be S."""
+    _need_cuda(indptr, cols, pos, ratings, est, T, S, out)
+    _chk_f64(ratings, est, T, S)
+    _chk_idx(cols)
+    assert indptr.dtype == torch.int64 and indptr.numel() == S.shape[0] + 1 and T.shape[1] == S.shape[1]
+    assert pos is None or (pos.dtype == torch.int64 and pos.is_contiguous())
+    if out is None:
+        with torch.cuda.device(S.device):
+            out = torch.empty_like(S)
+    _chk_f64(out)
+    _call("eb_nnmf_row_update_f64", S, _ptr(indptr), _ptr(cols), _ptr(pos), S.shape[0], _ptr(ratings), _ptr(est), _ptr(T),
+          _ptr(S), _ptr(out), S.shape[1], float(reg))
+    return out
+
+
 # ---------------------------------------------------------------- NeuMF pieces (neumf.cu)
 def _call(name, dev_tensor, *args):
     with torch.cuda.device(dev_tensor.device):

@@ -14,3 +14,4 @@ from .rp3beta import RP3beta, RP3Model  # noqa: F401
 from .slim import Slim, SlimModel  # noqa: F401
 from .pure_svd import PureSVD, PureSVDModel  # noqa: F401
 from .slope_one import SlopeOne, SlopeOneModel  # noqa: F401
+from .nonneg_mf import NonNegMF, NonNegMFModel  # noqa: F401

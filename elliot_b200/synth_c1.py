@@ -109,6 +109,13 @@ def slope_one_yaml(tsv, out_dir, extra="", model_extra=""):
     return experiment_yaml(tsv, out_dir, "SlopeOne", "", extra=extra, model_extra=model_extra)
 
 
+def nonneg_mf_yaml(tsv, out_dir, extra="", model_extra=""):
+    """The NonNegMF block of the reference's docstring (epochs 10, batch_size 512, factors 10, lr 0.001, reg 0.1) with
+    save_recs."""
+    return experiment_yaml(tsv, out_dir, "NonNegMF", "      epochs: 10\n      batch_size: 512\n      factors: 10\n"
+                           "      lr: 0.001\n      reg: 0.1\n", extra=extra, model_extra=model_extra)
+
+
 def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra="", seed=42):
     """A `BPRMF:` block with BPRMF.py:43-56 keys, the reference's default hyper-parameters, save_recs and verbose off."""
     return experiment_yaml(tsv, out_dir, model_key, f"""      epochs: {epochs}

@@ -698,6 +698,31 @@ int eb_slope_one_score_topk_f64(const double *E, int64_t lde, int32_t n_items, c
                                 const int32_t *users, int32_t user_begin, int64_t n_sel, int k, int32_t *out_idx,
                                 double *out_val, void *stream);
 
+/* ------------------------------------------------------------------------
+ * NonNegMF (latent_factor_models/NonNegMF/non_negative_matrix_factorization_model.py:42-84), fp64, one epoch in three
+ * steps; every product, sum and quotient is rounded on its own (no FMA), so the results equal the reference's bit for
+ * bit.  The ratings k are those of a CSR indptr [n_users + 1] / items (users ascending, each user's items in the
+ * reference's dict order); P [n_users][F] and Q [n_items][F] are dense with row stride F.
+ * eb_nnmf_dots_f64: dots[k] = sum over f = 0..F-1 of Q[i][f] * P[u][f], summed in f order from +0.0.
+ * eb_nnmf_bias_chain_f64: for k in order: est[k] = ((mu + bu[u]) + bi[i]) + dots[k], err = ratings[k] - est[k],
+ *   bu[u] += lr * (err - reg * bu[u]), then bi[i] += lr * (err - reg * bi[i]).  bu and bi are updated in place; bu of a
+ *   user without ratings is unchanged.  One thread walks the ratings; bi is staged in shared memory when n_items doubles
+ *   fit the device's opt-in dynamic shared memory, and read and written in global memory otherwise.
+ * eb_nnmf_row_update_f64: for every row r and f < F, over the row's entries e in stored order (k = pos[e], or e when
+ *   pos is NULL): num = sum T[cols[e]][f] * ratings[k], den = sum T[cols[e]][f] * est[k], both from +0.0; then
+ *   den += (n * reg) * S[r][f] with n the row's entry count, and S_out[r][f] = S[r][f] * (num / den) (IEEE inf / NaN
+ *   when den is 0).  S_out may be S; it must not be T.  The user side passes the CSR above with T = Q, S = P; the item
+ *   side the CSC (items' entries in ascending user order) with pos = each entry's k, T = P, S = Q.
+ * ------------------------------------------------------------------------ */
+int eb_nnmf_dots_f64(const double *P, const double *Q, int F, const int64_t *indptr, const int32_t *items, int32_t n_users,
+                     double *dots, void *stream);
+int eb_nnmf_bias_chain_f64(const int64_t *indptr, const int32_t *items, const double *ratings, const double *dots,
+                           int32_t n_users, int32_t n_items, double mu, double lr, double reg, double *bu, double *bi,
+                           double *est, void *stream);
+int eb_nnmf_row_update_f64(const int64_t *indptr, const int32_t *cols, const int64_t *pos, int32_t n_rows,
+                           const double *ratings, const double *est, const double *T, const double *S, double *S_out, int F,
+                           double reg, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
