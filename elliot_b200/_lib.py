@@ -104,6 +104,9 @@ SIGNATURES = {
     "eb_eval_topk_workspace_bytes": (c_size, [c_i64, c_int]),
     "eb_eval_topk_f64": (c_int, [c_void, c_i64, c_int, c_int, c_void, c_void, c_void, c_void, c_void, c_void, c_void, c_void,
                          c_void, c_size, c_void]),
+    "eb_eval_metrics_workspace_bytes": (c_size, [c_i64, c_int, c_int]),
+    "eb_eval_metrics_f64": (c_int, [c_void, c_i64, c_int, c_int, c_void, c_void, c_void, c_void, c_void, c_void, c_void,
+                            c_int, c_void, c_void, c_void, c_void, c_void, c_void, c_size, c_void]),
     "eb_partition_streams_create": (c_int, [c_int, c_int, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(c_int)]),
     "eb_table_apply_delta_late_f32": (c_int, [c_void, c_void, c_void, c_void, c_i64, c_f32, c_void]),
     "eb_gmf_step_grads": (c_int, [c_void, c_void, c_i64, c_int, c_void, c_void, c_void, c_void, c_i64, c_i64, c_void, c_void, c_void,

@@ -240,3 +240,17 @@ def eval_csr_of(data, which="test"):
                 gain.append(2 ** (score - thr + 1) - 1)              # relevance.py:80-82
         indptr[pu + 1] = len(idx)
     return indptr, np.array(idx, np.int64), np.array(gain, np.float64)
+
+
+def eval_users_of(data, which="test"):
+    """Boolean mask over private users: the user has any row in the split, whatever its rating (the users the reference
+    Evaluator keeps, evaluator.py:117); None when the split does not exist."""
+    if hasattr(data, "eval_arrays"):                                  # the mirror: no dicts
+        arr = data.eval_arrays(which)
+        if arr is None:
+            return None
+        return np.bincount(arr[0], minlength=len(data.users)) > 0
+    d = data.test_dict if which == "test" else getattr(data, "val_dict", None)
+    if d is None:
+        return None
+    return np.array([bool(d.get(u)) for u in data.users], dtype=bool)

@@ -1234,6 +1234,48 @@ def eval_topk(topk_idx, k, rel_indptr, rel_items, rel_gains, idcg, discount, use
     return out, pu
 
 
+_eval_metrics_ws = None
+EVAL_METRICS_SLOTS = 29
+EVAL_METRICS_PER_USER = ("nDCGRendle2020", "MRR", "MAP", "MAR", "F1", "LAUC", "NumRetrieved", "EPC", "EFD", "ARP", "APLT",
+                         "ACLT")
+
+
+def eval_topk_metrics(topk_idx, k, rel_indptr, rel_items, user_info, item_pop, item_long_tail, item_novelty, discount,
+                      map_tail, inv_binary_idcg, users=None, per_user=False):
+    """The reference's ranking, novelty, popularity-bias, coverage and diversity metrics of a (rows x >=k) int32 top-k
+    index tensor (eval_metrics.cu; tables as in include/elliot_b200.h).  Returns (out, per_user): out = device
+    double[29] of counts, sums and numerators; per_user = (rows x 12) in EVAL_METRICS_PER_USER order, or None."""
+    global _eval_metrics_ws
+    _need_cuda(topk_idx, rel_indptr, rel_items, user_info, item_pop, item_long_tail, item_novelty, discount, map_tail,
+               inv_binary_idcg, users)
+    assert topk_idx.dtype == torch.int32 and topk_idx.stride(1) == 1 and topk_idx.shape[1] >= k
+    assert rel_indptr.dtype == torch.int64 and rel_items.dtype == torch.int32
+    assert user_info.dtype == torch.int32 and user_info.is_contiguous() and user_info.shape[1:] == (6,)
+    assert user_info.shape[0] == rel_indptr.numel() - 1
+    n_items = item_pop.numel()
+    assert item_pop.dtype == torch.int32 and item_long_tail.dtype == torch.uint8 and item_long_tail.numel() == n_items
+    assert item_novelty.dtype == torch.float64 and item_novelty.is_contiguous() and item_novelty.shape == (n_items, 2)
+    for t in (discount, map_tail, inv_binary_idcg):
+        assert t.dtype == torch.float64 and t.is_contiguous()
+    assert discount.numel() >= k and map_tail.numel() >= k and inv_binary_idcg.numel() >= k + 1
+    n = topk_idx.shape[0]
+    if users is not None:
+        _chk_idx(users); assert users.numel() == n
+    dev = topk_idx.device
+    out = torch.empty(EVAL_METRICS_SLOTS, dtype=torch.float64, device=dev)
+    pu = torch.empty(n, len(EVAL_METRICS_PER_USER), dtype=torch.float64, device=dev) if per_user else None
+    need = lib().eb_eval_metrics_workspace_bytes(n, k, n_items)
+    if _eval_metrics_ws is None or _eval_metrics_ws.numel() < need or _eval_metrics_ws.device != dev:
+        _eval_metrics_ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        check(lib().eb_eval_metrics_f64(_ptr(topk_idx), n, topk_idx.stride(0), k, _ptr(users), _ptr(rel_indptr),
+                                        _ptr(rel_items), _ptr(user_info), _ptr(item_pop), _ptr(item_long_tail),
+                                        _ptr(item_novelty), n_items, _ptr(discount), _ptr(map_tail), _ptr(inv_binary_idcg),
+                                        _ptr(pu), _ptr(out), _ptr(_eval_metrics_ws), _eval_metrics_ws.numel(),
+                                        _stream(topk_idx)))
+    return out, pu
+
+
 def partition_streams(device, reserve_sms, n_streams=1):
     """Streams bound to a green context that leaves >= reserve_sms SMs of `device` free (partition.cu).
     Returns (list of torch streams, SMs in the partition)."""

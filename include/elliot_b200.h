@@ -357,6 +357,33 @@ int eb_eval_topk_f64(const int32_t *topk_idx, int64_t n_rows, int ld, int k, con
                      const double *idcg, const double *discount, double *per_user, double *out,
                      void *workspace, size_t workspace_bytes, void *stream);
 
+/* ------------------------------------------------------------------------
+ * The reference's other list metrics, on the device (elliot/evaluation/metrics): nDCGRendle2020, MRR, MAP, MAR, F1,
+ * LAUC, NumRetrieved, EPC, EFD, ARP, APLT, ACLT, PopREO, PopRSP, ItemCoverage, UserCoverage, UserCoverageAtN, Gini,
+ * SEntropy.  topk_idx / ld / k / users as for eb_eval_topk_f64; a row's list is its entries before the first -1.
+ * rel_indptr/rel_items: the item-sorted relevant CSR of eb_eval_topk_f64 (gains are not needed: relevance is binary).
+ * user_info[n_users][6] int32: has any test row, |train_u|, PopREO denominators (short head, long tail: relevant items
+ * not in train_u), PopRSP denominators (|short head - train_u|, |long tail - train_u|).  Per private item: item_pop
+ * (train users), item_long_tail (1 = long tail, 0 = short head), item_novelty[n_items][2] (EPC, EFD novelty).
+ * Per position r < k: discount[r] = ln2/ln(r+2), map_tail[r] = H(k) - H(r); inv_binary_idcg[m] (m = 1..k) = 1 / sum_{i<m}
+ * discount[i].  Rows whose user has no test row are skipped; the accuracy and novelty sums also skip users without a
+ * relevant item.  Lists must hold distinct items.
+ * out[29] (device, fp64, deterministic): {users with a relevant item, sums of nDCGRendle2020 MRR MAP MAR F1 LAUC
+ * NumRetrieved EPC EFD, PopREO hits in short head / long tail, PopREO denominators (2), users with test rows, sums of
+ * ARP APLT ACLT, PopRSP numerators (2), PopRSP denominators (2), UserCoverage, UserCoverageAtN, sum of list lengths,
+ * users with test rows and an empty list, ItemCoverage, Gini rank sum sum_j j*cs_j over the ascending item counts,
+ * SEntropy sum_u (1/n_u) sum_i -log2(c_i / sum n_u)}.
+ * per_user (optional, device double[n_rows][12]): nDCGRendle2020 MRR MAP MAR F1 LAUC NumRetrieved EPC EFD ARP APLT
+ * ACLT per row, NaN where the reference has no value for the user.
+ * ------------------------------------------------------------------------ */
+size_t eb_eval_metrics_workspace_bytes(int64_t n_rows, int k, int n_items);
+int eb_eval_metrics_f64(const int32_t *topk_idx, int64_t n_rows, int ld, int k, const int32_t *users,
+                        const int64_t *rel_indptr, const int32_t *rel_items, const int32_t *user_info,
+                        const int32_t *item_pop, const uint8_t *item_long_tail, const double *item_novelty,
+                        int n_items, const double *discount, const double *map_tail,
+                        const double *inv_binary_idcg, double *per_user, double *out, void *workspace,
+                        size_t workspace_bytes, void *stream);
+
 /* SM partition for compute/collective overlap (no reference counterpart): creates a green context holding
  * all but >= reserve_sms SMs of the current device (rounded to the driver's 8-SM granularity) and n_streams
  * CUDA streams bound to it.  Kernels launched on those streams run only inside the partition, so a collective
