@@ -2,9 +2,11 @@
 all arithmetic happens in elliot_b200/csrc/*.cu.  Every op raises if its tensors are not on a
 CUDA device — there is no CPU path.
 
-Streams: every op launches on torch's CURRENT stream of the tensors' device.  The C ABI never allocates, so a few
-wrappers keep a grow-only scratch buffer per device (scoring, evaluation, the native MultiVAE step, the MF2020
-global-bias accumulator): those ops must not run concurrently on two streams of the same device from one process.
+Streams: every op launches on torch's CURRENT stream of the tensors' device.  The C ABI never allocates, so these ops
+keep grow-only scratch per device from call to call (_scratch): bpr_exact_f64, MtSampler.step, score_topk,
+score_topk_tc, bpr_step_sampled_f32 (the schedule prefetch keeps two schedule slots of its own), gram_f64, eval_topk,
+eval_topk_metrics and vae_train_step; mf_pointwise_step_f32 keeps a global-bias accumulator per device.  Those ops must
+not run concurrently on two streams of the same device from one process.
 """
 import ctypes
 import os
@@ -44,6 +46,72 @@ def _chk_idx(*ts):
             raise TypeError("index tensors must be contiguous int32")
 
 
+def _chk_f64_rows(*ts):
+    """fp64 row blocks: 2-D with unit column stride, so row-strided views pass."""
+    for t in ts:
+        if t.dtype != torch.float64 or t.dim() != 2 or t.stride(1) != 1:
+            raise TypeError("fp64 blocks must be 2-D with unit column stride")
+
+
+def _chk_f64_dense(*ts):
+    """fp64 dense arrays: contiguous."""
+    for t in ts:
+        assert t.dtype == torch.float64 and t.is_contiguous()
+
+
+def _nonempty(t):
+    """The C ABI takes no NULL arrays: an empty one is passed as a one-element dummy."""
+    return t if t.numel() else torch.zeros(1, dtype=t.dtype, device=t.device)
+
+
+def _call(name, dev_tensor, *args):
+    """Entry point `name` on dev_tensor's device, with that device's current stream appended as the last argument."""
+    with torch.cuda.device(dev_tensor.device):
+        check(getattr(lib(), name)(*args, _stream(dev_tensor)))
+
+
+_scratch_bufs = {}
+
+
+def _scratch(name, nbytes, device):
+    """Grow-only device scratch of at least nbytes (and 256) bytes, one buffer per (name, device) kept from call to call;
+    only ever used on the caller's current stream."""
+    key = (name, device.index)
+    buf = _scratch_bufs.get(key)
+    if buf is None or buf.numel() < nbytes:
+        buf = _scratch_bufs[key] = torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=device)
+    return buf
+
+
+def _topk_out(users, n_rows, user_begin, n_sel, k, dtype, device):
+    """(n_sel, idx int32 [n_sel][k], val [n_sel][k]) of a top-k over the int32 ids `users`, or else over the rows
+    user_begin .. user_begin + n_sel (n_sel None: to the last of n_rows rows)."""
+    if users is not None:
+        _chk_idx(users)
+        n_sel = users.numel()
+    elif n_sel is None:
+        n_sel = n_rows - user_begin
+    return (n_sel, torch.empty((n_sel, k), dtype=torch.int32, device=device),
+            torch.empty((n_sel, k), dtype=dtype, device=device))
+
+
+def _bpr_flags(racy=False, sync=True, no_item_updates=False, variant=0, deterministic=False, reserve_sms=0):
+    """The flags word of the eb_bpr_step_* entry points: bit 0 plain stores (racy Hogwild), bit 1 no synchronise (host
+    triples), bit 2 no item-row updates, bits 4-5 kernel variant (16 or 32), bit 6 deterministic rounds, bits 8-15 SMs
+    the grid leaves free."""
+    return ((1 if racy else 0) | (0 if sync else 2) | (4 if no_item_updates else 0) | int(variant)
+            | (64 if deterministic else 0) | ((int(reserve_sms) & 0xff) << 8))
+
+
+def _out_ptrs(out):
+    """Device pointers of an optional out=(u, i, j) triple of contiguous int32 tensors (NULLs when out is None)."""
+    if out is None:
+        return 0, 0, 0
+    u, i, j = out
+    _need_cuda(u, i, j); _chk_idx(u, i, j)
+    return _ptr(u), _ptr(i), _ptr(j)
+
+
 def device_info():
     sm = ctypes.c_int(0); cc = ctypes.c_int(0)
     check(lib().eb_device_info(ctypes.byref(sm), ctypes.byref(cc)))
@@ -56,10 +124,8 @@ def bpr_step_f32(U, V, b, d, tu, ti, tj, lr, reg_u, reg_b, reg_pos, reg_neg, los
     _chk_idx(tu, ti, tj)
     assert U.dtype == torch.float32 and V.dtype == torch.float32 and b.dtype == torch.float32
     assert U.stride(1) == 1 and V.stride(1) == 1 and U.stride(0) == V.stride(0)
-    with torch.cuda.device(U.device):
-        check(lib().eb_bpr_step_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), _ptr(tu), _ptr(ti), _ptr(tj), tu.numel(),
-                                    lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), (1 if racy else 0) | (64 if deterministic else 0),
-                                    _stream(U)))
+    _call("eb_bpr_step_f32", U, _ptr(U), _ptr(V), _ptr(b), d, U.stride(0), _ptr(tu), _ptr(ti), _ptr(tj), tu.numel(), lr, reg_u,
+          reg_b, reg_pos, reg_neg, _ptr(loss), _bpr_flags(racy=racy, deterministic=deterministic))
 
 
 def bloom_build(indptr, indices, n_users, words=32):
@@ -68,8 +134,7 @@ def bloom_build(indptr, indices, n_users, words=32):
     _need_cuda(indptr, indices)
     assert indptr.dtype == torch.int64 and indices.dtype == torch.int32
     out = torch.empty((n_users, words), dtype=torch.int32, device=indptr.device)
-    with torch.cuda.device(indptr.device):
-        check(lib().eb_bloom_build(_ptr(indptr), _ptr(indices), n_users, words, _ptr(out), _stream(indptr)))
+    _call("eb_bloom_build", indptr, _ptr(indptr), _ptr(indices), n_users, words, _ptr(out))
     return out
 
 
@@ -87,25 +152,20 @@ def bpr_step_sampled_f32(U, V, b, d, n_users, n_items, indptr, indices, n, seed,
     exists for sharded item tables only and is refused here."""
     _need_cuda(U, V, b, indptr, indices, loss, filter)
     assert indptr.dtype == torch.int64 and indices.dtype == torch.int32
-    ou = oi = oj = None
-    if out is not None:
-        ou, oi, oj = out
-        _need_cuda(ou, oi, oj); _chk_idx(ou, oi, oj)
-    flags = (1 if racy else 0) | (64 if deterministic else 0) | ((int(reserve_sms) & 0xff) << 8) | int(_variant)
+    out = _out_ptrs(out)
+    flags = _bpr_flags(racy=racy, variant=_variant, deterministic=deterministic, reserve_sms=reserve_sms)
     fw = 0 if filter is None else filter.shape[1]
     if _prefetch_on and not deterministic and not _variant and 1 <= n <= _SCHEDULE_MAX:
         with torch.cuda.device(U.device):
             _schedules_of(U.device).step(U, V, b, d, n_users, n_items, indptr, indices, filter, fw, n, seed, first,
-                                         (lr, reg_u, reg_b, reg_pos, reg_neg), loss, (ou, oi, oj), flags)
+                                         (lr, reg_u, reg_b, reg_pos, reg_neg), loss, out, flags)
         return
     ws = None
     if not deterministic:
-        ws = _ws_grouped.get(lib().eb_bpr_step_sampled_workspace_bytes(n, n_users), U.device)
-    with torch.cuda.device(U.device):
-        check(lib().eb_bpr_step_sampled_filter_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), n_users, n_items, _ptr(indptr),
-                                                   _ptr(indices), _ptr(filter), fw, n, seed,
-                                                   first, lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), _ptr(ou), _ptr(oi),
-                                                   _ptr(oj), _ptr(ws), 0 if ws is None else ws.numel(), flags, _stream(U)))
+        ws = _scratch("bpr_grouped", lib().eb_bpr_step_sampled_workspace_bytes(n, n_users), U.device)
+    _call("eb_bpr_step_sampled_filter_f32", U, _ptr(U), _ptr(V), _ptr(b), d, U.stride(0), n_users, n_items, _ptr(indptr),
+          _ptr(indices), _ptr(filter), fw, n, seed, first, lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), *out, _ptr(ws),
+          0 if ws is None else ws.numel(), flags)
 
 
 # ---- schedule prefetch of the grouped sampled step
@@ -192,8 +252,8 @@ class _Schedules:
             self.ready.record(st)
         order = self.buf[s].data_ptr() + self.off[s]
         check(lib().eb_bpr_apply_sampled_filter_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), n_users, n_items, _ptr(indptr),
-                                                    _ptr(indices), _ptr(filt), fw, n, seed, first, *hp, _ptr(loss),
-                                                    *(_ptr(x) for x in out), order, flags, st.cuda_stream))
+                                                    _ptr(indices), _ptr(filt), fw, n, seed, first, *hp, _ptr(loss), *out, order,
+                                                    flags, st.cuda_stream))
         self.read[s].record(st)
         self.cur, self.last = s, (first, n)
         if ahead:
@@ -209,10 +269,8 @@ def bpr_sample_philox(n_users, n_items, indptr, indices, n, seed, first=0, filte
     _need_cuda(indptr, indices, filter)
     dev = indptr.device
     u = torch.empty(n, dtype=torch.int32, device=dev); i = torch.empty_like(u); j = torch.empty_like(u)
-    with torch.cuda.device(dev):
-        check(lib().eb_bpr_sample_philox_filter(n_users, n_items, _ptr(indptr), _ptr(indices), _ptr(filter),
-                                                0 if filter is None else filter.shape[1], n, seed, first, _ptr(u), _ptr(i), _ptr(j),
-                                                _stream(indptr)))
+    _call("eb_bpr_sample_philox_filter", indptr, n_users, n_items, _ptr(indptr), _ptr(indices), _ptr(filter),
+          0 if filter is None else filter.shape[1], n, seed, first, _ptr(u), _ptr(i), _ptr(j))
     return u, i, j
 
 
@@ -222,11 +280,9 @@ def bpr_step_host_f32(U, V, b, d, tu_host, ti_host, tj_host, lr, reg_u, reg_b, r
     _need_cuda(U, V, b, staging, loss_dev)
     n = tu_host.numel()
     assert not tu_host.is_cuda and tu_host.dtype == torch.int32 and staging.numel() >= 3 * n
-    with torch.cuda.device(U.device):
-        check(lib().eb_bpr_step_host_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), _ptr(tu_host), _ptr(ti_host),
-                                         _ptr(tj_host), n, lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(staging),
-                                         _ptr(loss_dev), _ptr(loss_host), (1 if racy else 0) | (0 if sync else 2) | ((int(reserve_sms) & 0xff) << 8),
-                                         _stream(U)))
+    _call("eb_bpr_step_host_f32", U, _ptr(U), _ptr(V), _ptr(b), d, U.stride(0), _ptr(tu_host), _ptr(ti_host), _ptr(tj_host), n,
+          lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(staging), _ptr(loss_dev), _ptr(loss_host),
+          _bpr_flags(racy=racy, sync=sync, reserve_sms=reserve_sms))
 
 
 def pack_bits(n_users, n_items):
@@ -251,25 +307,8 @@ def bpr_step_host_packed_f32(U, V, b, d, packed_host, n_users, n_items, lr, reg_
     n = packed_host.numel()
     assert not packed_host.is_cuda and packed_host.dtype == torch.int64 and staging.dtype == torch.int64 and staging.numel() >= n
     bu, bi = pack_bits(n_users, n_items)
-    with torch.cuda.device(U.device):
-        check(lib().eb_bpr_step_host_packed_f32(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), _ptr(packed_host), n, bu, bi,
-                                                lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(staging), _ptr(loss_dev), _ptr(loss_host),
-                                                (0 if sync else 2) | ((int(reserve_sms) & 0xff) << 8), _stream(U)))
-
-
-class _Workspace:
-    """Grow-only device scratch buffer (the C ABI never allocates)."""
-
-    def __init__(self):
-        self.buf = None
-
-    def get(self, nbytes, device):
-        if self.buf is None or self.buf.numel() < nbytes or self.buf.device != device:
-            self.buf = torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=device)
-        return self.buf
-
-
-_ws_exact, _ws_sampler, _ws_score, _ws_grouped = _Workspace(), _Workspace(), _Workspace(), _Workspace()
+    _call("eb_bpr_step_host_packed_f32", U, _ptr(U), _ptr(V), _ptr(b), d, U.stride(0), _ptr(packed_host), n, bu, bi, lr, reg_u,
+          reg_b, reg_pos, reg_neg, _ptr(staging), _ptr(loss_dev), _ptr(loss_host), _bpr_flags(sync=sync, reserve_sms=reserve_sms))
 
 
 def bpr_exact_f64(U, V, b, d, tu, ti, tj, lr, reg_u, reg_b, reg_pos, reg_neg, loss=None):
@@ -279,11 +318,9 @@ def bpr_exact_f64(U, V, b, d, tu, ti, tj, lr, reg_u, reg_b, reg_pos, reg_neg, lo
     assert U.dtype == torch.float64 and V.dtype == torch.float64 and b.dtype == torch.float64
     n = tu.numel()
     nu, ni = U.shape[0], V.shape[0]
-    nbytes = lib().eb_bpr_exact_workspace_bytes(n, nu, ni)
-    ws = _ws_exact.get(nbytes, U.device)
-    with torch.cuda.device(U.device):
-        check(lib().eb_bpr_exact_f64(_ptr(U), _ptr(V), _ptr(b), d, U.stride(0), nu, ni, _ptr(tu), _ptr(ti), _ptr(tj), n,
-                                     lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), _ptr(ws), ws.numel(), _stream(U)))
+    ws = _scratch("bpr_exact", lib().eb_bpr_exact_workspace_bytes(n, nu, ni), U.device)
+    _call("eb_bpr_exact_f64", U, _ptr(U), _ptr(V), _ptr(b), d, U.stride(0), nu, ni, _ptr(tu), _ptr(ti), _ptr(tj), n, lr, reg_u,
+          reg_b, reg_pos, reg_neg, _ptr(loss), _ptr(ws), ws.numel())
 
 
 class MtSampler:
@@ -300,49 +337,33 @@ class MtSampler:
         self.n_users, self.n_items = n_users, n_items
         self.indptr, self.set_indices, self.sorted_indices = indptr, set_indices, sorted_indices
         self.state = torch.empty(625, dtype=torch.int32, device=indptr.device)
-        with torch.cuda.device(indptr.device):
-            check(lib().eb_mt_seed(_ptr(self.state), seed, _stream(indptr)))
+        _call("eb_mt_seed", indptr, _ptr(self.state), seed)
 
     def raw(self, n):
         out = torch.empty(n, dtype=torch.int32, device=self.state.device)
-        with torch.cuda.device(self.state.device):
-            check(lib().eb_mt_raw(_ptr(self.state), _ptr(out), n, _stream(out)))
+        _call("eb_mt_raw", out, _ptr(self.state), _ptr(out), n)
         return out
 
     def step(self, events):
         dev = self.state.device
         u = torch.empty(events, dtype=torch.int32, device=dev); i = torch.empty_like(u); j = torch.empty_like(u)
-        ws = _ws_sampler.get(lib().eb_mt_sampler_workspace_bytes(events), dev)
-        with torch.cuda.device(dev):
-            check(lib().eb_mt_sampler_step(_ptr(self.state), self.n_users, self.n_items, _ptr(self.indptr),
-                                           _ptr(self.set_indices), _ptr(self.sorted_indices), events, _ptr(u), _ptr(i),
-                                           _ptr(j), _ptr(ws), ws.numel(), _stream(u)))
+        ws = _scratch("mt_sampler", lib().eb_mt_sampler_workspace_bytes(events), dev)
+        _call("eb_mt_sampler_step", u, _ptr(self.state), self.n_users, self.n_items, _ptr(self.indptr), _ptr(self.set_indices),
+              _ptr(self.sorted_indices), events, _ptr(u), _ptr(i), _ptr(j), _ptr(ws), ws.numel())
         return u, i, j
 
 
 def score_topk(U, V, bias, d, k, mask_indptr=None, mask_indices=None, users=None, user_begin=0, n_sel=None):
     """Exact full-catalogue score + train mask + top-k (BPRMF_model.py:70-85 / BPRMF_batch_model.py:82-88)."""
     _need_cuda(U, V, bias, mask_indptr, mask_indices, users)
-    if users is not None:
-        _chk_idx(users)
-        n_sel = users.numel()
-    elif n_sel is None:
-        n_sel = U.shape[0] - user_begin
-    n_items = V.shape[0]
-    dev = U.device
-    idx = torch.empty((n_sel, k), dtype=torch.int32, device=dev)
-    val = torch.empty((n_sel, k), dtype=U.dtype, device=dev)
-    esz = U.element_size()
-    ws = _ws_score.get(lib().eb_score_topk_workspace_bytes(n_sel, n_items, esz), dev)
-    fn = lib().eb_score_topk_f32 if U.dtype == torch.float32 else lib().eb_score_topk_f64
     assert U.dtype in (torch.float32, torch.float64) and V.dtype == U.dtype
-    with torch.cuda.device(dev):
-        check(fn(_ptr(U), _ptr(V), _ptr(bias), n_items, d, U.stride(0), _ptr(mask_indptr), _ptr(mask_indices),
-                 _ptr(users), user_begin, n_sel, k, _ptr(idx), _ptr(val), _ptr(ws), ws.numel(), _stream(U)))
+    n_sel, idx, val = _topk_out(users, U.shape[0], user_begin, n_sel, k, U.dtype, U.device)
+    n_items = V.shape[0]
+    ws = _scratch("score_topk", lib().eb_score_topk_workspace_bytes(n_sel, n_items, U.element_size()), U.device)
+    _call("eb_score_topk_f32" if U.dtype == torch.float32 else "eb_score_topk_f64", U, _ptr(U), _ptr(V), _ptr(bias), n_items, d,
+          U.stride(0), _ptr(mask_indptr), _ptr(mask_indices), _ptr(users), user_begin, n_sel, k, _ptr(idx), _ptr(val), _ptr(ws),
+          ws.numel())
     return idx, val
-
-
-_ws_tc = _Workspace()
 
 
 def score_topk_tc(U, V, bias, d, k, mask_indptr=None, mask_indices=None, user_begin=0, n_sel=None, dump=False, stats=True):
@@ -352,19 +373,14 @@ def score_topk_tc(U, V, bias, d, k, mask_indptr=None, mask_indices=None, user_be
     stays asynchronous (the models' path) and the dict is empty."""
     _need_cuda(U, V, bias, mask_indptr, mask_indices)
     assert U.dtype == torch.float32 and V.dtype == torch.float32 and U.stride(0) == V.stride(0)
-    if n_sel is None:
-        n_sel = U.shape[0] - user_begin
+    n_sel, idx, val = _topk_out(None, U.shape[0], user_begin, n_sel, k, torch.float32, U.device)
     n_items = V.shape[0]
-    dev = U.device
-    idx = torch.empty((n_sel, k), dtype=torch.int32, device=dev)
-    val = torch.empty((n_sel, k), dtype=torch.float32, device=dev)
-    dmp = torch.zeros((n_sel, n_items), dtype=torch.float32, device=dev) if dump else None
-    ws = _ws_tc.get(lib().eb_score_topk_tc_workspace_bytes(n_sel, n_items, d), dev)
+    dmp = torch.zeros((n_sel, n_items), dtype=torch.float32, device=U.device) if dump else None
+    ws = _scratch("score_topk_tc", lib().eb_score_topk_tc_workspace_bytes(n_sel, n_items, d), U.device)
     st = (ctypes.c_int64 * 16)() if stats else None
-    with torch.cuda.device(dev):
-        check(lib().eb_score_topk_tc_f32(_ptr(U), _ptr(V), _ptr(bias), n_items, d, U.stride(0), _ptr(mask_indptr),
-                                         _ptr(mask_indices), user_begin, n_sel, k, _ptr(idx), _ptr(val), _ptr(dmp),
-                                         _ptr(ws), ws.numel(), ctypes.cast(st, ctypes.c_void_p) if stats else None, _stream(U)))
+    _call("eb_score_topk_tc_f32", U, _ptr(U), _ptr(V), _ptr(bias), n_items, d, U.stride(0), _ptr(mask_indptr), _ptr(mask_indices),
+          user_begin, n_sel, k, _ptr(idx), _ptr(val), _ptr(dmp), _ptr(ws), ws.numel(),
+          ctypes.cast(st, ctypes.c_void_p) if stats else None)
     out = {"rechecked": int(st[0]), "kp": int(st[1]), "prof": [int(x) for x in st[2:16]]} if stats else {}
     if dump:
         out["dump"] = dmp
@@ -376,9 +392,8 @@ def bpr_batch_grad_f32(Gu, Gi, Bi, dGu, dGi, dBi, d, tu, ti, tj, l_w, l_b, loss=
     _need_cuda(Gu, Gi, Bi, dGu, dGi, dBi, tu, ti, tj, loss)
     _chk_idx(tu, ti, tj)
     assert Gu.stride(0) == Gi.stride(0) == dGu.stride(0) == dGi.stride(0)
-    with torch.cuda.device(Gu.device):
-        check(lib().eb_bpr_batch_grad_f32(_ptr(Gu), _ptr(Gi), _ptr(Bi), _ptr(dGu), _ptr(dGi), _ptr(dBi), d, Gu.stride(0),
-                                          _ptr(tu), _ptr(ti), _ptr(tj), tu.numel(), l_w, l_b, _ptr(loss), _stream(Gu)))
+    _call("eb_bpr_batch_grad_f32", Gu, _ptr(Gu), _ptr(Gi), _ptr(Bi), _ptr(dGu), _ptr(dGi), _ptr(dBi), d, Gu.stride(0), _ptr(tu),
+          _ptr(ti), _ptr(tj), tu.numel(), l_w, l_b, _ptr(loss))
 
 
 def adam_dense_f32(var, m, v, grad, lr, step, beta1=0.9, beta2=0.999, eps=1e-7):
@@ -386,22 +401,18 @@ def adam_dense_f32(var, m, v, grad, lr, step, beta1=0.9, beta2=0.999, eps=1e-7):
     _need_cuda(var, m, v, grad)
     n = var.numel()
     assert var.is_contiguous() and m.numel() == n and v.numel() == n and grad.numel() == n and n % 4 == 0
-    with torch.cuda.device(var.device):
-        check(lib().eb_adam_dense_f32(_ptr(var), _ptr(m), _ptr(v), _ptr(grad), n, lr, beta1, beta2, eps, step,
-                                      _stream(var)))
+    _call("eb_adam_dense_f32", var, _ptr(var), _ptr(m), _ptr(v), _ptr(grad), n, lr, beta1, beta2, eps, step)
 
 
 def table_delta_f32(cur, prev, delta):
     _need_cuda(cur, prev, delta)
     assert cur.is_contiguous() and prev.is_contiguous() and delta.is_contiguous() and cur.numel() % 4 == 0
-    with torch.cuda.device(cur.device):
-        check(lib().eb_table_delta_f32(_ptr(cur), _ptr(prev), _ptr(delta), cur.numel(), _stream(cur)))
+    _call("eb_table_delta_f32", cur, _ptr(cur), _ptr(prev), _ptr(delta), cur.numel())
 
 
 def table_apply_delta_f32(cur, prev, delta_sum, scale=1.0):
     _need_cuda(cur, prev, delta_sum)
-    with torch.cuda.device(cur.device):
-        check(lib().eb_table_apply_delta_f32(_ptr(cur), _ptr(prev), _ptr(delta_sum), cur.numel(), scale, _stream(cur)))
+    _call("eb_table_apply_delta_f32", cur, _ptr(cur), _ptr(prev), _ptr(delta_sum), cur.numel(), scale)
 
 
 _EXACT_GEMM = False
@@ -430,9 +441,8 @@ def _gemm_ref(A, B, M, N, K, a_mn, b_mn, bias, alpha, act, out):
     assert A.dtype == torch.float32 and B.dtype == torch.float32
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=A.device)
-    with torch.cuda.device(A.device):
-        check(lib().eb_gemm_f32_ref(_ptr(A), A.stride(0), 1 if a_mn else 0, _ptr(B), B.stride(0), 1 if b_mn else 0, _ptr(out),
-                                    out.stride(0), M, N, K, _ptr(bias), alpha, act, _stream(A)))
+    _call("eb_gemm_f32_ref", A, _ptr(A), A.stride(0), 1 if a_mn else 0, _ptr(B), B.stride(0), 1 if b_mn else 0, _ptr(out),
+          out.stride(0), M, N, K, _ptr(bias), alpha, act)
     return out
 
 
@@ -447,8 +457,7 @@ def to_bf16(src, transpose=False, out=None):
     ldd = (cols + 7) // 8 * 8
     if out is None:
         out = torch.empty((rows, ldd), dtype=torch.bfloat16, device=src.device)
-    with torch.cuda.device(src.device):
-        check(lib().eb_convert_bf16(_ptr(src), R, C, src.stride(0), _ptr(out), ldd, 1 if transpose else 0, _stream(src)))
+    _call("eb_convert_bf16", src, _ptr(src), R, C, src.stride(0), _ptr(out), ldd, 1 if transpose else 0)
     return out
 
 
@@ -465,16 +474,14 @@ def gemm_bf16_tn(A, B, M, N, K, bias=None, alpha=1.0, act=0, out=None, out_bf16=
             out = torch.empty((M, N), dtype=torch.float32, device=A.device)
         ldb = (N + 7) // 8 * 8
         Cb = torch.empty((M, ldb), dtype=torch.bfloat16, device=A.device) if ldb == N else torch.zeros((M, ldb), dtype=torch.bfloat16, device=A.device)
-        with torch.cuda.device(A.device):
-            check(lib().eb_gemm_bf16_out(_ptr(A), A.stride(0), 0, _ptr(B), B.stride(0), 0, _ptr(out), out.stride(0), _ptr(Cb), ldb,
-                                         M, N, K, _ptr(bias), alpha, act, _stream(A)))
+        _call("eb_gemm_bf16_out", A, _ptr(A), A.stride(0), 0, _ptr(B), B.stride(0), 0, _ptr(out), out.stride(0), _ptr(Cb), ldb, M,
+              N, K, _ptr(bias), alpha, act)
         return out, Cb
     assert A.dtype == torch.bfloat16 and B.dtype == torch.bfloat16
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=A.device)
-    with torch.cuda.device(A.device):
-        check(lib().eb_gemm_bf16_tn(_ptr(A), A.stride(0), _ptr(B), B.stride(0), _ptr(out), out.stride(0), M, N, K, _ptr(bias),
-                                    alpha, act, _stream(A)))
+    _call("eb_gemm_bf16_tn", A, _ptr(A), A.stride(0), _ptr(B), B.stride(0), _ptr(out), out.stride(0), M, N, K, _ptr(bias), alpha,
+          act)
     return out
 
 
@@ -487,9 +494,8 @@ def gemm_bf16(A, B, M, N, K, a_rows_are_k=False, b_rows_are_k=False, bias=None, 
     assert A.dtype == torch.bfloat16 and B.dtype == torch.bfloat16
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=A.device)
-    with torch.cuda.device(A.device):
-        check(lib().eb_gemm_bf16(_ptr(A), A.stride(0), 1 if a_rows_are_k else 0, _ptr(B), B.stride(0), 1 if b_rows_are_k else 0,
-                                 _ptr(out), out.stride(0), M, N, K, _ptr(bias), alpha, act, _stream(A)))
+    _call("eb_gemm_bf16", A, _ptr(A), A.stride(0), 1 if a_rows_are_k else 0, _ptr(B), B.stride(0), 1 if b_rows_are_k else 0,
+          _ptr(out), out.stride(0), M, N, K, _ptr(bias), alpha, act)
     return out
 
 
@@ -520,60 +526,46 @@ def vae_model_struct(n_items, H, L, P, G, M, V, bf16_copies, indptr, indices):
     return st
 
 
-_vae_ws = {}
-
-
 def vae_train_step(model, n_items, H, L, rows, drop_rate, noise_seed, drop_seed, step, anneal, lr, acc, phase=3):
     """eb_vae_train_step: phase bit 0 = forward+backward into the gradient buffers, bit 1 = Adam + operand refresh."""
     _need_cuda(acc, rows)
-    dev = acc.device
     B = rows.numel() if rows is not None else 0
     ws = None
     if phase & 1:
         _chk_idx(rows)
-        need = lib().eb_vae_step_workspace_bytes(n_items, H, L, B)
-        ws = _vae_ws.get(dev)
-        if ws is None or ws.numel() < need:
-            ws = _vae_ws[dev] = torch.empty(need, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        check(lib().eb_vae_train_step(ctypes.byref(model), _ptr(rows), B, drop_rate, noise_seed, drop_seed, step, anneal, lr,
-                                      _ptr(acc), _ptr(ws), ws.numel() if ws is not None else 0, phase, _stream(acc)))
+        ws = _scratch("vae_step", lib().eb_vae_step_workspace_bytes(n_items, H, L, B), acc.device)
+    _call("eb_vae_train_step", acc, ctypes.byref(model), _ptr(rows), B, drop_rate, noise_seed, drop_seed, step, anneal, lr,
+          _ptr(acc), _ptr(ws), ws.numel() if ws is not None else 0, phase)
 
 
 # ---------------------------------------------------------------- MultiVAE pieces (vae.cu)
 def vae_embed_fwd(W1, b1, indptr, indices, rows, h1, drop_rate=0.0, seed=0):
     _need_cuda(W1, b1, indptr, indices, rows, h1)
-    with torch.cuda.device(W1.device):
-        check(lib().eb_vae_embed_fwd(_ptr(W1), _ptr(b1), W1.shape[1], _ptr(indptr), _ptr(indices), _ptr(rows), rows.numel(),
-                                     _ptr(h1), h1.stride(0), drop_rate, seed, _stream(W1)))
+    _call("eb_vae_embed_fwd", W1, _ptr(W1), _ptr(b1), W1.shape[1], _ptr(indptr), _ptr(indices), _ptr(rows), rows.numel(),
+          _ptr(h1), h1.stride(0), drop_rate, seed)
 
 
 def vae_embed_bwd(dW1, indptr, indices, rows, dpre1, drop_rate=0.0, seed=0):
     _need_cuda(dW1, indptr, indices, rows, dpre1)
-    with torch.cuda.device(dW1.device):
-        check(lib().eb_vae_embed_bwd(_ptr(dW1), dW1.shape[1], _ptr(indptr), _ptr(indices), _ptr(rows), rows.numel(), _ptr(dpre1),
-                                     dpre1.stride(0), drop_rate, seed, _stream(dW1)))
+    _call("eb_vae_embed_bwd", dW1, _ptr(dW1), dW1.shape[1], _ptr(indptr), _ptr(indices), _ptr(rows), rows.numel(), _ptr(dpre1),
+          dpre1.stride(0), drop_rate, seed)
 
 
 def vae_reparam_fwd(ml, L, z, seed, step, kl_sum=None):
     _need_cuda(ml, z, kl_sum)
-    with torch.cuda.device(ml.device):
-        check(lib().eb_vae_reparam_fwd(_ptr(ml), ml.stride(0), ml.shape[0], L, _ptr(z), z.stride(0), seed, step, _ptr(kl_sum),
-                                       _stream(ml)))
+    _call("eb_vae_reparam_fwd", ml, _ptr(ml), ml.stride(0), ml.shape[0], L, _ptr(z), z.stride(0), seed, step, _ptr(kl_sum))
 
 
 def vae_reparam_bwd(ml, L, dz, dml, seed, step, anneal):
     _need_cuda(ml, dz, dml)
-    with torch.cuda.device(ml.device):
-        check(lib().eb_vae_reparam_bwd(_ptr(ml), ml.stride(0), ml.shape[0], L, _ptr(dz), dz.stride(0), _ptr(dml), dml.stride(0),
-                                       seed, step, anneal, _stream(ml)))
+    _call("eb_vae_reparam_bwd", ml, _ptr(ml), ml.stride(0), ml.shape[0], L, _ptr(dz), dz.stride(0), _ptr(dml), dml.stride(0),
+          seed, step, anneal)
 
 
 def vae_softmax(logits, indptr, indices, rows, nll_sum=None, lse_out=None, write_grad=True):
     _need_cuda(logits, indptr, indices, rows, nll_sum, lse_out)
-    with torch.cuda.device(logits.device):
-        check(lib().eb_vae_softmax(_ptr(logits), logits.stride(0), logits.shape[1], _ptr(indptr), _ptr(indices), _ptr(rows),
-                                   logits.shape[0], _ptr(nll_sum), _ptr(lse_out), 1 if write_grad else 0, _stream(logits)))
+    _call("eb_vae_softmax", logits, _ptr(logits), logits.stride(0), logits.shape[1], _ptr(indptr), _ptr(indices), _ptr(rows),
+          logits.shape[0], _ptr(nll_sum), _ptr(lse_out), 1 if write_grad else 0)
 
 
 def tanh_bwd(dout, out, dpre=None):
@@ -581,8 +573,7 @@ def tanh_bwd(dout, out, dpre=None):
     assert dout.is_contiguous() and out.is_contiguous()
     if dpre is None:
         dpre = torch.empty_like(dout)
-    with torch.cuda.device(dout.device):
-        check(lib().eb_tanh_bwd(_ptr(dout), _ptr(out), _ptr(dpre), dout.numel(), _stream(dout)))
+    _call("eb_tanh_bwd", dout, _ptr(dout), _ptr(out), _ptr(dpre), dout.numel())
     return dpre
 
 
@@ -590,8 +581,7 @@ def colsum(src, out=None):
     _need_cuda(src, out)
     if out is None:
         out = torch.empty(src.shape[1], dtype=torch.float32, device=src.device)
-    with torch.cuda.device(src.device):
-        check(lib().eb_colsum(_ptr(src), src.shape[0], src.shape[1], src.stride(0), _ptr(out), _stream(src)))
+    _call("eb_colsum", src, _ptr(src), src.shape[0], src.shape[1], src.stride(0), _ptr(out))
     return out
 
 
@@ -638,19 +628,10 @@ def knn_score_topk(A, B, n_cols, k, frac_bits, mask_indptr=None, mask_indices=No
     _need_cuda(ap, ai, av, bp, bi, bv, mask_indptr, mask_indices, users)
     assert ap.dtype == bp.dtype == torch.int64 and av.dtype == bv.dtype == torch.float32
     _chk_idx(ai, bi)
-    if users is not None:
-        _chk_idx(users)
-        n_sel = users.numel()
-    elif n_sel is None:
-        n_sel = ap.numel() - 1 - user_begin
-    idx = torch.empty((n_sel, k), dtype=torch.int32, device=ap.device)
-    val = torch.empty((n_sel, k), dtype=torch.float32, device=ap.device)
+    n_sel, idx, val = _topk_out(users, ap.numel() - 1, user_begin, n_sel, k, torch.float32, ap.device)
     _call("eb_knn_score_topk_f32", ap, _ptr(ap), _ptr(ai), _ptr(av), _ptr(bp), _ptr(bi), _ptr(bv), n_cols, _ptr(mask_indptr),
           _ptr(mask_indices), _ptr(users), user_begin, n_sel, k, int(frac_bits), _ptr(idx), _ptr(val))
     return idx, val
-
-
-_ws_gram = _Workspace()
 
 
 def gram_f64(Y, d, n=None, out=None):
@@ -661,7 +642,7 @@ def gram_f64(Y, d, n=None, out=None):
     if out is None:
         out = torch.empty((d, d), dtype=torch.float64, device=Y.device)
     assert out.dtype == torch.float64 and out.is_contiguous() and out.numel() == d * d
-    ws = _ws_gram.get(lib().eb_gram_f64_workspace_bytes(n, d), Y.device)
+    ws = _scratch("gram", lib().eb_gram_f64_workspace_bytes(n, d), Y.device)
     _call("eb_gram_f64", Y, _ptr(Y), n, d, Y.stride(0), _ptr(out), _ptr(ws), ws.numel())
     return out
 
@@ -669,11 +650,6 @@ def gram_f64(Y, d, n=None, out=None):
 def als_small_d_max():
     """Largest d solved one row per warp by als_solve_f64 (larger d: one row per CTA)."""
     return int(lib().eb_als_small_d_max())
-
-
-def _nonempty(t):
-    """The C ABI takes no NULL arrays: an empty one is passed as a one-element dummy."""
-    return t if t.numel() else torch.zeros(1, dtype=t.dtype, device=t.device)
 
 
 def als_solve_f64(G, Y, d, indptr, indices, w, c, order, reg, X):
@@ -733,13 +709,7 @@ def dense_score_topk(A, B, k, frac_bits, mask_indptr=None, mask_indices=None, us
     _need_cuda(ap, ai, av, B, mask_indptr, mask_indices, users)
     assert ap.dtype == torch.int64 and av.dtype == B.dtype == torch.float32 and B.stride(1) == 1
     _chk_idx(ai)
-    if users is not None:
-        _chk_idx(users)
-        n_sel = users.numel()
-    elif n_sel is None:
-        n_sel = ap.numel() - 1 - user_begin
-    idx = torch.empty((n_sel, k), dtype=torch.int32, device=ap.device)
-    val = torch.empty((n_sel, k), dtype=torch.float32, device=ap.device)
+    n_sel, idx, val = _topk_out(users, ap.numel() - 1, user_begin, n_sel, k, torch.float32, ap.device)
     ai, av = _nonempty(ai), _nonempty(av)
     _call("eb_dense_score_topk_f32", ap, _ptr(ap), _ptr(ai), _ptr(av), _ptr(B), B.stride(0), B.shape[1],
           _ptr(mask_indptr), _ptr(mask_indices), _ptr(users), user_begin, n_sel, k, int(frac_bits), _ptr(idx), _ptr(val))
@@ -750,8 +720,13 @@ def rp3_tile_cols():
     return int(lib().eb_rp3_tile_cols())
 
 
+def rp3_row_workspace_bytes(n_cols):
+    """Bytes of the row workspace rp3_similarity and rp3_score_topk allocate for n_cols columns (0 up to rp3_tile_cols())."""
+    return int(lib().eb_rp3_row_workspace_bytes(n_cols))
+
+
 def _rp3_row_ws(n_cols, device):
-    return torch.empty(max(int(lib().eb_rp3_row_workspace_bytes(n_cols)), 1), dtype=torch.uint8, device=device)
+    return torch.empty(max(rp3_row_workspace_bytes(n_cols), 1), dtype=torch.uint8, device=device)
 
 
 def rp3_similarity(A, B, degree, k, order=None):
@@ -811,15 +786,9 @@ def rp3_score_topk(A, B, n_cols, k, mask_indptr=None, mask_indices=None, users=N
     _need_cuda(ap, ai, av, bp, bi, bv, mask_indptr, mask_indices, users, order)
     assert ap.dtype == bp.dtype == torch.int64 and av.dtype == bv.dtype == torch.float32
     _chk_idx(ai, bi)
-    if users is not None:
-        _chk_idx(users)
-        n_sel = users.numel()
-    elif n_sel is None:
-        n_sel = ap.numel() - 1 - user_begin
     if order is not None:
         _chk_idx(order)
-    idx = torch.empty((n_sel, k), dtype=torch.int32, device=ap.device)
-    val = torch.empty((n_sel, k), dtype=torch.float32, device=ap.device)
+    n_sel, idx, val = _topk_out(users, ap.numel() - 1, user_begin, n_sel, k, torch.float32, ap.device)
     ws = _rp3_row_ws(n_cols, ap.device)
     ai, av, bi, bv = _nonempty(ai), _nonempty(av), _nonempty(bi), _nonempty(bv)
     _call("eb_rp3_score_topk_f32", ap, _ptr(ap), _ptr(ai), _ptr(av), _ptr(bp), _ptr(bi), _ptr(bv), n_cols, _ptr(mask_indptr),
@@ -832,9 +801,8 @@ def dense_topk(scores, k, mask_indptr=None, mask_indices=None, rows=None, shift=
     n = scores.shape[0]
     idx = torch.empty((n, k), dtype=torch.int32, device=scores.device)
     val = torch.empty((n, k), dtype=torch.float32, device=scores.device)
-    with torch.cuda.device(scores.device):
-        check(lib().eb_dense_topk_f32(_ptr(scores), scores.stride(0), n, scores.shape[1], _ptr(mask_indptr), _ptr(mask_indices),
-                                      _ptr(rows), _ptr(shift), k, _ptr(idx), _ptr(val), _stream(scores)))
+    _call("eb_dense_topk_f32", scores, _ptr(scores), scores.stride(0), n, scores.shape[1], _ptr(mask_indptr), _ptr(mask_indices),
+          _ptr(rows), _ptr(shift), k, _ptr(idx), _ptr(val))
     return idx, val
 
 
@@ -890,17 +858,15 @@ def slim_weights(coef_t, drop, nnz, neighborhood):
     _need_cuda(coef_t, drop, nnz)
     n = coef_t.shape[0]
     dev = coef_t.device
-    with torch.cuda.device(dev):
-        vals = coef_t.clone()
+    vals = coef_t.clone()
     _call("eb_slim_drop_f32", vals, n, _ptr(drop), _ptr(vals))
-    with torch.cuda.device(dev):
-        total = int(torch.clamp(nnz.to(torch.int64), min=0).sum().item())
-        idx = torch.arange(n, dtype=torch.int32, device=dev).repeat(n)
-        cnt = torch.full((n,), n, dtype=torch.int32, device=dev)
-        indptr = torch.empty(n + 1, dtype=torch.int64, device=dev)
-        indices = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
-        values = torch.empty(max(total, 1), dtype=torch.float32, device=dev)
-        ws = torch.empty(int(lib().eb_rp3_prune_workspace_bytes(n, n, total)), dtype=torch.uint8, device=dev)
+    total = int(torch.clamp(nnz.to(torch.int64), min=0).sum().item())
+    idx = torch.arange(n, dtype=torch.int32, device=dev).repeat(n)
+    cnt = torch.full((n,), n, dtype=torch.int32, device=dev)
+    indptr = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    indices = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
+    values = torch.empty(max(total, 1), dtype=torch.float32, device=dev)
+    ws = torch.empty(int(lib().eb_rp3_prune_workspace_bytes(n, n, total)), dtype=torch.uint8, device=dev)
     _call("eb_rp3_prune_cols_f32", vals, n, n, _ptr(cnt), _ptr(idx), _ptr(vals), total, int(neighborhood), _ptr(indptr),
           _ptr(indices), _ptr(values), _ptr(ws), ws.numel())
     m = int(indptr[-1].item())
@@ -913,25 +879,18 @@ def svd_max_width():
     return int(lib().eb_svd_max_width())
 
 
-def _chk_f64(*ts):
-    for t in ts:
-        if t.dtype != torch.float64 or t.dim() != 2 or t.stride(1) != 1:
-            raise TypeError("fp64 blocks must be 2-D with unit column stride")
-
-
 def csr_spmm_f64(csr, X, out=None):
     """A X (eb_csr_spmm_f64) for csr = (indptr int64, indices int32, data fp32) of A and an fp64 X with one row per column
     of A; every output element summed over its row's entries in stored order.  Returns out [rows of A][X.shape[1]]."""
     indptr, indices, data = csr
     _need_cuda(indptr, indices, data, X, out)
-    _chk_f64(X)
+    _chk_f64_rows(X)
     _chk_idx(indices)
     assert indptr.dtype == torch.int64 and data.dtype == torch.float32 and indptr.is_contiguous() and data.is_contiguous()
     n, w = indptr.numel() - 1, X.shape[1]
     if out is None:
-        with torch.cuda.device(X.device):
-            out = torch.empty((n, w), dtype=torch.float64, device=X.device)
-    _chk_f64(out)
+        out = torch.empty((n, w), dtype=torch.float64, device=X.device)
+    _chk_f64_rows(out)
     assert out.shape[0] == n and out.shape[1] >= w
     indices, data = _nonempty(indices), _nonempty(data)
     _call("eb_csr_spmm_f64", X, _ptr(indptr), _ptr(indices), _ptr(data), n, _ptr(X), w, X.stride(0), _ptr(out), out.stride(0))
@@ -945,8 +904,7 @@ def chol_pivoted_f64(G, M=None, rank=None):
     w = G.shape[0]
     assert G.dtype == torch.float64 and G.is_contiguous() and G.shape == (w, w)
     if M is None:
-        with torch.cuda.device(G.device):
-            M = torch.empty((w, w), dtype=torch.float64, device=G.device)
+        M = torch.empty((w, w), dtype=torch.float64, device=G.device)
     assert M.dtype == torch.float64 and M.is_contiguous() and M.shape == (w, w)
     assert rank is None or (rank.dtype == torch.int32 and rank.numel() >= 1)
     _call("eb_chol_pivoted_f64", G, _ptr(G), w, _ptr(M), _ptr(rank))
@@ -957,14 +915,13 @@ def tall_times_small_f64(X, M, out=None):
     """X M (eb_tall_times_small_f64) for a tall fp64 X [n][w] and a contiguous M [w][d]; `out` may be X itself when
     d == w."""
     _need_cuda(X, M, out)
-    _chk_f64(X)
+    _chk_f64_rows(X)
     n, w = X.shape
     assert M.dtype == torch.float64 and M.is_contiguous() and M.shape[0] == w
     d = M.shape[1]
     if out is None:
-        with torch.cuda.device(X.device):
-            out = torch.empty((n, d), dtype=torch.float64, device=X.device)
-    _chk_f64(out)
+        out = torch.empty((n, d), dtype=torch.float64, device=X.device)
+    _chk_f64_rows(out)
     assert out.shape[0] == n and out.shape[1] >= d
     _call("eb_tall_times_small_f64", X, _ptr(X), n, w, X.stride(0), _ptr(M), d, _ptr(out), out.stride(0))
     return out
@@ -975,10 +932,9 @@ def sym_eig_f64(A):
     _need_cuda(A)
     w = A.shape[0]
     assert A.dtype == torch.float64 and A.is_contiguous() and A.shape == (w, w)
-    with torch.cuda.device(A.device):
-        evals = torch.empty(w, dtype=torch.float64, device=A.device)
-        evecs = torch.empty((w, w), dtype=torch.float64, device=A.device)
-        ws = torch.empty(max(1, int(lib().eb_sym_eig_f64_workspace_bytes(w))), dtype=torch.uint8, device=A.device)
+    evals = torch.empty(w, dtype=torch.float64, device=A.device)
+    evecs = torch.empty((w, w), dtype=torch.float64, device=A.device)
+    ws = torch.empty(max(1, int(lib().eb_sym_eig_f64_workspace_bytes(w))), dtype=torch.uint8, device=A.device)
     _call("eb_sym_eig_f64", A, _ptr(A), w, _ptr(evals), _ptr(evecs), _ptr(ws), ws.numel())
     return evals, evecs
 
@@ -987,11 +943,10 @@ def svd_finish_f64(evals, user, item, scale_user_by_inv_s):
     """In place on the first d = user.shape[1] columns (eb_svd_finish_f64): the optional 1/s and s column scaling and
     the sign of each user column's largest entry; returns s [d]."""
     _need_cuda(evals, user, item)
-    _chk_f64(user, item)
+    _chk_f64_rows(user, item)
     d = user.shape[1]
     assert evals.dtype == torch.float64 and evals.is_contiguous() and item.shape[1] == d
-    with torch.cuda.device(user.device):
-        s = torch.empty(d, dtype=torch.float64, device=user.device)
+    s = torch.empty(d, dtype=torch.float64, device=user.device)
     _call("eb_svd_finish_f64", user, _ptr(evals), evals.numel(), d, _ptr(user), user.shape[0], user.stride(0), _ptr(item),
           item.shape[0], item.stride(0), int(bool(scale_user_by_inv_s)), _ptr(s))
     return s
@@ -1006,8 +961,7 @@ def slope_one_dev_f64(F, M1, M2, n, s, out=None):
         assert t.dtype == torch.float32 and t.stride(1) == 1 and t.stride(0) == F.stride(0) and t.shape[0] == F.shape[0]
     rows = F.shape[0]
     if out is None:
-        with torch.cuda.device(F.device):
-            out = torch.empty((rows, n), dtype=torch.float64, device=F.device)
+        out = torch.empty((rows, n), dtype=torch.float64, device=F.device)
     assert out.dtype == torch.float64 and out.stride(1) == 1 and out.shape[0] == rows and out.shape[1] >= n
     _call("eb_slope_one_dev_f64", F, _ptr(F), _ptr(M1), _ptr(M2), F.stride(0), rows, n, int(s), _ptr(out), out.stride(0))
     return out
@@ -1022,14 +976,7 @@ def slope_one_score_topk(E, train, k, mask_indptr=None, mask_indices=None, users
     assert E.dtype == torch.float64 and E.stride(1) == 1
     assert indptr.dtype == torch.int64 and ratings.dtype == torch.float32 and ratings.is_contiguous()
     _chk_idx(items)
-    if users is not None:
-        _chk_idx(users)
-        n_sel = users.numel()
-    elif n_sel is None:
-        n_sel = indptr.numel() - 1 - user_begin
-    with torch.cuda.device(E.device):
-        idx = torch.empty((n_sel, k), dtype=torch.int32, device=E.device)
-        val = torch.empty((n_sel, k), dtype=torch.float64, device=E.device)
+    n_sel, idx, val = _topk_out(users, indptr.numel() - 1, user_begin, n_sel, k, torch.float64, E.device)
     items, ratings = _nonempty(items), _nonempty(ratings)
     if mask_indices is not None:
         _chk_idx(mask_indices)
@@ -1040,22 +987,16 @@ def slope_one_score_topk(E, train, k, mask_indptr=None, mask_indices=None, users
 
 
 # ---------------------------------------------------------------- NonNegMF (nonneg_mf.cu)
-def _chk_f64(*ts):
-    for t in ts:
-        assert t.dtype == torch.float64 and t.is_contiguous()
-
-
 def nnmf_dots_f64(P, Q, indptr, items, out=None):
     """dot_k = Q[i_k] . P[u_k] for every rating k of the CSR (indptr int64, items int32), summed in f order from +0.0
     (eb_nnmf_dots_f64).  P [n_users][F] and Q [n_items][F] fp64, contiguous."""
     _need_cuda(P, Q, indptr, items, out)
-    _chk_f64(P, Q)
+    _chk_f64_dense(P, Q)
     _chk_idx(items)
     assert indptr.dtype == torch.int64 and P.shape[1] == Q.shape[1] and indptr.numel() == P.shape[0] + 1
     if out is None:
-        with torch.cuda.device(P.device):
-            out = torch.empty(items.numel(), dtype=torch.float64, device=P.device)
-    _chk_f64(out)
+        out = torch.empty(items.numel(), dtype=torch.float64, device=P.device)
+    _chk_f64_dense(out)
     _call("eb_nnmf_dots_f64", P, _ptr(P), _ptr(Q), P.shape[1], _ptr(indptr), _ptr(items), P.shape[0], _ptr(out))
     return out
 
@@ -1064,13 +1005,12 @@ def nnmf_bias_chain_f64(indptr, items, ratings, dots, mu, lr, reg, bu, bi, out=N
     """est_k for every rating k in order, updating bu and bi in place as the reference's loop does
     (eb_nnmf_bias_chain_f64).  ratings, dots, bu, bi: fp64 contiguous."""
     _need_cuda(indptr, items, ratings, dots, bu, bi, out)
-    _chk_f64(ratings, dots, bu, bi)
+    _chk_f64_dense(ratings, dots, bu, bi)
     _chk_idx(items)
     assert indptr.dtype == torch.int64 and indptr.numel() == bu.numel() + 1
     if out is None:
-        with torch.cuda.device(bu.device):
-            out = torch.empty(items.numel(), dtype=torch.float64, device=bu.device)
-    _chk_f64(out)
+        out = torch.empty(items.numel(), dtype=torch.float64, device=bu.device)
+    _chk_f64_dense(out)
     _call("eb_nnmf_bias_chain_f64", bu, _ptr(indptr), _ptr(items), _ptr(ratings), _ptr(dots), bu.numel(), bi.numel(),
           float(mu), float(lr), float(reg), _ptr(bu), _ptr(bi), _ptr(out))
     return out
@@ -1080,25 +1020,19 @@ def nnmf_row_update_f64(indptr, cols, pos, ratings, est, T, S, reg, out=None):
     """S * (num / den) row by row (eb_nnmf_row_update_f64): num and den the ordered sums of T[col] * r_k and
     T[col] * est_k over each row's entries (k = pos[e], or e when pos is None), den + (n reg) S.  `out` may be S."""
     _need_cuda(indptr, cols, pos, ratings, est, T, S, out)
-    _chk_f64(ratings, est, T, S)
+    _chk_f64_dense(ratings, est, T, S)
     _chk_idx(cols)
     assert indptr.dtype == torch.int64 and indptr.numel() == S.shape[0] + 1 and T.shape[1] == S.shape[1]
     assert pos is None or (pos.dtype == torch.int64 and pos.is_contiguous())
     if out is None:
-        with torch.cuda.device(S.device):
-            out = torch.empty_like(S)
-    _chk_f64(out)
+        out = torch.empty_like(S)
+    _chk_f64_dense(out)
     _call("eb_nnmf_row_update_f64", S, _ptr(indptr), _ptr(cols), _ptr(pos), S.shape[0], _ptr(ratings), _ptr(est), _ptr(T),
           _ptr(S), _ptr(out), S.shape[1], float(reg))
     return out
 
 
 # ---------------------------------------------------------------- NeuMF pieces (neumf.cu)
-def _call(name, dev_tensor, *args):
-    with torch.cuda.device(dev_tensor.device):
-        check(getattr(lib(), name)(*args, _stream(dev_tensor)))
-
-
 def neumf_gather(Umf, Imf, Umlp, Imlp, f, u, it, x0, pm):
     _need_cuda(Umf, Imf, Umlp, Imlp, u, it, x0, pm)
     _call("eb_neumf_gather", Umf, _ptr(Umf), _ptr(Imf), _ptr(Umlp), _ptr(Imlp), f, Umf.stride(0), _ptr(u), _ptr(it), u.numel(),
@@ -1157,9 +1091,8 @@ def neumf_pair_head(Umf, Imf, f, u0, n_ub, n_items, h3, wp, bp, prob):
 
 def table_apply_delta_late_f32(cur, prev, delta_sum, delta_local, scale=1.0):
     _need_cuda(cur, prev, delta_sum, delta_local)
-    with torch.cuda.device(cur.device):
-        check(lib().eb_table_apply_delta_late_f32(_ptr(cur), _ptr(prev), _ptr(delta_sum), _ptr(delta_local), cur.numel(),
-                                                  float(scale), _stream(cur)))
+    _call("eb_table_apply_delta_late_f32", cur, _ptr(cur), _ptr(prev), _ptr(delta_sum), _ptr(delta_local), cur.numel(),
+          float(scale))
 
 
 def mf_pointwise_exact_f64(U, V, ub, ib, gb, d, su, si, sr, lr, reg, batch=100000, batch_loss=None):
@@ -1172,9 +1105,8 @@ def mf_pointwise_exact_f64(U, V, ub, ib, gb, d, su, si, sr, lr, reg, batch=10000
     n = su.numel()
     if batch_loss is not None:
         assert batch_loss.dtype == torch.float64 and batch_loss.numel() >= (n + batch - 1) // batch
-    with torch.cuda.device(U.device):
-        check(lib().eb_mf_pointwise_exact_f64(_ptr(U), _ptr(V), _ptr(ub), _ptr(ib), _ptr(gb), d, U.stride(0), _ptr(su), _ptr(si),
-                                              _ptr(sr), n, lr, reg, batch, _ptr(batch_loss), _stream(U)))
+    _call("eb_mf_pointwise_exact_f64", U, _ptr(U), _ptr(V), _ptr(ub), _ptr(ib), _ptr(gb), d, U.stride(0), _ptr(su), _ptr(si),
+          _ptr(sr), n, lr, reg, batch, _ptr(batch_loss))
 
 
 _mf_gb_work = {}
@@ -1189,30 +1121,21 @@ def mf_pointwise_step_f32(U, V, ub, ib, gb, d, pos_u, pos_i, m, n_items, seed, e
     for t in (U, V, ub, ib, gb):
         assert t.dtype == torch.float32
     assert U.stride(1) == 1 and V.stride(1) == 1 and U.stride(0) == V.stride(0)
-    ou = oi = orr = None
-    if out is not None:
-        ou, oi, orr = out
-        _need_cuda(ou, oi, orr); _chk_idx(ou, oi, orr)
+    out = _out_ptrs(out)
     n_epoch = pos_u.numel() * (1 + m)
     if count is None:
         count = n_epoch - first
     work = _mf_gb_work.get(U.device)
     if work is None:
         work = _mf_gb_work[U.device] = torch.zeros(4, dtype=torch.float64, device=U.device)
-    with torch.cuda.device(U.device):
-        check(lib().eb_mf_pointwise_step_f32(_ptr(U), _ptr(V), _ptr(ub), _ptr(ib), _ptr(gb), d, U.stride(0), _ptr(pos_u), _ptr(pos_i),
-                                             pos_u.numel(), m, n_items, seed, epoch, first, count, lr, reg, _ptr(loss), _ptr(work),
-                                             _ptr(ou), _ptr(oi), _ptr(orr), _stream(U)))
-
-
-_eval_ws = None
+    _call("eb_mf_pointwise_step_f32", U, _ptr(U), _ptr(V), _ptr(ub), _ptr(ib), _ptr(gb), d, U.stride(0), _ptr(pos_u), _ptr(pos_i),
+          pos_u.numel(), m, n_items, seed, epoch, first, count, lr, reg, _ptr(loss), _ptr(work), *out)
 
 
 def eval_topk(topk_idx, k, rel_indptr, rel_items, rel_gains, idcg, discount, users=None, per_user=False):
     """Accuracy metrics of a (rows x >=k) int32 top-k index tensor against an item-sorted relevant-item CSR
     (evaluator.py:117-147 semantics).  Returns (out, per_user): out = device double[5]
     {evaluated users, sum nDCG, sum HR, sum Precision, sum Recall}; per_user = (rows x 4) or None."""
-    global _eval_ws
     _need_cuda(topk_idx, rel_indptr, rel_items, rel_gains, idcg, discount, users)
     assert topk_idx.dtype == torch.int32 and topk_idx.stride(1) == 1 and topk_idx.shape[1] >= k
     assert rel_indptr.dtype == torch.int64 and rel_items.dtype == torch.int32
@@ -1224,17 +1147,12 @@ def eval_topk(topk_idx, k, rel_indptr, rel_items, rel_gains, idcg, discount, use
     dev = topk_idx.device
     out = torch.empty(5, dtype=torch.float64, device=dev)
     pu = torch.empty(n, 4, dtype=torch.float64, device=dev) if per_user else None
-    need = lib().eb_eval_topk_workspace_bytes(n, k)
-    if _eval_ws is None or _eval_ws.numel() < need or _eval_ws.device != dev:
-        _eval_ws = torch.empty(need, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        check(lib().eb_eval_topk_f64(_ptr(topk_idx), n, topk_idx.stride(0), k, _ptr(users), _ptr(rel_indptr), _ptr(rel_items),
-                                     _ptr(rel_gains), _ptr(idcg), _ptr(discount), _ptr(pu), _ptr(out), _ptr(_eval_ws),
-                                     _eval_ws.numel(), _stream(topk_idx)))
+    ws = _scratch("eval_topk", lib().eb_eval_topk_workspace_bytes(n, k), dev)
+    _call("eb_eval_topk_f64", topk_idx, _ptr(topk_idx), n, topk_idx.stride(0), k, _ptr(users), _ptr(rel_indptr), _ptr(rel_items),
+          _ptr(rel_gains), _ptr(idcg), _ptr(discount), _ptr(pu), _ptr(out), _ptr(ws), ws.numel())
     return out, pu
 
 
-_eval_metrics_ws = None
 EVAL_METRICS_SLOTS = 29
 EVAL_METRICS_PER_USER = ("nDCGRendle2020", "MRR", "MAP", "MAR", "F1", "LAUC", "NumRetrieved", "EPC", "EFD", "ARP", "APLT",
                          "ACLT")
@@ -1245,7 +1163,6 @@ def eval_topk_metrics(topk_idx, k, rel_indptr, rel_items, user_info, item_pop, i
     """The reference's ranking, novelty, popularity-bias, coverage and diversity metrics of a (rows x >=k) int32 top-k
     index tensor (eval_metrics.cu; tables as in include/elliot_b200.h).  Returns (out, per_user): out = device
     double[29] of counts, sums and numerators; per_user = (rows x 12) in EVAL_METRICS_PER_USER order, or None."""
-    global _eval_metrics_ws
     _need_cuda(topk_idx, rel_indptr, rel_items, user_info, item_pop, item_long_tail, item_novelty, discount, map_tail,
                inv_binary_idcg, users)
     assert topk_idx.dtype == torch.int32 and topk_idx.stride(1) == 1 and topk_idx.shape[1] >= k
@@ -1264,15 +1181,10 @@ def eval_topk_metrics(topk_idx, k, rel_indptr, rel_items, user_info, item_pop, i
     dev = topk_idx.device
     out = torch.empty(EVAL_METRICS_SLOTS, dtype=torch.float64, device=dev)
     pu = torch.empty(n, len(EVAL_METRICS_PER_USER), dtype=torch.float64, device=dev) if per_user else None
-    need = lib().eb_eval_metrics_workspace_bytes(n, k, n_items)
-    if _eval_metrics_ws is None or _eval_metrics_ws.numel() < need or _eval_metrics_ws.device != dev:
-        _eval_metrics_ws = torch.empty(need, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        check(lib().eb_eval_metrics_f64(_ptr(topk_idx), n, topk_idx.stride(0), k, _ptr(users), _ptr(rel_indptr),
-                                        _ptr(rel_items), _ptr(user_info), _ptr(item_pop), _ptr(item_long_tail),
-                                        _ptr(item_novelty), n_items, _ptr(discount), _ptr(map_tail), _ptr(inv_binary_idcg),
-                                        _ptr(pu), _ptr(out), _ptr(_eval_metrics_ws), _eval_metrics_ws.numel(),
-                                        _stream(topk_idx)))
+    ws = _scratch("eval_metrics", lib().eb_eval_metrics_workspace_bytes(n, k, n_items), dev)
+    _call("eb_eval_metrics_f64", topk_idx, _ptr(topk_idx), n, topk_idx.stride(0), k, _ptr(users), _ptr(rel_indptr),
+          _ptr(rel_items), _ptr(user_info), _ptr(item_pop), _ptr(item_long_tail), _ptr(item_novelty), n_items, _ptr(discount),
+          _ptr(map_tail), _ptr(inv_binary_idcg), _ptr(pu), _ptr(out), _ptr(ws), ws.numel())
     return out, pu
 
 
@@ -1327,9 +1239,8 @@ def bpr_step_peer_f32(U, V_shards, b_shards, shard_rows, d, n_items, tu, ti, tj,
     _need_cuda(U, tu, ti, tj, loss); _chk_idx(tu, ti, tj)
     va, n = _ptr_array(V_shards); ba, nb = _ptr_array(b_shards)
     assert n == nb and U.dtype == torch.float32 and U.stride(1) == 1
-    with torch.cuda.device(U.device):
-        check(lib().eb_bpr_step_peer_f32(_ptr(U), va, ba, n, shard_rows, d, U.stride(0), n_items, _ptr(tu), _ptr(ti), _ptr(tj),
-                                         tu.numel(), lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), _variant, _stream(U)))
+    _call("eb_bpr_step_peer_f32", U, _ptr(U), va, ba, n, shard_rows, d, U.stride(0), n_items, _ptr(tu), _ptr(ti), _ptr(tj),
+          tu.numel(), lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss), _bpr_flags(variant=_variant))
 
 
 def bpr_step_sampled_peer_f32(U, V_shards, b_shards, shard_rows, d, n_users, n_items, indptr, indices, n, seed, first, lr, reg_u,
@@ -1341,24 +1252,17 @@ def bpr_step_sampled_peer_f32(U, V_shards, b_shards, shard_rows, d, n_users, n_i
     assert indptr.dtype == torch.int64 and indices.dtype == torch.int32 and U.dtype == torch.float32 and U.stride(1) == 1
     va, ns = _ptr_array(V_shards); ba, nb = _ptr_array(b_shards)
     assert ns == nb
-    ou = oi = oj = None
-    if out is not None:
-        ou, oi, oj = out
-        _need_cuda(ou, oi, oj); _chk_idx(ou, oi, oj)
-    with torch.cuda.device(U.device):
-        check(lib().eb_bpr_step_sampled_peer_f32(_ptr(U), va, ba, ns, shard_rows, d, U.stride(0), n_users, n_items, _ptr(indptr),
-                                                 _ptr(indices), _ptr(filter), 0 if filter is None else filter.shape[1], n, seed, first, lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(loss),
-                                                 _ptr(ou), _ptr(oi), _ptr(oj), ((int(reserve_sms) & 0xff) << 8) | (4 if _no_item_updates else 0) | int(_variant),
-                                                 _stream(U)))
+    out = _out_ptrs(out)
+    _call("eb_bpr_step_sampled_peer_f32", U, _ptr(U), va, ba, ns, shard_rows, d, U.stride(0), n_users, n_items, _ptr(indptr),
+          _ptr(indices), _ptr(filter), 0 if filter is None else filter.shape[1], n, seed, first, lr, reg_u, reg_b, reg_pos, reg_neg,
+          _ptr(loss), *out, _bpr_flags(no_item_updates=_no_item_updates, variant=_variant, reserve_sms=reserve_sms))
 
 
 def table_reconcile_peer_f32(slice_ptrs, prev_slice, scale, max_ctas=0):
     """One-kernel reconciliation of a replicated table's slice (see eb_table_reconcile_peer_f32)."""
     _need_cuda(prev_slice)
     pa, n = _ptr_array(slice_ptrs)
-    with torch.cuda.device(prev_slice.device):
-        check(lib().eb_table_reconcile_peer_f32(pa, n, _ptr(prev_slice), prev_slice.numel(), float(scale), int(max_ctas),
-                                                _stream(prev_slice)))
+    _call("eb_table_reconcile_peer_f32", prev_slice, pa, n, _ptr(prev_slice), prev_slice.numel(), float(scale), int(max_ctas))
 
 
 def neumf_gather_peer(Umf, Umlp, I_shards, shard_rows, ldi, f, u, it, x0, pm):

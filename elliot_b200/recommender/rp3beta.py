@@ -88,7 +88,7 @@ class RP3Model:
         lists = n * kk * 8 + n * 4
         prune = n * kk * 9 + n * 16
         operands = 2 * (nnz_r * 8 + (max(n, self.n_users) + 1) * 8)
-        rows = int(ops.lib().eb_rp3_row_workspace_bytes(n))
+        rows = ops.rp3_row_workspace_bytes(n)
         g = 2 ** 30
         return lists + prune + operands + rows, (f"the similarity lists {lists / g:.1f} GiB ({n} x {kk} entries), the "
                                                  f"column prune {prune / g:.1f} GiB, the operands {operands / g:.1f} GiB")

@@ -29,6 +29,25 @@ def test_ctypes_table_mirrors_header():
     assert sorted(SIGNATURES) == _header_functions()
 
 
+def test_ctypes_table_types_read_from_header():
+    from ctypes import c_char_p, c_float, c_int, c_int32, c_int64, c_size_t, c_uint32, c_uint64, c_void_p
+    from elliot_b200._lib import SIGNATURES
+    P = c_void_p
+    assert SIGNATURES["eb_last_error"] == (c_char_p, [])
+    assert SIGNATURES["eb_bpr_schedule_sampled"] == (c_int, [c_int32, c_int32, P, c_int64, c_uint64, c_uint64, P, c_size_t, P,
+                                                              c_int, P])
+    assert SIGNATURES["eb_slim_fit_f32"] == (c_int, [P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, c_float, c_float,
+                                                      c_float, c_uint32, c_int, c_int, c_int, c_int32, P, P, P, P, P, P,
+                                                      c_size_t, P])
+
+
+def test_header_type_without_ctypes_mapping_raises():
+    import pytest
+    from elliot_b200._lib import EbError, parse_header
+    with pytest.raises(EbError, match="eb_x.*long"):
+        parse_header("int eb_x(long n, void *stream);")
+
+
 def test_version_and_error_string_without_gpu():
     from elliot_b200._lib import lib
     assert lib().eb_version() >= 100

@@ -76,6 +76,21 @@ def test_cholesky_qr_matches_the_oracle(n, w, rank):
     assert np.abs(Yn[:, :want_rank].T @ Yn[:, :want_rank] - np.eye(want_rank)).max() < 1e-12
 
 
+def test_row_strided_out_matches_contiguous_out():
+    """The sparse and tall-times-small products write row blocks with unit column stride: a [:, :w] view of a wider
+    buffer receives the same bits as a contiguous output, and its padding columns are left alone."""
+    g = np.random.default_rng(3)
+    A = sp.random(500, 300, density=0.05, random_state=3, dtype=np.float32, format="csr")
+    A.data[:] = g.integers(1, 6, A.nnz)
+    Ad, X, M = dev_csr(A), to_dev(g.standard_normal((300, 20))), to_dev(g.standard_normal((20, 12)))
+    wide = torch.full((500, 32), float("nan"), dtype=torch.float64, device=DEV)
+    Y = ops.csr_spmm_f64(Ad, X)
+    assert torch.equal(ops.csr_spmm_f64(Ad, X, out=wide[:, :20]), Y) and torch.isnan(wide[:, 20:]).all()
+    wide = torch.full((500, 16), float("nan"), dtype=torch.float64, device=DEV)
+    Z = ops.tall_times_small_f64(Y, M)
+    assert torch.equal(ops.tall_times_small_f64(Y, M, out=wide[:, :12]), Z) and torch.isnan(wide[:, 12:]).all()
+
+
 @pytest.mark.parametrize("w,rank", [(1, 1), (2, 2), (20, 20), (45, 30), (199, 199), (200, 120)])
 def test_jacobi_eigensolver_matches_eigh(w, rank):
     g = np.random.default_rng(w)
