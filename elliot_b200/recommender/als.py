@@ -98,18 +98,29 @@ class ALSModel:
                              f"this build needs reg > 0 and confidences that keep every weight w = C - 1 (iALS) or "
                              f"C (WRMF) >= 0, for example alpha >= 0 ({e})") from None
 
-    def train_step(self):
-        """One alternating step: iALS_model.py:40-65 / wrmf_model.py:40-58."""
+    def train_step(self, mark=None):
+        """One alternating step: iALS_model.py:40-65 / wrmf_model.py:40-58.  `mark(phase)`, when given, is called as
+        each phase's work has been queued (iALS: gram, user_half, gram, item_half; WRMF: gram, gram, user_half,
+        item_half), so that a caller can time the phases with CUDA events."""
+        mark = mark or (lambda phase: None)
         if self.kind == "iALS":
             ops.gram_f64(self.Y, self.d, out=self.G)
+            mark("gram")
             self._solve(self.G, self.Y, self.users, self.X)
+            mark("user_half")
             ops.gram_f64(self.X, self.d, out=self.G)
+            mark("gram")
             self._solve(self.G, self.X, self.items, self.Y)
+            mark("item_half")
         else:
             ops.gram_f64(self.Y, self.d, out=self.G)
+            mark("gram")
             ops.gram_f64(self.X, self.d, out=self.G2)         # wrmf_model.py:42: X^T X before the user half
+            mark("gram")
             self._solve(self.G, self.Y, self.users, self.X)
+            mark("user_half")
             self._solve(self.G2, self.X, self.items, self.Y)
+            mark("item_half")
 
     def topk(self, k, mask_indptr, mask_indices, users=None):
         return ops.score_topk(self.X, self.Y, None, self.d, k, mask_indptr, mask_indices, users=users)

@@ -55,16 +55,22 @@ class EASEModel:
         return a + max(x, b), (f"the fp64 normal matrix {a / g:.1f} GiB ({n} x {n} x 8 bytes), then either the dense bf16 "
                                f"ratings and a Gram slab {x / g:.1f} GiB or the fp32 weights {b / g:.1f} GiB")
 
-    def initialize(self):
+    def initialize(self, mark=None):
+        """B.  `mark(phase)`, when given, is called as each phase's work has been queued (gram, inverse, weights), so
+        that a caller can time the phases with CUDA events."""
+        mark = mark or (lambda phase: None)
         n = self.n_items
+        self.B = None
         check_free("EASER", self.device, *self.working_set())
         X, s, _ = dense_operand(self.urm, self.n_users, n, "items", who="EASER needs")
         A = torch.empty((n, n), dtype=torch.float64, device=self.device)
         for j0, C in gram_slabs(X, self.n_users, n, "items"):
             ops.ease_normal_f64(C, j0, self.count, self.l2_norm, 4.0 ** -s, A)
         del X, C
+        mark("gram")
         try:
             ops.inverse_f64(A)
+            mark("inverse")
             self.B = ops.ease_weights_f32(A)
         except EbError as e:
             if "error -4" not in str(e):
@@ -74,6 +80,7 @@ class EASEModel:
                 from None
         del A
         self.frac_bits = frac_bits(_bound(self.urm, (None, None, self.B.view(-1))))
+        mark("weights")
 
     def topk(self, k, mask_indptr, mask_indices, users=None, user_begin=0, n_sel=None):
         return ops.dense_score_topk(self.urm, self.B, k, self.frac_bits, mask_indptr, mask_indices, users=users,

@@ -104,16 +104,21 @@ def gram_slabs(X, n_users, n_items, over, slab_rows=None):
         yield j0, C
 
 
-def neighbours(urm, n_users, n_items, over, k, cosine, slab_rows=None):
+def neighbours(urm, n_users, n_items, over, k, cosine, slab_rows=None, mark=None):
     """Neighbour lists of every item (over="items") or user (over="users").  urm: (indptr, indices, values) on the device.
-    Returns (idx int32 [n][k], val fp32 [n][k]): value desc then index asc, -1 / 0 padded."""
+    Returns (idx int32 [n][k], val fp32 [n][k]): value desc then index asc, -1 / 0 padded.  `mark(phase)`, when given, is
+    called as each phase's work has been queued (densify, then gram and neighbours per slab)."""
+    mark = mark or (lambda phase: None)
     X, s, diag = dense_operand(urm, n_users, n_items, over)
+    mark("densify")
     n = n_items if over == "items" else n_users
     idx = torch.empty((n, k), dtype=torch.int32, device=X.device)
     val = torch.empty((n, k), dtype=torch.float32, device=X.device)
     for j0, C in gram_slabs(X, n_users, n_items, over, slab_rows):
+        mark("gram")
         i, v, _ = ops.knn_neighbors(C, n, j0, diag, k, cosine=cosine, dot_scale=4.0 ** -s)
         idx[j0:j0 + C.shape[0]], val[j0:j0 + C.shape[0]] = i, v
+        mark("neighbours")
     return idx, val
 
 
@@ -143,15 +148,20 @@ class KNNModel:
         self.n_users, self.n_items = m.shape
         self.A = self.B = None
 
-    def initialize(self):
+    def initialize(self, mark=None):
+        """W.  `mark(phase)`, when given, is called as each phase's work has been queued (densify, gram, neighbours,
+        transpose), so that a caller can time the phases with CUDA events."""
+        mark = mark or (lambda phase: None)
         if not 1 <= self._k <= 1024:
             raise ValueError(f"neighbors={self._k}: 1 to 1024 are supported")
+        self.A = self.B = None
         n = self.n_items if self._over == "items" else self.n_users
         idx, val = neighbours(self.urm, self.n_users, self.n_items, self._over, min(self._k, max(n, 1)),
-                              self._similarity == "cosine")
+                              self._similarity == "cosine", mark=mark)
         W = transpose_lists(idx, val)
         self.A, self.B = (self.urm, W) if self._over == "items" else (W, self.urm)
         self.frac_bits = frac_bits(_bound(self.A, self.B))
+        mark("transpose")
 
     def topk(self, k, mask_indptr, mask_indices, users=None, user_begin=0, n_sel=None):
         return ops.knn_score_topk(self.A, self.B, self.n_items, k, self.frac_bits, mask_indptr, mask_indices, users=users,

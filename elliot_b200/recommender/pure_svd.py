@@ -91,6 +91,7 @@ class PureSVDModel:
         """The fit.  `mark(phase)`, when given, is called as each phase's work has been queued (upload, spmm, orth,
         eig, finish), so that a caller can time the phases with CUDA events."""
         mark = mark or (lambda phase: None)
+        self.user_vec = self.item_vec = self.s = None
         check_free("PureSVD", self.device, *self.working_set())
         dev = self.device
         a = upload_csr(self._A.indptr, self._A.indices, self._A.data, dev)

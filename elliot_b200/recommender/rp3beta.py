@@ -93,20 +93,30 @@ class RP3Model:
         return lists + prune + operands + rows, (f"the similarity lists {lists / g:.1f} GiB ({n} x {kk} entries), the "
                                                  f"column prune {prune / g:.1f} GiB, the operands {operands / g:.1f} GiB")
 
-    def initialize(self):
+    def initialize(self, mark=None):
+        """W.  `mark(phase)`, when given, is called as each phase's work has been queued (host_prepare, upload,
+        similarity, normalize when it runs, prune), so that a caller can time the phases with CUDA events."""
+        mark = mark or (lambda phase: None)
+        self.W = None
         check_free("RP3beta", self.device, *self.working_set(self.R.nnz))
         pui, piu, degree = self.host_operands()
-        Pui, Piu = upload_csr(*pui, self.device), upload_csr(*piu, self.device)
         # longest rows first: row i costs sum over its users of their rating counts
         work = np.bincount(self.R.indices, weights=np.diff(self.R.indptr)[np.repeat(np.arange(self.n_users),
                                                                                     np.diff(self.R.indptr))],
                            minlength=self.n_items)
-        order = upload(np.argsort(-work, kind="stable"), self.device, torch.int32)
-        idx, val, cnt = ops.rp3_similarity(Piu, Pui, upload(degree, self.device, torch.float64), self.k, order=order)
+        order = np.argsort(-work, kind="stable")
+        mark("host_prepare")
+        Pui, Piu = upload_csr(*pui, self.device), upload_csr(*piu, self.device)
+        deg, order = upload(degree, self.device, torch.float64), upload(order, self.device, torch.int32)
+        mark("upload")
+        idx, val, cnt = ops.rp3_similarity(Piu, Pui, deg, self.k, order=order)
+        mark("similarity")
         del Pui, Piu
         if self.normalize:
             ops.rp3_l1_rows(val, cnt)
+            mark("normalize")
         self.W = ops.rp3_prune_cols(idx, val, cnt, self.k)
+        mark("prune")
 
     def topk(self, k, mask_indptr, mask_indices, users=None, user_begin=0, n_sel=None):
         return sparse_score_topk(self.urm, self.W, self.n_items, k, mask_indptr, mask_indices, users, user_begin, n_sel)

@@ -68,7 +68,11 @@ class SlimModel:
                                                     f"{solver / g:.1f} GiB ({slots} problems at once), W's assembly "
                                                     f"{weights / g:.1f} GiB")
 
-    def initialize(self, shared_residual=None, slots=None):
+    def initialize(self, shared_residual=None, slots=None, mark=None):
+        """W.  `mark(phase)`, when given, is called as each phase's work has been queued (operands, fit, weights), so
+        that a caller can time the phases with CUDA events."""
+        mark = mark or (lambda phase: None)
+        self.W = self.coef_t = self.n_iter = self.gap = self.nnz = None
         shared = ops.slim_shared_residual_fits(self.n_users) if shared_residual is None else bool(shared_residual)
         cap = ops.slim_slots(self.n_users, shared)
         slots = cap if slots is None else max(1, min(int(slots), cap))
@@ -77,10 +81,13 @@ class SlimModel:
         C.sort_indices()
         csc = upload_csr(C.indptr, C.indices, C.data, self.device)
         csr = (self.urm[0], self.urm[1])
+        mark("operands")
         self.coef_t, self.n_iter, self.gap, self.nnz, drop = ops.slim_fit(
             csc, csr, self.n_users, self.n_items, self.l1, self.l2, seed_state(self.seed), self.k,
             shared_residual=shared, slots=slots)
+        mark("fit")
         self.W = ops.slim_weights(self.coef_t, drop, self.nnz, self.k)
+        mark("weights")
 
     def topk(self, k, mask_indptr, mask_indices, users=None, user_begin=0, n_sel=None):
         return sparse_score_topk(self.urm, self.W, self.n_items, k, mask_indptr, mask_indices, users, user_begin, n_sel)

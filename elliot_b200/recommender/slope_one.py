@@ -73,6 +73,7 @@ class SlopeOneModel:
         """E.  `mark(phase)`, when given, is called as each phase's work has been queued (upload, operands, products,
         dev), so that a caller can time the phases with CUDA events."""
         mark = mark or (lambda phase: None)
+        self.train = self.E = None
         check_free("SlopeOne", self.device, *self.working_set())
         n, U = self.n_items, self.n_users
         self.train = upload_csr(self.indptr, self.items, self.ratings, self.device)

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """iALS per-epoch phase timings on one GPU; prints one JSON line.
 
-Per data set and factor count d, CUDA-event times of the phases of one alternating step (elliot_b200/recommender/als.py,
-iALS order): Gram Y^T Y and X^T X (eb_gram_f64, both summed), the user half and the item half (eb_als_solve_f64), and the
-masked top-10 of every user (eb_score_topk_f64).  WRMF runs the same kernels (its two Grams are taken before the user
-half), so it is not timed separately.  One epoch warms up, then --epochs epochs are timed and the mean is reported.
-d <= eb_als_small_d_max() (32) runs the one-row-per-warp mapping, larger d the one-row-per-CTA mapping: d = 10 and
-d = 64 / 200 time both sides of the threshold.
+Per data set and factor count d, ALSModel.train_step (elliot_b200/recommender/als.py, iALS order) and the masked top-10
+of every user (eb_score_topk_f64) are timed through the model's phase marks (tools/benchlib.py): Gram Y^T Y and X^T X
+(eb_gram_f64, both summed), the user half and the item half (eb_als_solve_f64) and the top-10.  WRMF runs the same
+kernels (its two Grams are taken before the user half), so it is not timed separately.  One epoch warms up, then
+--epochs epochs are timed and the median is reported.  d <= eb_als_small_d_max() (32) runs the one-row-per-warp mapping,
+larger d the one-row-per-CTA mapping: d = 10 and d = 64 / 200 time both sides of the threshold.
 
 Rates are counted from shapes: a half costs nnz d^2 fp64 FLOP for the rank-k updates and n_rows d^3 / 3 for the Cholesky
 factorisations (the right-hand sides and triangular solves, 2 nnz d + 2 n_rows d^2, are left out); its bytes are the
@@ -17,37 +17,24 @@ not one reached) and bytes / 3.35 TB/s (data-sheet HBM3 bandwidth); `bound` name
 The reference's per-epoch host time comes from tests/golden/als_c1.npz: the reference's own iALS train_step at C1 shape,
 d = 10, on one host core, timed when the golden was minted, not in this run.
 
-Data sets: C1 = the (user, item) pairs of elliot_b200/synth_c1.py's file (6 040 x 3 706, ~1.0 M entries, no test split);
-ML-20M-shaped = tools/knn_bench.py's generator (138 493 x 26 744, ~18.4 M entries).
+Data sets (benchlib, binarised as sp_i_train is): C1 = the (user, item) pairs of elliot_b200/synth_c1.py's file
+(6 040 x 3 706, ~1.0 M entries, no test split); ML-20M-shaped = 138 493 x 26 744, ~18.4 M entries.
 
     python tools/als_bench.py [--skip-ml20m] [--epochs N]
 """
 import argparse
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
-import scipy.sparse as sp
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from elliot_b200 import ops  # noqa: E402
-from elliot_b200.recommender.als import ALSModel  # noqa: E402
-from knn_bench import c1_matrix, ml20m_matrix  # noqa: E402
+import benchlib as bl
+from elliot_b200 import ops
+from elliot_b200.recommender.als import ALSModel
 
-DEV = "cuda:0"
 PEAK_FP64_TC = 67e12
 PEAK_HBM = 3.35e12
-
-
-class _Data:
-    def __init__(self, u, i, U, I):
-        self.sp_i_train = sp.csr_matrix((np.ones(len(u), np.float32), (u, i)), shape=(U, I), dtype=np.float32)
-        self.users, self.items = range(U), range(I)
 
 
 def _half_cost(nnz, rows, d):
@@ -56,37 +43,19 @@ def _half_cost(nnz, rows, d):
     return flops, nbytes
 
 
-def epoch(m, mask):
-    names = ("gram", "user_half", "item_half", "score_top10")
-    ev = {n: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(2)] for n in names}
-    used = {n: 0 for n in names}
-
-    def timed(name, fn):
-        a, b = ev[name][used[name]]
-        used[name] += 1
-        a.record(); fn(); b.record()
-    torch.cuda.synchronize()
-    timed("gram", lambda: ops.gram_f64(m.Y, m.d, out=m.G))
-    timed("user_half", lambda: m._solve(m.G, m.Y, m.users, m.X))
-    timed("gram", lambda: ops.gram_f64(m.X, m.d, out=m.G))
-    timed("item_half", lambda: m._solve(m.G, m.X, m.items, m.Y))
-    timed("score_top10", lambda: m.topk(10, *mask))
-    torch.cuda.synchronize()
-    return {n: sum(ev[n][j][0].elapsed_time(ev[n][j][1]) for j in range(used[n])) / 1e3 for n in names}
-
-
-def run(u, i, U, I, d, epochs):
-    data = _Data(u, i, U, I)
+def run(data, mask, d, epochs):
     np.random.seed(42)
-    m = ALSModel("iALS", d, data, 1.0, 0.1, 1.0, "linear", DEV)
-    mask = (m.users[0], m.users[1])
-    epoch(m, mask)                                                            # warm-up
-    runs = [epoch(m, mask) for _ in range(epochs)]
-    t = {k: float(np.mean([r[k] for r in runs])) for k in runs[0]}
+    m = ALSModel("iALS", d, data, 1.0, 0.1, 1.0, "linear", bl.DEV)
+
+    def epoch(mark):
+        m.train_step(mark)
+        m.topk(10, *mask)
+        mark("score_top10")
+    t = bl.repeat(epoch, epochs, seconds=True)
     t["epoch_train"] = t["gram"] + t["user_half"] + t["item_half"]
     nnz = int(data.sp_i_train.nnz)
     t["mapping"] = "warp_per_row" if d <= ops.als_small_d_max() else "cta_per_row"
-    for half, rows in (("user_half", U), ("item_half", int(m.items[4].numel()))):
+    for half, rows in (("user_half", data.num_users), ("item_half", int(m.items[4].numel()))):
         fl, by = _half_cost(nnz, rows, d)
         t[f"{half}_tflops"] = fl / t[half] / 1e12
         t[f"{half}_gbytes_per_s"] = by / t[half] / 1e9
@@ -103,22 +72,18 @@ def main():
     ap.add_argument("--skip-ml20m", action="store_true")
     ap.add_argument("--epochs", type=int, default=2)
     args = ap.parse_args()
-    out = {"gpu": torch.cuda.get_device_properties(0).name}
-    try:
-        out["power_limit_w"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
-                                              capture_output=True, text=True).stdout.strip()
-    except OSError:
-        out["power_limit_w"] = "not read"
-    sets = {"c1": (c1_matrix, (10, 64))}
+    out = bl.card()
+    sets = {"c1": (bl.c1_matrix, (10, 64))}
     if not args.skip_ml20m:
-        sets["ml20m_shape"] = (ml20m_matrix, (10, 64, 200))
+        sets["ml20m_shape"] = (bl.ml20m_matrix, (10, 64, 200))
     for name, (make, ds) in sets.items():
-        u, i, _, U, I = make()
+        u, i, r, U, I = make()
+        data, mask = bl.Data(u, i, r, U, I), bl.train_mask(u, i, U)
         out[name] = {"users": U, "items": I, "entries": int(len(u))}
         for d in ds:
-            out[name][f"d{d}"] = run(u, i, U, I, d, args.epochs)
+            out[name][f"d{d}"] = run(data, mask, d, args.epochs)
             torch.cuda.empty_cache()
-    g = np.load(os.path.join(ROOT, "tests", "golden", "als_c1.npz"))
+    g = np.load(os.path.join(bl.ROOT, "tests", "golden", "als_c1.npz"))
     out["reference_c1_ials_d10_epoch_seconds"] = {
         "value": float(np.mean(g["ials_reference_step_seconds"])),
         "note": "the reference's iALS train_step on one host core, timed when the golden was minted, not in this run"}

@@ -9,25 +9,17 @@ calls after `--warmup`; prints one JSON line per shape and k, with the card, its
 import argparse
 import json
 import os
-import subprocess
-import sys
 from types import SimpleNamespace
 
 import numpy as np
 import scipy.sparse as sp
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from elliot_b200 import ops  # noqa: E402
-from elliot_b200.evaluation import metric_tables, position_tables  # noqa: E402
+import benchlib as bl
+from elliot_b200 import ops
+from elliot_b200.evaluation import metric_tables, position_tables
 
 SHAPES = {"C1": (6040, 3706, 1_000_000), "ML-20M": (138493, 26744, 20_000_000)}
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[0] if q else "unknown"
 
 
 def synth(n_users, n_items, nnz, seed=0):
@@ -82,8 +74,8 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: nothing to measure")
     dev = torch.device("cuda:0")
-    gpu = card()
-    ref = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden", "metrics_c1.npz"))
+    gpu = bl.card()
+    ref = np.load(os.path.join(bl.ROOT, "tests", "golden", "metrics_c1.npz"))
     rows = []
     for shape, (n_users, n_items, nnz) in SHAPES.items():
         train, test, logp = synth(n_users, n_items, nnz)
