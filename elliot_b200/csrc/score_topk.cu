@@ -40,6 +40,18 @@ __device__ __forceinline__ bool better(T v, int i, T bv, int bi) {
     return v > bv || (v == bv && v > neg_inf<T>() && i < bi);
 }
 
+// Score of item row vr for the user row su, as every exact scoring path computes it (score_topk_exact_kernel and
+// score_rank_kernel call this; the re-check filter below repeats the order for four items at once): lane-strided fma
+// from 0, the xor-shuffle tree, then bias + acc.  Called by a whole warp; every lane returns the score.
+template <typename T>
+__device__ __forceinline__ T warp_score(const T *su, const T *vr, const T *bias, int it, int d, int lane) {
+    T acc = 0;
+    for (int k = lane; k < d; k += 32) acc = fma(su[k], vr[k], acc);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+    return (bias ? bias[it] : (T)0) + acc;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256) score_topk_exact_kernel(const ScoreParams<T> p) {
     extern __shared__ unsigned char smem_raw[];
@@ -58,12 +70,8 @@ __global__ void __launch_bounds__(256) score_topk_exact_kernel(const ScoreParams
         __syncthreads();
         // phase 1: scores
         for (int it = warp; it < p.n_items; it += 8) {
-            const T *vr = p.V + (int64_t)it * p.ld;
-            T acc = 0;
-            for (int k = lane; k < p.d; k += 32) acc = fma(su[k], vr[k], acc);   // score_topk_tc.cu re-rank mirrors this order
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
-            if (lane == 0) s[it] = (p.bias ? p.bias[it] : (T)0) + acc;
+            const T v = warp_score(su, p.V + (int64_t)it * p.ld, p.bias, it, p.d, lane);   // score_topk_tc.cu re-rank mirrors this order
+            if (lane == 0) s[it] = v;
         }
         __syncthreads();
         // phase 2: train items -> -inf  (BPRMF_model.py:73-74, BPRMF_batch_model.py:88)
@@ -275,6 +283,141 @@ static int score_topk_exact(const T *U, const T *V, const T *bias, int32_t n_ite
     return EB_OK;
 }
 
+// ---------------------------------------------------------------- rank of every relevant item in the full list
+// For one user the full list is what score_topk_exact_kernel lists with k = n_items: every item outside the train mask
+// whose score is neither -inf nor NaN, by (score desc, item asc).  For each relevant item in that list (a positive) the
+// kernel counts the non-relevant entries ahead of it (c_i, the reference's r_i - i in auc.py / gauc.py).  One CTA per
+// row, RANK_CHUNK relevant-CSR entries per pass:
+//   score   : a warp per entry scores the chunk's positives (warp_score: the list's own scores, bit for bit);
+//   sort    : each positive's place in (score desc, item asc) order is the number of positives better than it;
+//   stream  : each warp scores 32 catalogue items, then every lane takes one: an item that is finite, not relevant and
+//             not a train item adds 1 to hist[p], p = the number of positives ahead of it (binary search);
+//   finish  : c of the j-th positive is hist[0] + .. + hist[j], so sum c = sum_p hist[p] * (n - p).
+// Only integer atomics, so the counts do not depend on the order the warps run in.  No score row, no bitmap: any
+// catalogue the scorer takes, and any number of positives (one pass over the catalogue per chunk).
+constexpr int RANK_CHUNK = 1024;
+
+template <typename T>
+struct RankParams {
+    const T *U, *V, *bias;
+    int32_t n_items;
+    int d, ld;
+    const int64_t *mask_indptr;
+    const int32_t *mask_indices;
+    const int64_t *rel_indptr;
+    const int32_t *rel_items;    // item-sorted per row, -1 (never listed) first
+    const int32_t *users;
+    int32_t user_begin;
+    int64_t n_sel;
+    int64_t *n_pos, *sum_c;
+    int64_t *c_out;              // optional, per relevant-CSR entry: c of a positive, -1 otherwise
+};
+
+template <typename T>
+static size_t rank_smem_bytes(int d) {
+    return ((sizeof(T) * (size_t)d + 15) / 16 * 16) + (size_t)RANK_CHUNK * (2 * sizeof(T) + 3 * sizeof(int32_t)) +
+           sizeof(uint32_t) * (RANK_CHUNK + 1);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) score_rank_kernel(const RankParams<T> p) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    T *su = reinterpret_cast<T *>(smem_raw);
+    T *cv = reinterpret_cast<T *>(smem_raw + (sizeof(T) * (size_t)p.d + 15) / 16 * 16);   // chunk scores, entry order
+    T *sv = cv + RANK_CHUNK;                                                              // positives, list order
+    int32_t *ci = reinterpret_cast<int32_t *>(sv + RANK_CHUNK);                           // chunk items, -1: not listed
+    int32_t *si = ci + RANK_CHUNK;                                                        // positives' items
+    int32_t *se = si + RANK_CHUNK;                                                        // their CSR entries
+    uint32_t *hist = reinterpret_cast<uint32_t *>(se + RANK_CHUNK);
+    __shared__ unsigned long long s_sum;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int64_t q = blockIdx.x; q < p.n_sel; q += gridDim.x) {
+        const int u = p.users ? p.users[q] : p.user_begin + (int)q;
+        const int64_t rb = p.rel_indptr[u], re = p.rel_indptr[u + 1];
+        const int64_t mb = p.mask_indptr ? p.mask_indptr[u] : 0;
+        const int mn = p.mask_indptr ? (int)(p.mask_indptr[u + 1] - mb) : 0;
+        const int32_t *mrow = p.mask_indptr ? p.mask_indices + mb : nullptr;
+        __syncthreads();
+        for (int k = threadIdx.x; k < p.d; k += blockDim.x) su[k] = p.U[(int64_t)u * p.ld + k];
+        if (threadIdx.x == 0) s_sum = 0;
+        int64_t n_pos = 0;
+        for (int64_t cb = rb; cb < re; cb += RANK_CHUNK) {
+            const int ne = (int)min((int64_t)RANK_CHUNK, re - cb);
+            __syncthreads();
+            for (int j = warp; j < ne; j += 8) {                                          // score
+                const int32_t it = p.rel_items[cb + j];
+                const bool listed = it >= 0 && it < p.n_items && !contains_sorted(mrow, mn, it);             // warp-uniform
+                const T v = listed ? warp_score(su, p.V + (int64_t)it * p.ld, p.bias, it, p.d, lane) : neg_inf<T>();
+                if (lane == 0) { cv[j] = v; ci[j] = v > neg_inf<T>() ? it : -1; }       // NaN and -inf are not listed
+            }
+            __syncthreads();
+            for (int j = threadIdx.x; j < ne; j += blockDim.x) {                          // sort
+                const T v = cv[j];
+                const int32_t it = ci[j];
+                if (it < 0) {
+                    if (p.c_out) p.c_out[cb + j] = -1;
+                    continue;
+                }
+                int r = 0;
+                for (int o = 0; o < ne; o++) r += ci[o] >= 0 && better<T>(cv[o], ci[o], v, it);
+                sv[r] = v; si[r] = it; se[r] = (int32_t)j;
+            }
+            int n = 0;                                                                    // positives in the chunk
+            for (int j0 = 0; j0 < RANK_CHUNK; j0 += 256) n += __syncthreads_count(j0 + (int)threadIdx.x < ne && ci[j0 + threadIdx.x] >= 0);
+            if (n == 0) continue;
+            for (int j = threadIdx.x; j <= n; j += blockDim.x) hist[j] = 0;
+            __syncthreads();
+            for (int64_t base = (int64_t)warp * 32; base < p.n_items; base += 8 * 32) {  // stream
+                T mine = neg_inf<T>();
+                const int m = (int)min((int64_t)32, p.n_items - base);
+                for (int l = 0; l < m; l++) {
+                    const int32_t it = (int32_t)(base + l);
+                    const T v = warp_score(su, p.V + (int64_t)it * p.ld, p.bias, it, p.d, lane);
+                    if (lane == l) mine = v;
+                }
+                const int32_t it = (int32_t)(base + lane);
+                if (lane < m && mine > neg_inf<T>() && !contains_sorted(p.rel_items + rb, (int)(re - rb), it) &&
+                    !contains_sorted(mrow, mn, it)) {
+                    int lo = 0, hi = n;
+                    while (lo < hi) {
+                        const int mid = (lo + hi) >> 1;
+                        if (better<T>(sv[mid], si[mid], mine, it)) lo = mid + 1; else hi = mid;
+                    }
+                    atomicAdd(hist + lo, 1u);
+                }
+            }
+            __syncthreads();
+            unsigned long long part = 0;                                                  // finish
+            for (int j = threadIdx.x; j <= n; j += blockDim.x) part += (unsigned long long)hist[j] * (unsigned)(n - j);
+            if (part) atomicAdd(&s_sum, part);
+            if (p.c_out && threadIdx.x == 0) {
+                int64_t c = 0;
+                for (int j = 0; j < n; j++) { c += hist[j]; p.c_out[cb + se[j]] = c; }
+            }
+            n_pos += n;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) { p.n_pos[q] = n_pos; p.sum_c[q] = (int64_t)s_sum; }
+    }
+}
+
+template <typename T>
+static int score_rank(const T *U, const T *V, const T *bias, int32_t n_items, int d, int ld, const int64_t *mask_indptr,
+                      const int32_t *mask_indices, const int64_t *rel_indptr, const int32_t *rel_items, const int32_t *users,
+                      int32_t user_begin, int64_t n_sel, int64_t *n_pos, int64_t *sum_c, int64_t *c_out, void *stream) {
+    EB_ARG(U && V && rel_indptr && rel_items && n_pos && sum_c, "null pointer");
+    EB_ARG(d >= 1 && ld >= d && n_items >= 1, "bad shape d=%d ld=%d n_items=%d", d, ld, n_items);
+    EB_ARG((mask_indptr == nullptr) == (mask_indices == nullptr), "mask CSR: both or neither");
+    if (n_sel <= 0) return EB_OK;
+    const size_t smem = rank_smem_bytes<T>(d);
+    if (smem > 48 * 1024) EB_CUDA(cudaFuncSetAttribute(score_rank_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    RankParams<T> p{U, V, bias, n_items, d, ld, mask_indptr, mask_indices, rel_indptr, rel_items, users, user_begin, n_sel,
+                    n_pos, sum_c, c_out};
+    score_rank_kernel<T><<<(unsigned)score_ctas(n_sel), 256, smem, (cudaStream_t)stream>>>(p);
+    EB_CUDA(cudaGetLastError());
+    return EB_OK;
+}
+
 }  // namespace eb
 
 extern "C" size_t eb_score_topk_workspace_bytes(int64_t n_sel, int32_t n_items, int elem_size) {
@@ -345,4 +488,20 @@ extern "C" int eb_score_topk_f32_mapped_dev(const float *U, const float *V, cons
     // whatever the filter could not take (normally nothing): one CTA per row, as eb_score_topk_f32
     return eb::score_topk_exact<float>(U, V, item_bias, n_items, d, ld, mask_indptr, mask_indices, nullptr, user_begin, n_sel_max, k,
                                        out_idx, out_val, ws + off, workspace_bytes - off, stream, ovf_list, ovf_count);
+}
+
+extern "C" int eb_score_rank_f32(const float *U, const float *V, const float *item_bias, int32_t n_items, int d, int ld,
+                                 const int64_t *mask_indptr, const int32_t *mask_indices, const int64_t *rel_indptr,
+                                 const int32_t *rel_items, const int32_t *users, int32_t user_begin, int64_t n_sel,
+                                 int64_t *out_n_pos, int64_t *out_sum_c, int64_t *out_c, void *stream) {
+    return eb::score_rank<float>(U, V, item_bias, n_items, d, ld, mask_indptr, mask_indices, rel_indptr, rel_items, users,
+                                 user_begin, n_sel, out_n_pos, out_sum_c, out_c, stream);
+}
+
+extern "C" int eb_score_rank_f64(const double *U, const double *V, const double *item_bias, int32_t n_items, int d, int ld,
+                                 const int64_t *mask_indptr, const int32_t *mask_indices, const int64_t *rel_indptr,
+                                 const int32_t *rel_items, const int32_t *users, int32_t user_begin, int64_t n_sel,
+                                 int64_t *out_n_pos, int64_t *out_sum_c, int64_t *out_c, void *stream) {
+    return eb::score_rank<double>(U, V, item_bias, n_items, d, ld, mask_indptr, mask_indices, rel_indptr, rel_items, users,
+                                  user_begin, n_sel, out_n_pos, out_sum_c, out_c, stream);
 }

@@ -2,7 +2,9 @@
 (elliot/evaluation/evaluator.py:79-147; ndcg.py:68-125; relevance.py:55,80-82; hit_rate.py, precision.py, recall.py),
 and 19 more of the reference's list metrics (METRICS below: ranking accuracy, novelty, popularity bias, coverage and
 diversity), vectorised over (users x k) index arrays.  tests/test_host_parity.py and tests/test_metrics_host.py check
-them against numbers the reference's own Evaluator produced on the same lists (tests/golden).
+them against numbers the reference's own Evaluator produced on the same lists (tests/golden).  AUC and GAUC rank every
+relevant item in the whole catalogue: they come from the model's rank pass (ops.score_rank, counts per user) through
+finish_auc, not from the lists, and are the same at every cutoff (tests/test_oracle_auc.py).
 
 `eval_tensors` is the device path (SURVEY.md §8f #1): the top-k index tensor written by the scoring kernels is
 scored against the test set by `eb_eval_topk_f64` (the four above) and `eb_eval_metrics_f64` (the 19 others) without
@@ -18,8 +20,13 @@ SUPPORTED = {"ndcg": "nDCG", "hr": "HR", "precision": "Precision", "recall": "Re
 METRICS = ("nDCGRendle2020", "MRR", "MAP", "MAR", "F1", "LAUC", "NumRetrieved", "EPC", "EFD", "ARP", "APLT", "ACLT",
            "PopREO", "PopRSP", "ItemCoverage", "UserCoverage", "UserCoverageAtN", "Gini", "SEntropy")
 _EXTENDED = {m.lower(): m for m in METRICS}
+# metrics of the rank of each relevant item in the whole catalogue: from the model's rank pass (counts per user), not from
+# the top-k lists, and the same at every cutoff; available to an evaluator built with rank_pass=True
+RANK = ("AUC", "GAUC")
+_RANKED = {m.lower(): m for m in RANK}
 _WHY_NOT = {
-    **dict.fromkeys(("auc", "gauc"), "it ranks every item (needs_full_recommendations), not a top-k list"),
+    **dict.fromkeys(("auc", "gauc"), "it ranks every relevant item in the whole catalogue, which takes a model's rank pass "
+                                     "(build the Evaluator with rank_pass=True and give eval() its rank_counts)"),
     **dict.fromkeys(("mae", "mse", "rmse"), "it needs the predicted scores and the test ratings, not a top-k list"),
     **dict.fromkeys(("dsc", "extendedf1", "extendedepc", "extendedefd", "extendedpopreo", "extendedpoprsp"),
                     "it is a complex metric with parameters"),
@@ -155,6 +162,26 @@ def host_metric_sums(tab, cs, priv_users, idx, k, per_user=False):
     return s, pv
 
 
+def finish_auc(n_pos, sum_c, n_rel, n_train, n_items, names):
+    """AUC and GAUC (auc.py, gauc.py) from the rank pass's per-user counts (ops.score_rank): n_pos relevant items in the
+    user's full list and sum_c, the sum over them of the non-relevant entries ahead of each.  With neg_u = n_items -
+    |train_u| - |R_u| + 1 each such item's term is (neg_u - c_i) / neg_u, so a user's terms sum to
+    (n_pos neg_u - sum_c) / neg_u.  AUC is the mean of every term of the users with |R_u| > 0, GAUC the mean over those
+    users of their sum / |R_u|; like np.average([]), no term (or no user) gives NaN, and neg_u = 0 under a term raises
+    ZeroDivisionError, as the reference's int / int does."""
+    n_pos, sum_c, n_rel, n_train = (np.asarray(a, np.int64) for a in (n_pos, sum_c, n_rel, n_train))
+    B = n_rel > 0
+    neg = n_items - n_train - n_rel + 1
+    if (B & (n_pos > 0) & (neg == 0)).any():
+        raise ZeroDivisionError("AUC/GAUC: a user with a ranked relevant item has no negative item (neg_num = 0)")
+    with np.errstate(divide="ignore", invalid="ignore"):
+        user_sum = np.where(n_pos > 0, (n_pos * neg - sum_c) / np.where(neg != 0, neg, 1), 0.0)[B]
+    n_terms, n_users = int(n_pos[B].sum()), int(B.sum())
+    out = {"AUC": float(user_sum.sum() / n_terms) if n_terms else float("nan"),
+           "GAUC": float((user_sum / n_rel[B]).sum() / n_users) if n_users else float("nan")}
+    return {m: out[m] for m in names}
+
+
 def finish_metrics(s, k, n_items, names):
     """Metric values from the slot vector: means over the users each metric averages over (0.0 when there are none,
     like the four accuracy metrics), the ratios of PopREO / PopRSP and the closed forms of Gini and SEntropy."""
@@ -193,7 +220,9 @@ def finish_metrics(s, k, n_items, names):
 
 
 class Evaluator:
-    def __init__(self, data, params):
+    def __init__(self, data, params, rank_pass=False):
+        """rank_pass: the caller supplies rank_counts (a model's ops.score_rank counts) to eval() / eval_tensors(), so
+        AUC and GAUC are available; without it they raise here, like every other name this evaluator cannot compute."""
         self._data, self._params = data, params
         ev = data.config.evaluation
         self._k = getattr(ev, "cutoffs", [data.config.top_k])
@@ -202,7 +231,7 @@ class Evaluator:
             raise Exception("Cutoff values must be smaller than recommendation list length (top_k)")
         self._metrics = []
         for m in ev.simple_metrics:
-            name = SUPPORTED.get(m.lower()) or _EXTENDED.get(m.lower())
+            name = SUPPORTED.get(m.lower()) or _EXTENDED.get(m.lower()) or (_RANKED.get(m.lower()) if rank_pass else None)
             if name is None:
                 why = _WHY_NOT.get(m.lower(), "the reference does not know this name")
                 raise Exception(f"metric {m} is not available in elliot_b200's evaluator: {why} "
@@ -210,19 +239,42 @@ class Evaluator:
             self._metrics.append(name)
         self._basic = [m for m in self._metrics if m in SUPPORTED.values()]
         self._extended = [m for m in self._metrics if m in METRICS]
+        self._ranked = [m for m in self._metrics if m in RANK]
         self._sets = {"test": eval_csr_of(data, "test"), "val": eval_csr_of(data, "val")}
 
     def get_needed_recommendations(self):
         return self._data.config.top_k
 
+    @property
+    def needs_rank(self):
+        """True when AUC or GAUC is asked for: evaluate() then runs the model's rank pass once per split
+        (rank_sets / rank_counts) besides its top-k lists."""
+        return bool(self._ranked)
+
+    def rank_sets(self, device):
+        """{split: (rel indptr int64, item-sorted rel items int32)} on `device` for every split that exists: the
+        arguments of a model's rank pass."""
+        return {w: self._device_set(w, self._k[0], device)[:2] for w in ("val", "test") if self._sets[w] is not None}
+
+    def _rank_values(self, which, rank_counts):
+        """AUC / GAUC of a split from the host (n_pos, sum_c) arrays of its rank pass (rows = private users)."""
+        if not self._ranked:
+            return {}
+        if rank_counts is None:
+            raise Exception(f"{'/'.join(self._ranked)} need the model's rank pass counts (rank_counts)")
+        n_train = np.diff(self._data.sp_i_train.tocsr().indptr)
+        return finish_auc(*rank_counts[which], np.diff(self._sets[which][0]), n_train, self._data.num_items, self._ranked)
+
     # recommendations: (val, test) pair of {public_user: [(public_item, score), ...]}
-    def eval(self, recommendations):
+    # rank_counts: {split: (n_pos, sum_c)} host arrays of the model's rank pass, when AUC or GAUC is asked for
+    def eval(self, recommendations, rank_counts=None):
         out = {}
+        ranked = {w: self._rank_values(w, rank_counts) for w in ("val", "test") if self._sets[w] is not None}
         for k in self._k:
             res = {}
             for slot, which in ((0, "val"), (1, "test")):
                 cs = self._sets[which]
-                res[which] = None if cs is None else self._eval_dict(recommendations[slot], which, k)
+                res[which] = None if cs is None else self._eval_dict(recommendations[slot], which, k, ranked[which])
             if res["val"] is None:
                 res["val"] = res["test"]
             if res["test"] is None:
@@ -278,11 +330,12 @@ class Evaluator:
                           *(t(a, torch.float64) for a in position_tables(k)))
         return cache[key]
 
-    def eval_tensors(self, idx, users=None):
+    def eval_tensors(self, idx, users=None, rank_counts=None):
         """Same result structure as eval(), from a device (rows x top_k) int32 tensor of PRIVATE item ids
         (-1 = empty), row r = private user r (or users[r])."""
         from . import ops
         out = {}
+        ranked = {w: self._rank_values(w, rank_counts) for w in ("val", "test") if self._sets[w] is not None}
         for k in self._k:
             res = {}
             for which in ("val", "test"):
@@ -290,7 +343,7 @@ class Evaluator:
                 if ds is None:
                     res[which] = None
                     continue
-                vals = {}
+                vals = dict(ranked[which])
                 if self._basic:
                     sums, _ = ops.eval_topk(idx, k, *ds, users=users)
                     sums = sums.cpu().numpy()
@@ -308,7 +361,7 @@ class Evaluator:
                       "test_results": res["test"], "test_statistical_results": {}}
         return out
 
-    def _eval_dict(self, recs, which, k):
+    def _eval_dict(self, recs, which, k, ranked):
         pub_u, pub_i = self._data.public_users, self._data.public_items
         users = [u for u in recs if u in pub_u]
         idx = np.full((len(users), k), -1, np.int64)
@@ -321,6 +374,7 @@ class Evaluator:
             tab = self._tables(which)
             s, _ = host_metric_sums(tab, self._sets[which], priv, idx, k)
             vals.update(finish_metrics(s, k, tab.n_items, self._extended))
+        vals.update(ranked)
         return {m: vals[m] for m in self._metrics}
 
     def eval_arrays(self, priv_users, idx, cs, k):

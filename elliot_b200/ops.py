@@ -366,6 +366,28 @@ def score_topk(U, V, bias, d, k, mask_indptr=None, mask_indices=None, users=None
     return idx, val
 
 
+def score_rank(U, V, bias, d, rel_indptr, rel_items, mask_indptr=None, mask_indices=None, users=None, user_begin=0,
+               n_sel=None, per_positive=False):
+    """Rank of every relevant item in the full list score_topk(k=n_items) gives each selected user (the AUC / GAUC
+    counts of auc.py / gauc.py): rel CSR = int64 indptr over user ids, int32 items sorted per user, -1 for items outside
+    the catalogue.  Returns (n_pos, sum_c), int64 per row: the relevant items in the list, and the sum over them of the
+    non-relevant entries ahead of each; per_positive=True adds, per rel CSR entry, that count or -1 (tests)."""
+    _need_cuda(U, V, bias, mask_indptr, mask_indices, users, rel_indptr, rel_items)
+    assert U.dtype in (torch.float32, torch.float64) and V.dtype == U.dtype
+    assert rel_indptr.dtype == torch.int64 and rel_items.dtype == torch.int32 and rel_items.is_contiguous()
+    if users is not None:
+        _chk_idx(users)
+        n_sel = users.numel()
+    elif n_sel is None:
+        n_sel = U.shape[0] - user_begin
+    n_pos, sum_c = (torch.empty(n_sel, dtype=torch.int64, device=U.device) for _ in range(2))
+    c = torch.full((rel_items.numel(),), -1, dtype=torch.int64, device=U.device) if per_positive else None
+    _call("eb_score_rank_f32" if U.dtype == torch.float32 else "eb_score_rank_f64", U, _ptr(U), _ptr(V), _ptr(bias), V.shape[0],
+          d, U.stride(0), _ptr(mask_indptr), _ptr(mask_indices), _ptr(rel_indptr), _ptr(_nonempty(rel_items)), _ptr(users),
+          user_begin, n_sel, _ptr(n_pos), _ptr(sum_c), _ptr(c))
+    return (n_pos, sum_c, c) if per_positive else (n_pos, sum_c)
+
+
 def score_topk_tc(U, V, bias, d, k, mask_indptr=None, mask_indices=None, user_begin=0, n_sel=None, dump=False, stats=True):
     """Tensor-core scoring + top-k (fp32 tables); same result as score_topk().  Returns
     (idx, val, stats) with stats = {"rechecked": users re-done by the exact kernel, "kp": padded K}

@@ -41,6 +41,15 @@ class TopKRecs:
         return recs_dict(self._data, *self.get_recommendations_tensors(k))
 
 
+class RankRecs:
+    """The AUC / GAUC rank pass of a model whose `_model.rank(rel_indptr, rel_items, mask_indptr, mask_indices)` ranks
+    every relevant item in the full lists its `_model.topk` takes the top k of (ops.score_rank on the same tables)."""
+
+    def get_rank_tensors(self, rel_indptr, rel_items):
+        """(n_pos, sum_c) int64 device tensors, rows = private users."""
+        return self._model.rank(rel_indptr, rel_items, self._indptr, self._sorted_idx)
+
+
 def upload(a, device, dtype):
     """A numpy array on the device as a contiguous tensor of `dtype`, in its stored order."""
     return torch.from_numpy(np.ascontiguousarray(a)).to(device, dtype)

@@ -27,7 +27,7 @@ from .. import ops
 from .._lib import EbError
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
-from ._device import TopKRecs, cuda_device, upload
+from ._device import RankRecs, TopKRecs, cuda_device, upload
 
 MAX_FACTORS = 200              # the top of the reference's own search range (config_files/recsys_config.yml, iALS block)
 
@@ -125,8 +125,11 @@ class ALSModel:
     def topk(self, k, mask_indptr, mask_indices, users=None):
         return ops.score_topk(self.X, self.Y, None, self.d, k, mask_indptr, mask_indices, users=users)
 
+    def rank(self, rel_indptr, rel_items, mask_indptr, mask_indices):
+        return ops.score_rank(self.X, self.Y, None, self.d, rel_indptr, rel_items, mask_indptr, mask_indices)
 
-class _ALS(TopKRecs, RecMixin, BaseRecommenderModel):
+
+class _ALS(TopKRecs, RankRecs, RecMixin, BaseRecommenderModel):
     _kind = None
 
     def _check(self):

@@ -24,7 +24,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
-from ._device import TopKRecs, cuda_device
+from ._device import RankRecs, TopKRecs, cuda_device
 
 
 class MFModel:
@@ -86,6 +86,9 @@ class MFModel:
             return idx, val
         return ops.score_topk(self.U, self.V, self.b, self._factors, k, mask_indptr, mask_indices, users=users)
 
+    def rank(self, rel_indptr, rel_items, mask_indptr, mask_indices):
+        return ops.score_rank(self.U, self.V, self.b, self._factors, rel_indptr, rel_items, mask_indptr, mask_indices)
+
     # ---- state (BPRMF_model.py:119-139) ----------------------------------------------------
     def get_model_state(self):
         F = self._factors
@@ -107,7 +110,7 @@ class MFModel:
             pickle.dump(self.get_model_state(), f)
 
 
-class BPRMF(TopKRecs, RecMixin, BaseRecommenderModel):
+class BPRMF(TopKRecs, RankRecs, RecMixin, BaseRecommenderModel):
     r"""Bayesian Personalized Ranking MF (https://arxiv.org/abs/1205.2618) on the H100.
 
     YAML block identical to the reference's (BPRMF.py:37-56):

@@ -17,7 +17,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
-from ._device import TopKRecs, cuda_device
+from ._device import RankRecs, TopKRecs, cuda_device
 
 
 class BPRMFBatchModel:
@@ -61,6 +61,10 @@ class BPRMFBatchModel:
             return idx, val
         return ops.score_topk(self.Gu, self.Gi, bias, self._factors, k, mask_indptr, mask_indices)
 
+    def rank(self, rel_indptr, rel_items, mask_indptr, mask_indices):
+        return ops.score_rank(self.Gu, self.Gi, self.Bi[:self._num_items], self._factors, rel_indptr, rel_items, mask_indptr,
+                              mask_indices)
+
     def get_model_state(self):
         F = self._factors
         return {"Bi": self.Bi[:self._num_items].cpu().numpy(), "Gu": self.Gu[:, :F].cpu().numpy(),
@@ -85,7 +89,7 @@ class BPRMFBatchModel:
             self.set_model_state(pickle.load(f))
 
 
-class BPRMF_batch(TopKRecs, RecMixin, BaseRecommenderModel):
+class BPRMF_batch(TopKRecs, RankRecs, RecMixin, BaseRecommenderModel):
     r"""Batch BPR-MF (Adam).  YAML keys as in the reference (BPRMF_batch.py:37-48):
     `epochs, batch_size, factors, lr, l_w, l_b`."""
 

@@ -69,6 +69,11 @@ class GeneralizedMatrixFactorizationModel:
             idx, val = ops.score_topk(Uh, self.P["I"], None, self.f, k, mask_indptr, mask_indices)
         return idx, ops.sigmoid_(val.contiguous())
 
+    def rank(self, rel_indptr, rel_items, mask_indptr, mask_indices):
+        """The lists get_recs_topk() selects from: (U*h) . I^T before the sigmoid."""
+        Uh = ops.gmf_scale_rows(self.P["U"], self.P["h"], self.fp)
+        return ops.score_rank(Uh, self.P["I"], None, self.f, rel_indptr, rel_items, mask_indptr, mask_indices)
+
     def get_model_state(self):
         return {"P": {k: v.cpu().numpy() for k, v in self.P.items()}, "step": self.step,
                 "M": {k: v.cpu().numpy() for k, v in self.M.items()}, "V": {k: v.cpu().numpy() for k, v in self.V.items()}}
@@ -133,3 +138,6 @@ class GMF(RecMixin, BaseRecommenderModel):
 
     def get_recommendations_tensors(self, k: int = 10):
         return self._model.get_recs_topk(k, self._indptr, self._sorted_idx)
+
+    def get_rank_tensors(self, rel_indptr, rel_items):
+        return self._model.rank(rel_indptr, rel_items, self._indptr, self._sorted_idx)

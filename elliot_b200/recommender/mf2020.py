@@ -21,7 +21,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
-from ._device import TopKRecs, cuda_device, upload
+from ._device import RankRecs, TopKRecs, cuda_device, upload
 
 
 class RendleSampler:
@@ -95,6 +95,10 @@ class MF2020Model:
             idx, val = ops.score_topk(self.U, self.V, self.ib, self._factors, k, mask_indptr, mask_indices)
         return idx, val + (self.ub + self.gb).to(val.dtype).unsqueeze(1)
 
+    def rank(self, rel_indptr, rel_items, mask_indptr, mask_indices):
+        """The lists topk() selects from: ib + U.V, without the per-user constant."""
+        return ops.score_rank(self.U, self.V, self.ib, self._factors, rel_indptr, rel_items, mask_indptr, mask_indices)
+
     def load_weights(self, path):
         with open(path, "rb") as f:
             self.set_model_state(pickle.load(f))
@@ -104,7 +108,7 @@ class MF2020Model:
             pickle.dump(self.get_model_state(), f)
 
 
-class MF2020(TopKRecs, RecMixin, BaseRecommenderModel):
+class MF2020(TopKRecs, RankRecs, RecMixin, BaseRecommenderModel):
     r"""Matrix Factorization as in "NCF vs. MF Revisited" (https://dl.acm.org/doi/pdf/10.1145/3383313.3412488) on the H100.
 
     YAML block identical to the reference's (MF.py:41-52): MF2020: {meta: {...}, epochs, factors, lr, reg, m};

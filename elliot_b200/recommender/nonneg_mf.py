@@ -24,7 +24,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
-from ._device import TopKRecs, check_free, cuda_device, upload
+from ._device import RankRecs, TopKRecs, check_free, cuda_device, upload
 from .slope_one import dict_order_csr
 
 
@@ -89,6 +89,10 @@ class NonNegMFModel:
         bu = self.bu if users is None else self.bu[users.long()]
         return idx, (val + bu.unsqueeze(1)) + float(self._mu)
 
+    def rank(self, rel_indptr, rel_items, mask_indptr, mask_indices):
+        """The lists topk() selects from: P[u].Q[i] + bi[i], without the per-user terms."""
+        return ops.score_rank(self.P, self.Q, self.bi, self.F, rel_indptr, rel_items, mask_indptr, mask_indices)
+
     def get_model_state(self):
         return {"_user_bias": self.bu.cpu().numpy(), "_item_bias": self.bi.cpu().numpy(),
                 "_user_embeddings": self.P.cpu().numpy(), "_item_embeddings": self.Q.cpu().numpy()}
@@ -107,7 +111,7 @@ class NonNegMFModel:
             pickle.dump(self.get_model_state(), f)
 
 
-class NonNegMF(TopKRecs, RecMixin, BaseRecommenderModel):
+class NonNegMF(TopKRecs, RankRecs, RecMixin, BaseRecommenderModel):
     r"""Non-Negative Matrix Factorization (https://ieeexplore.ieee.org/document/6748996) on the H100.
 
     YAML block as the reference's: NonNegMF: {meta: {...}, epochs, batch_size, factors, lr, reg}; optional keys

@@ -31,7 +31,7 @@ import torch
 from .. import ops
 from ..dataset import train_csr_of
 from ._bases import BaseRecommenderModel, RecMixin, init_charger
-from ._device import TopKRecs, check_free, cuda_device, upload, upload_csr
+from ._device import RankRecs, TopKRecs, check_free, cuda_device, upload, upload_csr
 
 OVERSAMPLES = 10                # sklearn's n_oversamples default
 
@@ -122,8 +122,11 @@ class PureSVDModel:
     def topk(self, k, mask_indptr, mask_indices, users=None):
         return ops.score_topk(self.user_vec, self.item_vec, None, self.d, k, mask_indptr, mask_indices, users=users)
 
+    def rank(self, rel_indptr, rel_items, mask_indptr, mask_indices):
+        return ops.score_rank(self.user_vec, self.item_vec, None, self.d, rel_indptr, rel_items, mask_indptr, mask_indices)
 
-class PureSVD(TopKRecs, RecMixin, BaseRecommenderModel):
+
+class PureSVD(TopKRecs, RankRecs, RecMixin, BaseRecommenderModel):
     r"""PureSVD (https://link.springer.com/chapter/10.1007/978-0-387-85820-3_5), on the H100.  YAML block as the
     reference's: PureSVD: {meta: {...}, factors, seed}; optional keys `b200_eval` and `b200_device`."""
 

@@ -20,15 +20,21 @@ class RecMixin:
         on_device = (getattr(self._params, "b200_eval", "host") == "device" and hasattr(self, "get_recommendations_tensors")
                      and hasattr(self.evaluator, "eval_tensors") and not self._save_recs and not self._negative_sampling)
         self._losses.append(loss)
+        counts = None
+        if self.evaluator.needs_rank:
+            # AUC / GAUC: every relevant item's rank in the whole catalogue, from the model's rank pass once per split;
+            # the lists stay top_k
+            counts = {w: tuple(t.cpu().numpy() for t in self.get_rank_tensors(*rel))
+                      for w, rel in self.evaluator.rank_sets(self._device).items()}
         if on_device:
             # extension: the (users x k) index tensor goes from the scoring kernel straight into the metric
             # kernel; no {user: [(item, score)]} dicts are built (recommender_utils_mixin.py:84-88 / evaluator.py:117-147)
             idx, _ = self.get_recommendations_tensors(self.evaluator.get_needed_recommendations())
             recs = None
-            self._results.append(self.evaluator.eval_tensors(idx))
+            self._results.append(self.evaluator.eval_tensors(idx, rank_counts=counts))
         else:
             recs = self.get_recommendations(self.evaluator.get_needed_recommendations())
-            self._results.append(self.evaluator.eval(recs))
+            self._results.append(self.evaluator.eval(recs, rank_counts=counts))
         if it is not None:
             self.logger.info(f"Epoch {it + 1}/{self._epochs} loss {loss / (it + 1):.5f}")
         else:

@@ -40,10 +40,11 @@ def write_tsv(path, seed=SEED):
     return checksum(u, i, r)
 
 
-def experiment_yaml(tsv, out_dir, model_key, block, meta=("save_recs: True",), extra="", model_extra=""):
+def experiment_yaml(tsv, out_dir, model_key, block, meta=("save_recs: True",), extra="", model_extra="",
+                    metrics=("nDCG", "HR", "Precision", "Recall")):
     """The reference's YAML layout (sample_hello_world.yml:1-19) over the C1 file above: one `model_key` block with the
-    given `meta` lines (without indentation) and parameter lines (`block`, indented, newline-ended).
-    `extra` goes into the experiment section, `model_extra` after the model's parameters."""
+    given `meta` lines (without indentation) and parameter lines (`block`, indented, newline-ended), evaluated with
+    `metrics`.  `extra` goes into the experiment section, `model_extra` after the model's parameters."""
     meta = "".join(f"        {m}\n" for m in meta)
     return f"""experiment:
   dataset: c1_synth
@@ -56,7 +57,7 @@ def experiment_yaml(tsv, out_dir, model_key, block, meta=("save_recs: True",), e
       test_ratio: 0.2
   top_k: 10
   evaluation:
-    simple_metrics: [nDCG, HR, Precision, Recall]
+    simple_metrics: [{', '.join(metrics)}]
   path_output_rec_result: {out_dir}/recs
   path_output_rec_weight: {out_dir}/weights
   path_output_rec_performance: {out_dir}/performance
@@ -116,8 +117,10 @@ def nonneg_mf_yaml(tsv, out_dir, extra="", model_extra=""):
                            "      lr: 0.001\n      reg: 0.1\n", extra=extra, model_extra=model_extra)
 
 
-def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra="", seed=42):
-    """A `BPRMF:` block with BPRMF.py:43-56 keys, the reference's default hyper-parameters, save_recs and verbose off."""
+def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra="", seed=42, save_recs=True,
+              metrics=("nDCG", "HR", "Precision", "Recall")):
+    """A `BPRMF:` block with BPRMF.py:43-56 keys, the reference's default hyper-parameters, save_recs (unless
+    save_recs=False) and verbose off, evaluated with `metrics`."""
     return experiment_yaml(tsv, out_dir, model_key, f"""      epochs: {epochs}
       factors: {factors}
       lr: 0.05
@@ -126,4 +129,4 @@ def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra=""
       positive_item_regularization: 0.0025
       negative_item_regularization: 0.00025
       seed: {seed}
-""", meta=("save_recs: True", "verbose: False"), extra=extra, model_extra=model_extra)
+""", meta=(f"save_recs: {save_recs}", "verbose: False"), extra=extra, model_extra=model_extra, metrics=metrics)

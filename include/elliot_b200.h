@@ -203,6 +203,31 @@ int eb_score_topk_f64(const double *U, const double *V, const double *item_bias,
                       int32_t *out_idx, double *out_val, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------
+ * Rank of every relevant item in the user's full list (the AUC / GAUC
+ * counts of elliot/evaluation/metrics/accuracy/AUC/auc.py, gauc.py).
+ * The full list is what eb_score_topk_* lists with k = n_items: every item
+ * outside the train mask whose score (the same bits) is neither -inf nor
+ * NaN, by (score desc, item asc).  Same scoring arguments and row choice as
+ * eb_score_topk_*; rel CSR (indexed by user id): the user's relevant items,
+ * sorted by item, -1 for items outside the catalogue.  Per row q:
+ *   out_n_pos[q] = number of relevant items in the list (positives),
+ *   out_sum_c[q] = sum over them of the non-relevant entries ahead of each.
+ * out_c (optional, one per rel CSR entry of the selected users): that count
+ * for a positive, -1 for an entry that is not in the list.  Integer counts:
+ * the results do not depend on launch order.  No workspace.
+ * ------------------------------------------------------------------------ */
+int eb_score_rank_f32(const float *U, const float *V, const float *item_bias, int32_t n_items, int d, int ld,
+                      const int64_t *mask_indptr, const int32_t *mask_indices,
+                      const int64_t *rel_indptr, const int32_t *rel_items,
+                      const int32_t *users, int32_t user_begin, int64_t n_sel,
+                      int64_t *out_n_pos, int64_t *out_sum_c, int64_t *out_c, void *stream);
+int eb_score_rank_f64(const double *U, const double *V, const double *item_bias, int32_t n_items, int d, int ld,
+                      const int64_t *mask_indptr, const int32_t *mask_indices,
+                      const int64_t *rel_indptr, const int32_t *rel_items,
+                      const int32_t *users, int32_t user_begin, int64_t n_sel,
+                      int64_t *out_n_pos, int64_t *out_sum_c, int64_t *out_c, void *stream);
+
+/* ------------------------------------------------------------------------
  * Mini-batch BPR-MF with Adam (the reference's TensorFlow variant).
  * Replaces BPRMF_batch_model.call/train_step (BPRMF_batch_model.py:46-80):
  * eb_bpr_batch_grad_f32 accumulates the batch gradient of
