@@ -10,18 +10,17 @@
 //    the scatter-add.  Each lane of a warp first fetches/samples ONE triple (coalesced
 //    index loads or Philox), the groups then walk the warp's 32 triples with shuffles,
 //    prefetching the next triple's rows while the current one is reduced.
+//  * bpr_rounds_kernel   — the same update in deterministic rounds (flags bit 6).
 //  * bpr_grouped_kernel  — the free-running sampled step on local tables: the same update, applied to the triples
 //    grouped by user (user_key_kernel + a stable radix sort first), the user row kept in registers across a run.
-//  * bpr_exact_kernel   — exact mode, fp64.  Same arithmetic, but sequentially
-//    consistent with the array order of the triples: every row carries a turn counter,
-//    a triple waits until each of its three rows has seen exactly the touches that
-//    precede it in the sequence (ranks come from a radix sort of (row, position)).
+//  * bpr_hogwild_stage_kernel — the update on peer item tables with the rows staged through shared memory.
+// Exact mode (fp64) is in bpr_exact.cu, the sampler in bpr_sampler.cuh and its stand-alone kernels in bpr_sample.cu.
 #include <cooperative_groups.h>
 #include <cub/cub.cuh>
-#include <stdlib.h>
 
 #include <type_traits>
 
+#include "bpr_sampler.cuh"
 #include "bpr_update.cuh"
 
 namespace eb {
@@ -33,87 +32,25 @@ struct HogwildParams {
     int64_t n;
     BprHyper hp;
     double *loss;
-    // sampler
-    int32_t n_users, n_items;
-    const int64_t *indptr;
-    const int32_t *indices;
-    uint64_t seed, first;
+    SamplerParams sampler;
     int32_t *out_u, *out_i, *out_j;
     // PEER mode (item table row-sharded over the GPUs of one NVSwitch box, SURVEY.md §8e): shard s holds item rows
     // [s*shards.rows, (s+1)*shards.rows) at Vp[s] / bp[s] — local memory for this rank's shard, peer-mapped memory
     // (cudaIpcOpenMemHandle, peer.cu) for the others; loads and vector atomics go straight over NVLink.
     float *Vp[EB_MAX_PEERS], *bp[EB_MAX_PEERS];
     ShardMap shards;
-    // optional per-user membership signatures (eb_bloom_build): filter_log2bits bits per user
-    const uint32_t *filter;
-    int filter_log2bits;
     // optional PACKED triples (host boundary: 8 B instead of 12 B per triple over PCIe): u | i << bits_u | j << (bits_u + bits_i)
     const uint64_t *packed;
     int bits_u, bits_i;
-    int no_item_updates;      // profiling only (flags bit 2): item rows are read but not updated
     // grouped sampled step: the call's triple indices ordered by user (ascending u, then ascending t)
     const int32_t *order;
 };
-
-// u of triple t: uniform over the users that own at least one and not every item.  r keeps the Philox block that drew the
-// accepted u (its other words pick i and j), beg / len the user's CSR row.
-__device__ __forceinline__ void sample_user(const HogwildParams &p, int64_t t, uint32_t (&r)[4], int &u, int64_t &beg, int &len) {
-    Philox::gen(p.seed, p.first + (uint64_t)t, 0u, r);
-    u = (int)bounded(r[0], (uint32_t)p.n_users);
-    beg = __ldg(p.indptr + u);
-    int64_t end = __ldg(p.indptr + u + 1);
-    len = (int)(end - beg);
-    uint32_t attempt = 0;
-    while (len == 0 || len >= p.n_items) {  // users without train items never appear in the reference's dict; a user owning
-                                            // every item has no negative at all (the reference would loop forever)
-        Philox::gen(p.seed, p.first + (uint64_t)t, ++attempt | 0x80000000u, r);
-        u = (int)bounded(r[0], (uint32_t)p.n_users);
-        beg = __ldg(p.indptr + u); end = __ldg(p.indptr + u + 1); len = (int)(end - beg);
-    }
-}
-
-// u uniform over users, i uniform over the user's train items, j uniform over the
-// complement (rejection against the sorted CSR row) — custom_sampler.py:31-42 semantics,
-// Philox stream instead of MT19937.
-__device__ __forceinline__ void sample_triple(const HogwildParams &p, int64_t t, int &u, int &i, int &j) {
-    uint32_t r[4];
-    int64_t beg;
-    int len;
-    sample_user(p, t, r, u, beg, len);
-    uint32_t attempt = 0;
-    const int32_t *row = p.indices + beg;
-    int cand = (int)bounded(r[2], (uint32_t)p.n_items);
-    // the signature words depend on u only: their loads are in flight together with the pick of i
-    const bool maybe = p.filter ? bloom_maybe(p.filter + ((int64_t)u << (p.filter_log2bits - 5)), p.filter_log2bits, (uint32_t)cand) : true;
-    i = __ldg(row + bounded(r[1], (uint32_t)len));
-    if (!maybe || !contains_sorted(row, len, cand)) { j = cand; return; }
-    cand = (int)bounded(r[3], (uint32_t)p.n_items);
-    attempt = 0;
-    int q = 4;
-    while (contains_sorted(row, len, cand) && attempt < 16u) {
-        if (q == 4) { Philox::gen(p.seed, p.first + (uint64_t)t, ++attempt, r); q = 0; }
-        cand = (int)bounded(r[q++], (uint32_t)p.n_items);
-    }
-    if (attempt >= 16u && contains_sorted(row, len, cand)) {
-        // near-dense user: stop rejecting and draw the rank-th item of the complement directly (same uniform
-        // distribution over the non-train items, never a train item): smallest pos with row[pos] - pos > rank
-        Philox::gen(p.seed, p.first + (uint64_t)t, 0x40000000u, r);          // a fresh block: independent of the rejected candidates
-        const uint32_t rank = bounded(r[0], (uint32_t)(p.n_items - len));
-        int lo = 0, hi = len;
-        while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if ((uint32_t)(__ldg(row + mid) - mid) > rank) hi = mid; else lo = mid + 1;
-        }
-        cand = (int)rank + lo;
-    }
-    j = cand;
-}
 
 // triple t: sampled (and written to out_* when asked), unpacked from the 8-byte host format, or read from three arrays
 template <bool SAMPLE>
 __device__ __forceinline__ void fetch_triple(const HogwildParams &p, int64_t t, int &u, int &i, int &j) {
     if (SAMPLE) {
-        sample_triple(p, t, u, i, j);
+        sample_triple(p.sampler, t, u, i, j);
         if (p.out_u) { p.out_u[t] = u; p.out_i[t] = i; p.out_j[t] = j; }
     } else if (p.packed) {
         const uint64_t w = __ldg(p.packed + t);
@@ -143,109 +80,53 @@ struct Rows {
     float bi, bj;
 };
 
-// ROUNDS (opt-in, flags bit 6 / deterministic=True in ops) makes the step deterministic.  The launch is cooperative and runs in
-// rounds: every warp loads the rows of UNR triples per lane group, computes their updates from those values, the whole grid
-// waits, every warp adds its updates, the grid waits again.  A triple therefore reads exactly the values left by the
-// previous rounds — which round a triple falls into is fixed by its index and the grid size, not by timing — so the same
-// inputs give the same tables on every run (up to the order in which one round's atomic adds to a shared row land, i.e.
-// fp32 rounding).  Staleness stays bounded by one round (the grid's lane groups x UNR triples).  The barriers cost
-// throughput (the row loads of one round no longer overlap the previous round's atomics), so the default is free-running
-// Hogwild; rounds exist for local tables with atomic updates only.
-template <int DP, bool SAMPLE, bool ATOMIC, bool PEER, bool ROUNDS = false>
+// the lane's share of the rows and the biases of triple (u, i, j), nothing for u < 0; peer rows with system-scope loads
+template <int DP, bool PEER>
+__device__ __forceinline__ void load_rows(const HogwildParams &p, int gl, Rows<LaneGroup<DP>::VPL> &r, int u, int i, int j) {
+    constexpr int G = LaneGroup<DP>::G, VPL = LaneGroup<DP>::VPL;
+    if (u >= 0) {
+        float *ri, *rj, *bi, *bj;
+        item_row<PEER>(p, i, ri, bi); item_row<PEER>(p, j, rj, bj);
+        const float4 *pu = reinterpret_cast<const float4 *>(p.U + (int64_t)u * p.ld);
+        const float4 *pi = reinterpret_cast<const float4 *>(ri);
+        const float4 *pj = reinterpret_cast<const float4 *>(rj);
+#pragma unroll
+        for (int v = 0; v < VPL; v++) {
+            r.u[v] = pu[v * G + gl];
+            r.vi[v] = PEER ? ld_sys_v4(pi + v * G + gl) : pi[v * G + gl];
+            r.vj[v] = PEER ? ld_sys_v4(pj + v * G + gl) : pj[v * G + gl];
+        }
+        r.bi = *bi;
+        r.bj = *bj;
+    }
+}
+
+// W: how the item rows and biases are written.  Write::AtomicSys is the peer-table kernel (item rows in the owner shard's
+// memory); the user row, always local, takes GPU-scope atomics unless the step is the racy plain-store one.
+template <int DP, bool SAMPLE, Write W>
 __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p) {
-    static_assert(!ROUNDS || (ATOMIC && !PEER), "deterministic rounds: local tables, atomic updates");
-    constexpr int NV = DP / 4;                 // float4 per row
-    constexpr int G = NV >= 32 ? 32 : NV;      // lanes per triple
-    constexpr int VPL = NV / G;                // float4 per lane
-    const int lane = threadIdx.x & 31;
-    const int gl = lane % G;
-    const int gbase = lane - gl;
-    const int64_t warp_id = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    using LG = LaneGroup<DP>;
+    constexpr int G = LG::G, VPL = LG::VPL, UNR = LG::UNR;
+    constexpr bool PEER = W == Write::AtomicSys;
+    constexpr Write WU = W == Write::Store ? Write::Store : Write::Atomic;
+    const LG lg;
     const int64_t ld = p.ld;
     float loss_acc = 0.f;
 
-    auto load_rows = [&](Rows<VPL> &r, int u, int i, int j) {
-        if (u >= 0) {
-            float *ri, *rj, *bi, *bj;
-            item_row<PEER>(p, i, ri, bi); item_row<PEER>(p, j, rj, bj);
-            const float4 *pu = reinterpret_cast<const float4 *>(p.U + (int64_t)u * ld);
-            const float4 *pi = reinterpret_cast<const float4 *>(ri);
-            const float4 *pj = reinterpret_cast<const float4 *>(rj);
-#pragma unroll
-            for (int v = 0; v < VPL; v++) {
-                r.u[v] = pu[v * G + gl];
-                r.vi[v] = PEER ? ld_sys_v4(pi + v * G + gl) : pi[v * G + gl];
-                r.vj[v] = PEER ? ld_sys_v4(pj + v * G + gl) : pj[v * G + gl];
-            }
-            r.bi = *bi;
-            r.bj = *bj;
-        }
-    };
-
-    // ROUNDS: every warp runs the same number of iterations (idle ones with u = -1), so all of them reach every grid barrier
     const int64_t n_tiles = (p.n + 31) / 32;
-    const int64_t tile_end = ROUNDS ? (n_tiles + nwarps - 1) / nwarps * nwarps : n_tiles;
-    for (int64_t tile = warp_id; tile < tile_end; tile += nwarps) {
-        const int64_t t = tile * 32 + lane;
+    for (int64_t tile = lg.warp; tile < n_tiles; tile += lg.nwarps) {
+        const int64_t t = tile * 32 + lg.lane;
         int u = -1, i = 0, j = 0;
         if (t < p.n) fetch_triple<SAMPLE>(p, t, u, i, j);
         // UNR triples of the group in flight at once: all their row loads are issued before the first reduction
-        constexpr int UNR = G >= 4 ? 4 : G;
 #pragma unroll 1
         for (int s0 = 0; s0 < G; s0 += UNR) {
             Rows<VPL> rw[UNR];
             int tu_[UNR], ti_[UNR], tj_[UNR];
 #pragma unroll
             for (int q = 0; q < UNR; q++) {
-                tu_[q] = __shfl_sync(0xffffffffu, u, gbase + s0 + q);
-                ti_[q] = __shfl_sync(0xffffffffu, i, gbase + s0 + q);
-                tj_[q] = __shfl_sync(0xffffffffu, j, gbase + s0 + q);
-                load_rows(rw[q], tu_[q], ti_[q], tj_[q]);
-            }
-            if constexpr (ROUNDS) {
-                // ---- read phase: scores and updates of this round's triples from the values the previous rounds left; each
-                // triple's updates overwrite its rows in rw (registers: the rows are dead once the updates are formed)
-#pragma unroll
-                for (int q = 0; q < UNR; q++) {
-                    Rows<VPL> &cur = rw[q];
-                    float part = 0.f;
-                    if (tu_[q] >= 0) {
-#pragma unroll
-                        for (int v = 0; v < VPL; v++) part += bpr_partial_dot(cur.u[v], cur.vi[v], cur.vj[v]);
-                    }
-                    part = group_sum<G>(part);
-                    if (tu_[q] >= 0) {
-                        const float z = bpr_sigmoid_loss(part + (cur.bi - cur.bj), loss_acc, gl);
-#pragma unroll
-                        for (int v = 0; v < VPL; v++) {
-                            float4 du, di, dj;
-                            bpr_row_deltas(cur.u[v], cur.vi[v], cur.vj[v], z, p.hp, du, di, dj);
-                            cur.u[v] = du; cur.vi[v] = di; cur.vj[v] = dj;
-                        }
-                        float dbi, dbj;
-                        bpr_bias_deltas(z, cur.bi, cur.bj, p.hp, dbi, dbj);
-                        cur.bi = dbi; cur.bj = dbj;
-                    }
-                }
-                cooperative_groups::this_grid().sync();      // every read of this round is done
-                // ---- write phase
-#pragma unroll
-                for (int q = 0; q < UNR; q++) {
-                    if (tu_[q] < 0) continue;
-                    float *pu = p.U + (int64_t)tu_[q] * ld, *pi, *pj, *pbi, *pbj;
-                    item_row<PEER>(p, ti_[q], pi, pbi); item_row<PEER>(p, tj_[q], pj, pbj);
-#pragma unroll
-                    for (int v = 0; v < VPL; v++) {
-                        const int e = (v * G + gl) * 4;
-                        red_add_v4(pu + e, rw[q].u[v]);
-                        red_add_v4(pi + e, rw[q].vi[v]);
-                        red_add_v4(pj + e, rw[q].vj[v]);
-                    }
-                    if (gl == 0) { red_add_f32(pbi, rw[q].bi); red_add_f32(pbj, rw[q].bj); }
-                }
-                cooperative_groups::this_grid().sync();      // every write of this round has landed before the next reads
-                continue;
+                bcast_triple(u, i, j, lg.gbase + s0 + q, tu_[q], ti_[q], tj_[q]);
+                load_rows<DP, PEER>(p, lg.gl, rw[q], tu_[q], ti_[q], tj_[q]);
             }
 #pragma unroll
             for (int q = 0; q < UNR; q++) {
@@ -258,7 +139,7 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
                 }
                 part = group_sum<G>(part);
                 if (cu >= 0) {
-                    const float z = bpr_sigmoid_loss(part + (cur.bi - cur.bj), loss_acc, gl);
+                    const float z = bpr_sigmoid_loss(part + (cur.bi - cur.bj), loss_acc, lg.gl);
                     float *pu = p.U + (int64_t)cu * ld, *pi, *pj, *pbi, *pbj;
                     item_row<PEER>(p, ci, pi, pbi); item_row<PEER>(p, cj, pj, pbj);
 #pragma unroll
@@ -266,39 +147,100 @@ __global__ void __launch_bounds__(256) bpr_hogwild_kernel(const HogwildParams p)
                         const float4 a = cur.u[v], vi = cur.vi[v], vj = cur.vj[v];
                         float4 du, di, dj;
                         bpr_row_deltas(a, vi, vj, z, p.hp, du, di, dj);
-                        const int e = (v * G + gl) * 4;
-                        if (PEER) {
-                            red_add_v4(pu + e, du);
-                            if (!p.no_item_updates) {
-                                red_add_v4_sys(pi + e, di);
-                                red_add_v4_sys(pj + e, dj);
-                            }
-                        } else if (ATOMIC) {
-                            red_add_v4(pu + e, du);
-                            red_add_v4(pi + e, di);
-                            red_add_v4(pj + e, dj);
-                        } else {
-                            *reinterpret_cast<float4 *>(pu + e) = make_float4(a.x + du.x, a.y + du.y, a.z + du.z, a.w + du.w);
-                            *reinterpret_cast<float4 *>(pi + e) = make_float4(vi.x + di.x, vi.y + di.y, vi.z + di.z, vi.w + di.w);
-                            *reinterpret_cast<float4 *>(pj + e) = make_float4(vj.x + dj.x, vj.y + dj.y, vj.z + dj.z, vj.w + dj.w);
-                        }
+                        const int e = (v * G + lg.gl) * 4;
+                        write_row<WU>(pu + e, a, du);
+                        write_row<W>(pi + e, vi, di);
+                        write_row<W>(pj + e, vj, dj);
                     }
-                    if (gl == 0) {
+                    if (lg.gl == 0) {
                         float dbi, dbj;
                         bpr_bias_deltas(z, cur.bi, cur.bj, p.hp, dbi, dbj);
-                        if (PEER) { red_add_f32_sys(pbi, dbi); red_add_f32_sys(pbj, dbj); }
-                        else if (ATOMIC) { red_add_f32(pbi, dbi); red_add_f32(pbj, dbj); }
-                        else { *pbi = cur.bi + dbi; *pbj = cur.bj + dbj; }
+                        write_bias<W>(pbi, cur.bi, dbi);
+                        write_bias<W>(pbj, cur.bj, dbj);
                     }
                 }
             }
         }
     }
-    if (p.loss) {
+    flush_loss(loss_acc, p.loss, lg.lane);
+}
+
+// Deterministic rounds (opt-in, flags bit 6 / deterministic=True in ops) make the step deterministic.  The launch is
+// cooperative and runs in rounds: every warp loads the rows of UNR triples per lane group, computes their updates from those
+// values, the whole grid waits, every warp adds its updates, the grid waits again.  A triple therefore reads exactly the
+// values left by the previous rounds — which round a triple falls into is fixed by its index and the grid size, not by
+// timing — so the same inputs give the same tables on every run (up to the order in which one round's atomic adds to a
+// shared row land, i.e. fp32 rounding).  Staleness stays bounded by one round (the grid's lane groups x UNR triples).  The
+// barriers cost throughput (the row loads of one round no longer overlap the previous round's atomics), so the default is
+// free-running Hogwild; rounds exist for local tables with atomic updates only.
+template <int DP, bool SAMPLE>
+__global__ void __launch_bounds__(256) bpr_rounds_kernel(const HogwildParams p) {
+    using LG = LaneGroup<DP>;
+    constexpr int G = LG::G, VPL = LG::VPL, UNR = LG::UNR;
+    const LG lg;
+    const int64_t ld = p.ld;
+    float loss_acc = 0.f;
+
+    // every warp runs the same number of iterations (idle ones with u = -1), so all of them reach every grid barrier
+    const int64_t n_tiles = (p.n + 31) / 32;
+    const int64_t tile_end = (n_tiles + lg.nwarps - 1) / lg.nwarps * lg.nwarps;
+    for (int64_t tile = lg.warp; tile < tile_end; tile += lg.nwarps) {
+        const int64_t t = tile * 32 + lg.lane;
+        int u = -1, i = 0, j = 0;
+        if (t < p.n) fetch_triple<SAMPLE>(p, t, u, i, j);
+#pragma unroll 1
+        for (int s0 = 0; s0 < G; s0 += UNR) {
+            Rows<VPL> rw[UNR];
+            int tu_[UNR], ti_[UNR], tj_[UNR];
 #pragma unroll
-        for (int off = 16; off > 0; off >>= 1) loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, off);
-        if (lane == 0 && loss_acc != 0.f) atomicAdd(p.loss, (double)loss_acc);
+            for (int q = 0; q < UNR; q++) {
+                bcast_triple(u, i, j, lg.gbase + s0 + q, tu_[q], ti_[q], tj_[q]);
+                load_rows<DP, false>(p, lg.gl, rw[q], tu_[q], ti_[q], tj_[q]);
+            }
+            // ---- read phase: scores and updates of this round's triples from the values the previous rounds left; each
+            // triple's updates overwrite its rows in rw (registers: the rows are dead once the updates are formed)
+#pragma unroll
+            for (int q = 0; q < UNR; q++) {
+                Rows<VPL> &cur = rw[q];
+                float part = 0.f;
+                if (tu_[q] >= 0) {
+#pragma unroll
+                    for (int v = 0; v < VPL; v++) part += bpr_partial_dot(cur.u[v], cur.vi[v], cur.vj[v]);
+                }
+                part = group_sum<G>(part);
+                if (tu_[q] >= 0) {
+                    const float z = bpr_sigmoid_loss(part + (cur.bi - cur.bj), loss_acc, lg.gl);
+#pragma unroll
+                    for (int v = 0; v < VPL; v++) {
+                        float4 du, di, dj;
+                        bpr_row_deltas(cur.u[v], cur.vi[v], cur.vj[v], z, p.hp, du, di, dj);
+                        cur.u[v] = du; cur.vi[v] = di; cur.vj[v] = dj;
+                    }
+                    float dbi, dbj;
+                    bpr_bias_deltas(z, cur.bi, cur.bj, p.hp, dbi, dbj);
+                    cur.bi = dbi; cur.bj = dbj;
+                }
+            }
+            cooperative_groups::this_grid().sync();      // every read of this round is done
+            // ---- write phase
+#pragma unroll
+            for (int q = 0; q < UNR; q++) {
+                if (tu_[q] < 0) continue;
+                float *pu = p.U + (int64_t)tu_[q] * ld, *pi, *pj, *pbi, *pbj;
+                item_row<false>(p, ti_[q], pi, pbi); item_row<false>(p, tj_[q], pj, pbj);
+#pragma unroll
+                for (int v = 0; v < VPL; v++) {
+                    const int e = (v * G + lg.gl) * 4;
+                    red_add_v4(pu + e, rw[q].u[v]);
+                    red_add_v4(pi + e, rw[q].vi[v]);
+                    red_add_v4(pj + e, rw[q].vj[v]);
+                }
+                if (lg.gl == 0) { red_add_f32(pbi, rw[q].bi); red_add_f32(pbj, rw[q].bj); }
+            }
+            cooperative_groups::this_grid().sync();      // every write of this round has landed before the next reads
+        }
     }
+    flush_loss(loss_acc, p.loss, lg.lane);
 }
 
 // ---------------------------------------------------------------- grouped sampled step (local tables, free-running)
@@ -317,28 +259,23 @@ __global__ void __launch_bounds__(256) user_key_kernel(const HogwildParams p, ui
         uint32_t r[4];
         int u, len;
         int64_t beg;
-        sample_user(p, t, r, u, beg, len);
+        sample_user(p.sampler, t, r, u, beg, len);
         key[t] = (uint32_t)u; val[t] = (int32_t)t;
     }
 }
 
-template <int DP, bool ATOMIC>
+// W: Write::Atomic, or Write::Store for the racy step (the run's row `cur` is stored instead of acc added)
+template <int DP, Write W>
 __global__ void __launch_bounds__(256) bpr_grouped_kernel(const HogwildParams p) {
-    constexpr int NV = DP / 4;                 // float4 per row
-    constexpr int G = NV >= 32 ? 32 : NV;      // lanes per triple
-    constexpr int VPL = NV / G;                // float4 per lane
-    constexpr int UNR = G >= 4 ? 4 : G;        // triples of the slice whose rows are in flight at once
-    const int lane = threadIdx.x & 31;
-    const int gl = lane % G;
-    const int gbase = lane - gl;
-    const int64_t warp_id = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    using LG = LaneGroup<DP>;
+    constexpr int G = LG::G, VPL = LG::VPL, UNR = LG::UNR;
+    const LG lg;
     const int64_t ld = p.ld;
     float loss_acc = 0.f;
 
     const int64_t n_tiles = (p.n + 31) / 32;
-    for (int64_t tile = warp_id; tile < n_tiles; tile += nwarps) {
-        const int64_t pos = tile * 32 + lane;
+    for (int64_t tile = lg.warp; tile < n_tiles; tile += lg.nwarps) {
+        const int64_t pos = tile * 32 + lg.lane;
         int u = -1, i = 0, j = 0;
         if (pos < p.n) fetch_triple<true>(p, __ldg(p.order + pos), u, i, j);
         // the group's run: user cu (-1: none yet), its row as the run left it, the run's summed update
@@ -348,8 +285,8 @@ __global__ void __launch_bounds__(256) bpr_grouped_kernel(const HogwildParams p)
             float *pu = p.U + (int64_t)cu * ld;
 #pragma unroll
             for (int v = 0; v < VPL; v++) {
-                float *e = pu + (v * G + gl) * 4;
-                if (ATOMIC) red_add_v4(e, acc[v]);
+                float *e = pu + (v * G + lg.gl) * 4;
+                if (W == Write::Atomic) red_add_v4(e, acc[v]);
                 else *reinterpret_cast<float4 *>(e) = cur[v];
             }
         };
@@ -359,20 +296,18 @@ __global__ void __launch_bounds__(256) bpr_grouped_kernel(const HogwildParams p)
             int tu_[UNR], ti_[UNR], tj_[UNR];
 #pragma unroll
             for (int q = 0; q < UNR; q++) {
-                tu_[q] = __shfl_sync(0xffffffffu, u, gbase + s0 + q);
-                ti_[q] = __shfl_sync(0xffffffffu, i, gbase + s0 + q);
-                tj_[q] = __shfl_sync(0xffffffffu, j, gbase + s0 + q);
+                bcast_triple(u, i, j, lg.gbase + s0 + q, tu_[q], ti_[q], tj_[q]);
                 if (tu_[q] >= 0) {
                     // the user row only where a run starts: inside a run the row is `cur`
                     if (tu_[q] != (q == 0 ? cu : tu_[q - 1])) {
                         const float4 *pu = reinterpret_cast<const float4 *>(p.U + (int64_t)tu_[q] * ld);
 #pragma unroll
-                        for (int v = 0; v < VPL; v++) rw[q].u[v] = pu[v * G + gl];
+                        for (int v = 0; v < VPL; v++) rw[q].u[v] = pu[v * G + lg.gl];
                     }
                     const float4 *pi = reinterpret_cast<const float4 *>(p.V + (int64_t)ti_[q] * ld);
                     const float4 *pj = reinterpret_cast<const float4 *>(p.V + (int64_t)tj_[q] * ld);
 #pragma unroll
-                    for (int v = 0; v < VPL; v++) { rw[q].vi[v] = pi[v * G + gl]; rw[q].vj[v] = pj[v * G + gl]; }
+                    for (int v = 0; v < VPL; v++) { rw[q].vi[v] = pi[v * G + lg.gl]; rw[q].vj[v] = pj[v * G + lg.gl]; }
                     rw[q].bi = p.b[ti_[q]];
                     rw[q].bj = p.b[tj_[q]];
                 }
@@ -395,7 +330,7 @@ __global__ void __launch_bounds__(256) bpr_grouped_kernel(const HogwildParams p)
                 }
                 part = group_sum<G>(part);
                 if (qu >= 0) {
-                    const float z = bpr_sigmoid_loss(part + (nx.bi - nx.bj), loss_acc, gl);
+                    const float z = bpr_sigmoid_loss(part + (nx.bi - nx.bj), loss_acc, lg.gl);
                     float *pi = p.V + (int64_t)qi * ld, *pj = p.V + (int64_t)qj * ld;
 #pragma unroll
                     for (int v = 0; v < VPL; v++) {
@@ -404,35 +339,26 @@ __global__ void __launch_bounds__(256) bpr_grouped_kernel(const HogwildParams p)
                         bpr_row_deltas(a, vi, vj, z, p.hp, du, di, dj);
                         cur[v] = make_float4(a.x + du.x, a.y + du.y, a.z + du.z, a.w + du.w);
                         acc[v] = start ? du : make_float4(acc[v].x + du.x, acc[v].y + du.y, acc[v].z + du.z, acc[v].w + du.w);
-                        const int e = (v * G + gl) * 4;
-                        if (ATOMIC) {
-                            red_add_v4(pi + e, di);
-                            red_add_v4(pj + e, dj);
-                        } else {
-                            *reinterpret_cast<float4 *>(pi + e) = make_float4(vi.x + di.x, vi.y + di.y, vi.z + di.z, vi.w + di.w);
-                            *reinterpret_cast<float4 *>(pj + e) = make_float4(vj.x + dj.x, vj.y + dj.y, vj.z + dj.z, vj.w + dj.w);
-                        }
+                        const int e = (v * G + lg.gl) * 4;
+                        write_row<W>(pi + e, vi, di);
+                        write_row<W>(pj + e, vj, dj);
                     }
-                    if (gl == 0) {
+                    if (lg.gl == 0) {
                         float dbi, dbj;
                         bpr_bias_deltas(z, nx.bi, nx.bj, p.hp, dbi, dbj);
-                        if (ATOMIC) { red_add_f32(p.b + qi, dbi); red_add_f32(p.b + qj, dbj); }
-                        else { p.b[qi] = nx.bi + dbi; p.b[qj] = nx.bj + dbj; }
+                        write_bias<W>(p.b + qi, nx.bi, dbi);
+                        write_bias<W>(p.b + qj, nx.bj, dbj);
                     }
                 }
             }
         }
         if (cu >= 0) flush();
     }
-    if (p.loss) {
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, off);
-        if (lane == 0 && loss_acc != 0.f) atomicAdd(p.loss, (double)loss_acc);
-    }
+    flush_loss(loss_acc, p.loss, lg.lane);
 }
 
 // ---------------------------------------------------------------- staged variant of the Hogwild kernel (PEER mode only)
-// Same update, same sampler, same atomics as bpr_hogwild_kernel<..., PEER = true>; the difference is HOW the three
+// Same update, same sampler, same atomics as bpr_hogwild_kernel<..., Write::AtomicSys>; the difference is HOW the three
 // embedding rows of a triple reach the SM.  There every lane group loads "its" rows into registers (4 triples in flight per group, 118
 // registers, 16 warps/SM) and the loads of a round cannot start before the previous round's arithmetic has retired.
 // Here every lane, as soon as it has sampled its triple, hands the three rows to the copy engine
@@ -445,16 +371,15 @@ __global__ void __launch_bounds__(256) bpr_grouped_kernel(const HogwildParams p)
 constexpr int STAGE_CHUNK_BYTES = 4096;
 template <int DP, bool SAMPLE>
 __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildParams p) {
-    constexpr int NV = DP / 4;                 // float4 per row
-    constexpr int G = NV >= 32 ? 32 : NV;      // lanes per triple
-    constexpr int VPL = NV / G;                // float4 per lane
+    using LG = LaneGroup<DP>;
+    constexpr int NV = LG::NV, G = LG::G, VPL = LG::VPL;
     constexpr int ROWB = DP * 4;
     constexpr int TT = STAGE_CHUNK_BYTES / ROWB;  // triples per chunk (32 / 16 / 8 at 4 KB of rows per row kind)
     constexpr int NGRP = 32 / G;               // triples processed side by side
     static_assert(TT >= NGRP && TT <= 32 && 32 % TT == 0, "chunk shape");
     extern __shared__ __align__(128) uint8_t stage_smem[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const int gl = lane % G, grp = lane / G;
+    const LG lg;
+    const int lane = lg.lane, gl = lg.gl, wib = threadIdx.x >> 5, grp = lane / G;
     uint8_t *wbuf = stage_smem + (size_t)wib * (TT * 3 * ROWB);          // [TT][3][ROWB]
     uint64_t *bars = reinterpret_cast<uint64_t *>(stage_smem + (size_t)(blockDim.x >> 5) * (TT * 3 * ROWB));
     const uint32_t bar = (uint32_t)__cvta_generic_to_shared(bars + wib);
@@ -465,12 +390,10 @@ __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildPar
     }
     __syncwarp();
     uint32_t phase = 0;
-    const int64_t warp_id = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     const int64_t ld = p.ld;
     float loss_acc = 0.f;
 
-    for (int64_t tile = warp_id; tile * 32 < p.n; tile += nwarps) {
+    for (int64_t tile = lg.warp; tile * 32 < p.n; tile += lg.nwarps) {
         const int64_t t = tile * 32 + lane;
         int u = -1, i = 0, j = 0;
         float bi = 0.f, bj = 0.f;
@@ -514,7 +437,8 @@ __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildPar
             for (int s = 0; s < TT; s += NGRP) {
                 const int q = s + grp;                                             // triple slot inside the chunk
                 const int src = c0 + q;                                            // lane that sampled it
-                const int cu = __shfl_sync(0xffffffffu, u, src), ci = __shfl_sync(0xffffffffu, i, src), cj = __shfl_sync(0xffffffffu, j, src);
+                int cu, ci, cj;
+                bcast_triple(u, i, j, src, cu, ci, cj);
                 const float cbi = __shfl_sync(0xffffffffu, bi, src), cbj = __shfl_sync(0xffffffffu, bj, src);
                 const bool on = cu >= 0;
                 const float4 *su = reinterpret_cast<const float4 *>(wbuf + (size_t)q * (3 * ROWB));
@@ -537,7 +461,8 @@ __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildPar
                         bpr_row_deltas(a[v], vi[v], vj[v], z, p.hp, du, di, dj);
                         const int e = (v * G + gl) * 4;
                         red_add_v4(gu + e, du);
-                        if (!p.no_item_updates) { red_add_v4_sys(gi + e, di); red_add_v4_sys(gj + e, dj); }
+                        red_add_v4_sys(gi + e, di);
+                        red_add_v4_sys(gj + e, dj);
                     }
                     if (gl == 0) {
                         float dbi, dbj;
@@ -548,13 +473,10 @@ __global__ void __launch_bounds__(256) bpr_hogwild_stage_kernel(const HogwildPar
             }
         }
     }
-    if (p.loss) {
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, off);
-        if (lane == 0 && loss_acc != 0.f) atomicAdd(p.loss, (double)loss_acc);
-    }
+    flush_loss(loss_acc, p.loss, lane);
 }
 
+// ---------------------------------------------------------------- host side
 // Persistent grid of 256-thread CTAs: one CTA per 8 tiles of 32 triples (a tile per warp), at most what stays resident on the
 // SMs left after `reserve_sms` (SMs left free for a concurrent collective (NCCL) kernel).
 static int persistent_grid(const void *kern, int smem, int64_t n, int reserve_sms, unsigned &grid) {
@@ -571,127 +493,55 @@ static int persistent_grid(const void *kern, int smem, int64_t n, int reserve_sm
     return EB_OK;
 }
 
-template <int DP, bool SAMPLE>
-static int launch_stage_t(const HogwildParams &p, int reserve_sms, cudaStream_t st) {
-    constexpr int SMEM = 8 * 3 * STAGE_CHUNK_BYTES + 64;   // 8 warps x 3 row kinds x chunk + mbarriers
-    auto kern = bpr_hogwild_stage_kernel<DP, SAMPLE>;
-    EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+using StepKernel = void (*)(HogwildParams);
+
+// kern on the persistent grid; the rounds kernel is launched cooperatively, so every CTA is resident for its grid barriers
+static int launch_persistent(StepKernel kern, const HogwildParams &p, int reserve_sms, cudaStream_t st, int smem = 0,
+                             bool cooperative = false) {
     unsigned grid;
-    if (int rc = persistent_grid((const void *)kern, SMEM, p.n, reserve_sms, grid)) return rc;
-    kern<<<grid, 256, SMEM, st>>>(p);
-    EB_CUDA(cudaGetLastError());
-    return EB_OK;
-}
-
-// one warp per user: OR the two signature bits of every train item into the user's words
-__global__ void __launch_bounds__(256) bloom_build_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
-                                                          int32_t n_users, int log2bits, uint32_t *__restrict__ out) {
-    const int lane = threadIdx.x & 31;
-    int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const int words = 1 << (log2bits - 5);
-    for (; w < n_users; w += nw) {
-        uint32_t *f = out + w * words;
-        for (int k = lane; k < words; k += 32) f[k] = 0u;
-        __syncwarp();
-        const int64_t beg = indptr[w], end = indptr[w + 1];
-        for (int64_t e = beg + lane; e < end; e += 32) {
-            uint32_t a, b;
-            bloom_bits((uint32_t)indices[e], log2bits, a, b);
-            atomicOr(f + (a >> 5), 1u << (a & 31));
-            atomicOr(f + (b >> 5), 1u << (b & 31));
-        }
-        __syncwarp();
-    }
-}
-
-__global__ void __launch_bounds__(256) philox_sample_kernel(const HogwildParams p) {
-    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; t < p.n; t += stride) {
-        int u, i, j;
-        sample_triple(p, t, u, i, j);
-        p.out_u[t] = u; p.out_i[t] = i; p.out_j[t] = j;
-    }
-}
-
-// pointwise_pos_neg_sampler.py:24-48: u uniform; one fair bit decides between a uniform train item of u (label 1) and a
-// uniform non-train item (label 0).  The BPR sampler already draws both for u: keep one of them.
-__global__ void __launch_bounds__(256) pointwise_sample_kernel(const HogwildParams p, float *__restrict__ out_label) {
-    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; t < p.n; t += stride) {
-        int u, i, j;
-        sample_triple(p, t, u, i, j);
-        uint32_t r[4];
-        Philox::gen(p.seed, p.first + (uint64_t)t, 0x20000000u, r);
-        const bool pos = (r[0] >> 31) != 0;
-        p.out_u[t] = u; p.out_i[t] = pos ? i : j; out_label[t] = pos ? 1.f : 0.f;
-    }
-}
-
-template <int DP, bool SAMPLE, bool ATOMIC, bool PEER, bool ROUNDS>
-static int launch_hogwild_t(const HogwildParams &p, int reserve_sms, cudaStream_t st) {
-    auto kern = bpr_hogwild_kernel<DP, SAMPLE, ATOMIC, PEER, ROUNDS>;
-    unsigned grid;
-    if (int rc = persistent_grid((const void *)kern, 0, p.n, reserve_sms, grid)) return rc;
-    if (ROUNDS) {
-        // deterministic rounds (see bpr_hogwild_kernel): a cooperative launch, so every CTA is resident for the grid barriers
+    if (int rc = persistent_grid((const void *)kern, smem, p.n, reserve_sms, grid)) return rc;
+    if (cooperative) {
         void *args[] = {const_cast<HogwildParams *>(&p)};
-        EB_CUDA(cudaLaunchCooperativeKernel((const void *)kern, dim3(grid), dim3(256), args, 0, st));
+        EB_CUDA(cudaLaunchCooperativeKernel((const void *)kern, dim3(grid), dim3(256), args, smem, st));
     } else {
-        kern<<<grid, 256, 0, st>>>(p);
+        kern<<<grid, 256, smem, st>>>(p);
     }
     EB_CUDA(cudaGetLastError());
     return EB_OK;
 }
 
-// f(std::integral_constant<int, DP>{}) for the row stride DP == dp among the compiled ones (DPS), else EB_ERR_ARG
+// The flags word of the eb_bpr_step_* entry points (include/elliot_b200.h)
+struct StepFlags {
+    bool racy;      // bit 0: plain stores instead of atomics
+    bool no_sync;   // bit 1: the host-triple step returns without synchronising its stream
+    bool reg;       // bit 4: peer tables: the register kernel instead of the shared-memory-staged one
+    bool stage;     // bit 5: the shared-memory-staged kernel (peer tables only)
+    bool rounds;    // bit 6: deterministic rounds
+    int reserve;    // bits 8..15: SMs the grids leave free
+};
+
+static int decode_flags(int flags, StepFlags &f) {
+    EB_ARG(!(flags & 4), "flags bit 2 is not a BPR step option (item-row updates cannot be switched off)");
+    f = StepFlags{(flags & 1) != 0, (flags & 2) != 0, (flags & 16) != 0, (flags & 32) != 0, (flags & 64) != 0, (flags >> 8) & 0xff};
+    return EB_OK;
+}
+
+// The compiled row strides of each table kind
+template <int... DPS>
+struct Strides {};
+using LocalStrides = Strides<8, 16, 32, 64, 128, 256>;
+using PeerStrides = Strides<32, 64, 128>;            // sharded item tables
+
+// f(std::integral_constant<int, DP>{}) for the row stride DP == dp among the compiled ones, else EB_ERR_ARG
 template <int... DPS, class F>
-static int with_stride(int dp, const char *strides, F &&f) {
+static int with_stride(Strides<DPS...>, int dp, F &&f) {
     int rc = EB_OK;
-    const bool found = ((dp == DPS && (rc = f(std::integral_constant<int, DPS>{}), true)) || ...);
-    return found ? rc : set_err(EB_ERR_ARG, "row stride ld=%d must be one of %s", dp, strides);
+    if (((dp == DPS && (rc = f(std::integral_constant<int, DPS>{}), true)) || ...)) return rc;
+    char list[64];
+    int len = 0;
+    ((len += snprintf(list + len, sizeof list - len, len ? ",%d" : "%d", DPS)), ...);
+    return set_err(EB_ERR_ARG, "row stride ld=%d must be one of %s floats", dp, list);
 }
-
-// EB_L2_PERSIST=1: mark the item table's address range as persisting in L2 for the launch's stream (cudaAccessPolicyWindow) when it
-// fits the device's persisting carve-out — the table is hit by two of every triple's three row accesses, the user table and the
-// CSR are streamed once.  An A/B switch, off by default.
-static void item_table_l2_window(const HogwildParams &p, cudaStream_t st) {
-    static const int env = [] { const char *e = getenv("EB_L2_PERSIST"); return e ? atoi(e) : 0; }();
-    if (!env || !p.V) return;
-    static int max_persist = -1, max_window = 0;
-    if (max_persist < 0) {
-        int dev = 0; cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, dev);
-        cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, dev);
-    }
-    const size_t bytes = (size_t)p.n_items * (size_t)p.ld * sizeof(float);
-    if (max_persist <= 0 || bytes > (size_t)max_persist || bytes > (size_t)max_window) return;
-    static size_t carved = 0;                 // the carve-out is sized to the table, not to the device maximum
-    if (carved != bytes) { cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, bytes); carved = bytes; }
-    cudaStreamAttrValue attr{};
-    attr.accessPolicyWindow.base_ptr = (void *)p.V;
-    attr.accessPolicyWindow.num_bytes = bytes;
-    attr.accessPolicyWindow.hitRatio = 1.0f;
-    attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    attr.accessPolicyWindow.missProp = env == 2 ? cudaAccessPropertyNormal : cudaAccessPropertyStreaming;
-    cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &attr);
-}
-
-template <int DP, bool ATOMIC>
-static int launch_grouped_t(const HogwildParams &p, int reserve_sms, cudaStream_t st) {
-    auto kern = bpr_grouped_kernel<DP, ATOMIC>;
-    unsigned grid;
-    if (int rc = persistent_grid((const void *)kern, 0, p.n, reserve_sms, grid)) return rc;
-    kern<<<grid, 256, 0, st>>>(p);
-    EB_CUDA(cudaGetLastError());
-    return EB_OK;
-}
-
-static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
-
-static int bits_for(uint64_t v) { int b = 1; while ((v >> b) != 0) b++; return b; }
 
 // The grouped step sorts the triple indices of at most GROUP_MAX triples at a time (int32 offsets); longer calls run as
 // consecutive sub-steps of that size.
@@ -721,83 +571,71 @@ static GroupLayout group_layout(int64_t n, int32_t n_users) {
 }
 
 // The schedule of one sub-step (p.n <= GROUP_MAX): the user keys and the stable sort of the triple indices by user.  Reads
-// only seed, first, n, n_users, n_items and indptr, never the tables.  The ordered indices end up in one of the workspace's two
-// index buffers (cub's double buffer decides which): `order` points at it.  The key pass leaves `reserve` SMs free; cub's
-// sort kernels size their own grids.
+// only n and the sampler's seed, first, n_users, n_items and indptr, never the tables.  The ordered indices end up in one of
+// the workspace's two index buffers (cub's double buffer decides which): `order` points at it.  The key pass leaves
+// `reserve` SMs free; cub's sort kernels size their own grids.
 static int schedule_grouped(const HogwildParams &p, int reserve, char *ws, const GroupLayout &L, cudaStream_t st,
                             const int32_t *&order) {
-    int sms = sm_count() - reserve;
-    if (sms < 1) sms = 1;
     cub::DoubleBuffer<uint32_t> keys((uint32_t *)(ws + L.key_a), (uint32_t *)(ws + L.key_b));
     cub::DoubleBuffer<int32_t> vals((int32_t *)(ws + L.val_a), (int32_t *)(ws + L.val_b));
-    int64_t grid = (p.n + 255) / 256;
-    if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
-    user_key_kernel<<<(unsigned)grid, 256, 0, st>>>(p, keys.Current(), vals.Current());
+    user_key_kernel<<<capped_grid(p.n, reserve), 256, 0, st>>>(p, keys.Current(), vals.Current());
     EB_CUDA(cudaGetLastError());
     size_t cb = L.cub_bytes;
-    EB_CUDA(cub::DeviceRadixSort::SortPairs(ws + L.cub, cb, keys, vals, (int)p.n, 0, bits_for((uint64_t)p.n_users), st));
+    EB_CUDA(cub::DeviceRadixSort::SortPairs(ws + L.cub, cb, keys, vals, (int)p.n, 0, bits_for((uint64_t)p.sampler.n_users), st));
     order = vals.Current();
     return EB_OK;
 }
 
+template <int DP>
+static StepKernel grouped_kernel(bool racy) {
+    return racy ? bpr_grouped_kernel<DP, Write::Store> : bpr_grouped_kernel<DP, Write::Atomic>;
+}
+
 // Sampled step on local tables, free-running: per sub-step, the schedule above, then the grouped update (which leaves
 // `reserve` SMs free).
-template <int DP, bool ATOMIC>
-static int launch_grouped(HogwildParams p, int reserve, char *ws, const GroupLayout &L, cudaStream_t st) {
+static int launch_grouped(StepKernel kern, HogwildParams p, int reserve, char *ws, const GroupLayout &L, cudaStream_t st) {
     const int64_t n = p.n;
-    const uint64_t first = p.first;
+    const uint64_t first = p.sampler.first;
     int32_t *out_u = p.out_u, *out_i = p.out_i, *out_j = p.out_j;
     for (int64_t c0 = 0; c0 < n; c0 += GROUP_MAX) {
         p.n = n - c0 < GROUP_MAX ? n - c0 : GROUP_MAX;
-        p.first = first + (uint64_t)c0;
+        p.sampler.first = first + (uint64_t)c0;
         if (out_u) { p.out_u = out_u + c0; p.out_i = out_i + c0; p.out_j = out_j + c0; }
         if (int rc = schedule_grouped(p, reserve, ws, L, st, p.order)) return rc;
-        if (int rc = launch_grouped_t<DP, ATOMIC>(p, reserve, st)) return rc;
+        if (int rc = launch_persistent(kern, p, reserve, st)) return rc;
     }
     return EB_OK;
 }
 
-// SAMPLE: the sampled step; free-running on local tables it runs grouped by user (ws: eb_bpr_step_sampled_workspace_bytes)
+// One table.  SAMPLE: the sampled step; free-running it runs grouped by user (ws: eb_bpr_step_sampled_workspace_bytes).
+// Deterministic rounds run bpr_rounds_kernel, materialised triples free-running bpr_hogwild_kernel.
 template <bool SAMPLE>
-static int launch_hogwild(const HogwildParams &p, int dp, int flags, cudaStream_t st, void *ws = nullptr, size_t ws_bytes = 0) {
-    const bool atomic = !(flags & 1);
-    const bool rounds = (flags & 64) != 0;
-    const int reserve = (flags >> 8) & 0xff;
-    EB_ARG(!(flags & 32), "the shared-memory-staged kernel exists for sharded item tables only");
-    EB_ARG(atomic || !rounds, "deterministic rounds run with atomic updates");
-    if constexpr (SAMPLE) {
-        if (!rounds) {
-            const GroupLayout L = group_layout(p.n, p.n_users);
-            if (!ws || ws_bytes < L.total) return set_err(EB_ERR_WORKSPACE, "workspace %zu < required %zu", ws ? ws_bytes : 0, L.total);
-            // the row stride is checked before anything is launched
-            return with_stride<8, 16, 32, 64, 128, 256>(dp, "8,16,32,64,128,256 floats", [&](auto dpc) {
-                constexpr int DP = decltype(dpc)::value;
-                item_table_l2_window(p, st);
-                return atomic ? launch_grouped<DP, true>(p, reserve, (char *)ws, L, st)
-                              : launch_grouped<DP, false>(p, reserve, (char *)ws, L, st);
-            });
-        }
+static int launch_local(const HogwildParams &p, int flags, cudaStream_t st, void *ws = nullptr, size_t ws_bytes = 0) {
+    StepFlags f;
+    if (int rc = decode_flags(flags, f)) return rc;
+    EB_ARG(!f.stage, "the shared-memory-staged kernel exists for sharded item tables only");
+    EB_ARG(!f.racy || !f.rounds, "deterministic rounds run with atomic updates");
+    GroupLayout L{};
+    if (SAMPLE && !f.rounds) {
+        L = group_layout(p.n, p.sampler.n_users);
+        if (!ws || ws_bytes < L.total) return set_err(EB_ERR_WORKSPACE, "workspace %zu < required %zu", ws ? ws_bytes : 0, L.total);
     }
-    item_table_l2_window(p, st);
-    return with_stride<8, 16, 32, 64, 128, 256>(dp, "8,16,32,64,128,256 floats", [&](auto dpc) {
+    return with_stride(LocalStrides{}, p.ld, [&](auto dpc) {
         constexpr int DP = decltype(dpc)::value;
-        if constexpr (!SAMPLE) {
-            if (!rounds) return atomic ? launch_hogwild_t<DP, false, true, false, false>(p, reserve, st)
-                                       : launch_hogwild_t<DP, false, false, false, false>(p, reserve, st);
-        }
-        return launch_hogwild_t<DP, SAMPLE, true, false, true>(p, reserve, st);   // deterministic rounds
+        if (f.rounds) return launch_persistent(bpr_rounds_kernel<DP, SAMPLE>, p, f.reserve, st, 0, true);
+        if constexpr (SAMPLE) return launch_grouped(grouped_kernel<DP>(f.racy), p, f.reserve, (char *)ws, L, st);
+        else return launch_persistent(f.racy ? bpr_hogwild_kernel<DP, false, Write::Store> : bpr_hogwild_kernel<DP, false, Write::Atomic>,
+                                      p, f.reserve, st);
     });
 }
 
 // The grouped update alone, on an order the caller scheduled (p.order, p.n <= GROUP_MAX)
-static int launch_apply(const HogwildParams &p, int dp, int flags, cudaStream_t st) {
-    const bool atomic = !(flags & 1);
-    const int reserve = (flags >> 8) & 0xff;
-    EB_ARG(!(flags & (32 | 64)), "the grouped update runs free-running on local tables (no rounds, no staged kernel)");
-    return with_stride<8, 16, 32, 64, 128, 256>(dp, "8,16,32,64,128,256 floats", [&](auto dpc) {
-        constexpr int DP = decltype(dpc)::value;
-        item_table_l2_window(p, st);
-        return atomic ? launch_grouped_t<DP, true>(p, reserve, st) : launch_grouped_t<DP, false>(p, reserve, st);
+static int launch_apply(const HogwildParams &p, int flags, cudaStream_t st) {
+    StepFlags f;
+    if (int rc = decode_flags(flags, f)) return rc;
+    EB_ARG(!f.stage && !f.rounds, "the grouped update runs free-running on local tables (no rounds, no staged kernel)");
+    return with_stride(LocalStrides{}, p.ld, [&](auto dpc) {
+        return launch_persistent(grouped_kernel<decltype(dpc)::value>(f.racy), p, f.reserve, st);
     });
 }
 
@@ -805,18 +643,37 @@ static int launch_apply(const HogwildParams &p, int dp, int flags, cudaStream_t 
 // kernel is the default (its row copies are in flight without holding registers while the rows cross NVLink); flags bit 4 (16),
 // or bit 0, selects the register kernel (whose peer updates stay atomic).
 template <bool SAMPLE>
-static int launch_hogwild_peer(const HogwildParams &p, int dp, int flags, cudaStream_t st) {
-    const int reserve = (flags >> 8) & 0xff;
-    EB_ARG(!(flags & 64), "deterministic rounds exist for local tables only (other GPUs update peer rows concurrently)");
-    const bool stage = !(flags & (1 | 16));
-    return with_stride<32, 64, 128>(dp, "32,64,128 floats for sharded item tables", [&](auto dpc) {
+static int launch_peer(const HogwildParams &p, int flags, cudaStream_t st) {
+    StepFlags f;
+    if (int rc = decode_flags(flags, f)) return rc;
+    EB_ARG(!f.rounds, "deterministic rounds exist for local tables only (other GPUs update peer rows concurrently)");
+    return with_stride(PeerStrides{}, p.ld, [&](auto dpc) {
         constexpr int DP = decltype(dpc)::value;
-        return stage ? launch_stage_t<DP, SAMPLE>(p, reserve, st) : launch_hogwild_t<DP, SAMPLE, true, true, false>(p, reserve, st);
+        if (f.racy || f.reg) return launch_persistent(bpr_hogwild_kernel<DP, SAMPLE, Write::AtomicSys>, p, f.reserve, st);
+        constexpr int SMEM = 8 * 3 * STAGE_CHUNK_BYTES + 64;   // 8 warps x 3 row kinds x chunk + mbarriers
+        EB_CUDA(cudaFuncSetAttribute(bpr_hogwild_stage_kernel<DP, SAMPLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+        return launch_persistent(bpr_hogwild_stage_kernel<DP, SAMPLE>, p, f.reserve, st, SMEM);
     });
 }
 
-static int fill_peer(HogwildParams &p, float *const *V_shards, float *const *b_shards, int n_shards, int32_t shard_rows,
+// the fields every step fills
+static HogwildParams step_params(float *U, float *V, float *b, int ld, int64_t n, BprHyper hp, double *loss) {
+    HogwildParams p{};
+    p.U = U; p.V = V; p.b = b; p.ld = ld; p.n = n; p.hp = hp; p.loss = loss;
+    return p;
+}
+
+// the optional sampled-triple outputs: all three or none
+static int set_out(HogwildParams &p, int32_t *out_u, int32_t *out_i, int32_t *out_j) {
+    EB_ARG((!out_u && !out_i && !out_j) || (out_u && out_i && out_j), "out_u/out_i/out_j: all or none");
+    p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
+    return EB_OK;
+}
+
+// the user table (p.U, row stride p.ld) and the item shards of a peer step
+static int fill_peer(HogwildParams &p, int d, float *const *V_shards, float *const *b_shards, int n_shards, int32_t shard_rows,
                      int32_t n_items) {
+    EB_ARG(p.U && d >= 1 && p.ld >= d && ((uintptr_t)p.U % 16) == 0, "bad user table");
     EB_ARG(V_shards && b_shards && n_shards >= 1 && n_shards <= EB_MAX_PEERS, "1 <= n_shards <= %d", EB_MAX_PEERS);
     EB_ARG(shard_rows >= 1 && (int64_t)shard_rows * n_shards >= n_items, "shards do not cover the item range");
     for (int s = 0; s < n_shards; s++) {
@@ -826,166 +683,6 @@ static int fill_peer(HogwildParams &p, float *const *V_shards, float *const *b_s
     for (int s = n_shards; s < EB_MAX_PEERS; s++) { p.Vp[s] = V_shards[0]; p.bp[s] = b_shards[0]; }
     p.shards = shard_map(shard_rows);
     return EB_OK;
-}
-
-static int check_tables(const void *U, const void *V, const void *b, int d, int ld) {
-    EB_ARG(U && V && b, "null table pointer");
-    EB_ARG(d >= 1 && ld >= d, "need 1 <= d <= ld (d=%d ld=%d)", d, ld);
-    EB_ARG(((uintptr_t)U % 16) == 0 && ((uintptr_t)V % 16) == 0, "tables must be 16-byte aligned");
-    return EB_OK;
-}
-
-// ---------------------------------------------------------------- exact mode (fp64)
-struct ExactParams {
-    double *U, *V, *b;
-    int d, ld;
-    const int32_t *tu, *ti, *tj;
-    const int32_t *ku, *ki, *kj;
-    int32_t *cntU, *cntI, *ticket;
-    int64_t n;
-    double lr, reg_u, reg_b, reg_pos, reg_neg;
-    double *loss;
-};
-
-__device__ __forceinline__ int ld_acquire(const int32_t *p) {
-    int v;
-    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release(int32_t *p, int v) {
-    asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-
-template <int NE>  // elements per lane, d <= 32*NE
-__global__ void __launch_bounds__(128) bpr_exact_kernel(const ExactParams p) {
-    const int lane = threadIdx.x & 31;
-    double loss_acc = 0.0;
-    for (;;) {
-        int t = 0;
-        if (lane == 0) t = atomicAdd(p.ticket, 1);
-        t = __shfl_sync(0xffffffffu, t, 0);
-        if (t >= p.n) break;
-        const int u = __ldg(p.tu + t), i = __ldg(p.ti + t), j = __ldg(p.tj + t);
-        const int wu = __ldg(p.ku + t), wi = __ldg(p.ki + t), wj = __ldg(p.kj + t);
-        int32_t *cu = p.cntU + u, *ci = p.cntI + i, *cj = p.cntI + j;
-        // Every lane performs the three acquire loads itself and the exit decision is a
-        // warp vote: control flow stays warp-uniform and each lane's later row loads are
-        // ordered after ITS OWN acquires (no reliance on cross-lane ordering).
-        {
-            unsigned ns = 8;
-            for (;;) {
-                const bool ready = (ld_acquire(cu) == wu) & (ld_acquire(ci) == wi) & (ld_acquire(cj) == wj);
-                if (__all_sync(0xffffffffu, ready)) break;
-                __nanosleep(ns);
-                if (ns < 128) ns <<= 1;
-            }
-        }
-        double *pu = p.U + (int64_t)u * p.ld, *pi = p.V + (int64_t)i * p.ld, *pj = p.V + (int64_t)j * p.ld;
-        double a[NE], vi[NE], vj[NE];
-        double xi = 0.0, xj = 0.0;
-#pragma unroll
-        for (int e = 0; e < NE; e++) {
-            const int k = lane + 32 * e;
-            a[e] = 0.0; vi[e] = 0.0; vj[e] = 0.0;
-            if (k < p.d) {
-                a[e] = __ldcg(pu + k); vi[e] = __ldcg(pi + k); vj[e] = __ldcg(pj + k);
-                xi = __dadd_rn(xi, __dmul_rn(a[e], vi[e]));
-                xj = __dadd_rn(xj, __dmul_rn(a[e], vj[e]));
-            }
-        }
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) {
-            xi = __dadd_rn(xi, __shfl_xor_sync(0xffffffffu, xi, off));
-            xj = __dadd_rn(xj, __shfl_xor_sync(0xffffffffu, xj, off));
-        }
-        const double bi = __ldcg(p.b + i), bj = __ldcg(p.b + j);
-        xi = __dadd_rn(xi, bi);
-        xj = __dadd_rn(xj, bj);
-        const double x = __dadd_rn(xi, -xj);
-        const double z = 1.0 / (1.0 + exp(x));  // BPRMF_model.py:98
-        const double sp = (x > 0) ? log1p(exp(-x)) : (-x + log1p(exp(x)));   // all lanes: no divergence
-        loss_acc += (lane == 0) ? sp : 0.0;
-#pragma unroll
-        for (int e = 0; e < NE; e++) {
-            const int k = lane + 32 * e;
-            // d_u = (V_i - V_j) z - reg_u U[u];  U[u] += lr d_u   (BPRMF_model.py:108-109)
-            const double un = __dadd_rn(
-                a[e], __dmul_rn(p.lr, __dadd_rn(__dmul_rn(__dadd_rn(vi[e], -vj[e]), z), -__dmul_rn(p.reg_u, a[e]))));
-            // d_i = U'[u] z - reg_pos V_i (BPRMF_model.py:112-113), d_j = -U'[u] z - reg_neg V_j (:116-117)
-            const double uz = __dmul_rn(un, z);
-            const double in_ = __dadd_rn(vi[e], __dmul_rn(p.lr, __dadd_rn(uz, -__dmul_rn(p.reg_pos, vi[e]))));
-            const double jn = __dadd_rn(vj[e], __dmul_rn(p.lr, __dadd_rn(-uz, -__dmul_rn(p.reg_neg, vj[e]))));
-            if (k < p.d) { __stcg(pu + k, un); __stcg(pi + k, in_); __stcg(pj + k, jn); }
-        }
-        const double bin = __dadd_rn(bi, __dmul_rn(p.lr, __dadd_rn(z, -__dmul_rn(p.reg_b, bi))));
-        const double bjn = __dadd_rn(bj, __dmul_rn(p.lr, __dadd_rn(-z, -__dmul_rn(p.reg_b, bj))));
-        if (lane == 0) { __stcg(p.b + i, bin); __stcg(p.b + j, bjn); }
-        __threadfence();
-        // the release stores depend on a full-warp vote that every lane reaches only after
-        // its own fence: all 32 lanes' row stores are visible before any counter moves
-        const unsigned done = __ballot_sync(0xffffffffu, true);
-        if (done == 0xffffffffu) {
-            if (lane == 0) st_release(cu, wu + 1);
-            else if (lane == 1) st_release(ci, wi + 1);
-            else if (lane == 2) st_release(cj, wj + 1);
-        }
-    }
-    if (p.loss && lane == 0 && loss_acc != 0.0) atomicAdd(p.loss, loss_acc);
-}
-
-// keys: (row << ebits) | event ; events of table `which`: users -> event = t, items -> event = 2t+slot
-__global__ void make_keys_kernel(const int32_t *tu, const int32_t *ti, const int32_t *tj, int64_t n, int ebits,
-                                 uint64_t *keysU, uint64_t *keysI, int32_t n_users, int32_t n_items, int32_t *status) {
-    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n) return;
-    // a triple with i == j would wait on the same row counter twice (the turn never comes: the kernel would spin for
-    // ever), an id out of range would touch foreign memory: report both before the ordered kernel is launched
-    const uint32_t uu = (uint32_t)tu[t], ii = (uint32_t)ti[t], jj = (uint32_t)tj[t];
-    if (ii == jj) atomicOr(status, 1);
-    if (uu >= (uint32_t)n_users || ii >= (uint32_t)n_items || jj >= (uint32_t)n_items) { atomicOr(status, 2); return; }
-    keysU[t] = ((uint64_t)(uint32_t)tu[t] << ebits) | (uint64_t)t;
-    keysI[2 * t] = ((uint64_t)(uint32_t)ti[t] << ebits) | (uint64_t)(2 * t);
-    keysI[2 * t + 1] = ((uint64_t)(uint32_t)tj[t] << ebits) | (uint64_t)(2 * t + 1);
-}
-
-// rank of each event inside its row segment of the sorted key array
-__global__ void ranks_kernel(const uint64_t *keys, int64_t m, int ebits, int is_items, int32_t *ka, int32_t *kb) {
-    int64_t pos = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (pos >= m) return;
-    const uint64_t key = keys[pos];
-    const uint64_t first = (key >> ebits) << ebits;
-    int64_t lo = 0, hi = pos;  // lower_bound of `first`
-    while (lo < hi) {
-        int64_t mid = (lo + hi) >> 1;
-        if (keys[mid] < first) lo = mid + 1; else hi = mid;
-    }
-    const int32_t rank = (int32_t)(pos - lo);
-    const uint64_t ev = key & ((1ull << ebits) - 1);
-    if (!is_items) ka[ev] = rank;
-    else if (ev & 1) kb[ev >> 1] = rank;
-    else ka[ev >> 1] = rank;
-}
-
-struct ExactLayout {
-    size_t keys_in, keys_out, ku, ki, kj, cnt, cub, total, cub_bytes;
-};
-
-// keys_in / keys_out hold 3n entries each: user keys in [0,n), item keys in [n,3n)
-static ExactLayout exact_layout(int64_t n, int32_t n_users, int32_t n_items) {
-    ExactLayout L;
-    size_t off = 0;
-    L.keys_in = off; off += align_up(sizeof(uint64_t) * 3 * (size_t)n);
-    L.keys_out = off; off += align_up(sizeof(uint64_t) * 3 * (size_t)n);
-    L.ku = off; off += align_up(sizeof(int32_t) * (size_t)n);
-    L.ki = off; off += align_up(sizeof(int32_t) * (size_t)n);
-    L.kj = off; off += align_up(sizeof(int32_t) * (size_t)n);
-    L.cnt = off; off += align_up(sizeof(int32_t) * ((size_t)n_users + (size_t)n_items + 64));
-    size_t cb = 0;
-    cub::DeviceRadixSort::SortKeys(nullptr, cb, (const uint64_t *)nullptr, (uint64_t *)nullptr, (int64_t)(2 * n), 0, 64);
-    L.cub_bytes = cb;
-    L.cub = off; off += align_up(cb);
-    L.total = off;
-    return L;
 }
 
 }  // namespace eb
@@ -999,33 +696,9 @@ extern "C" int eb_bpr_step_f32(float *U, float *V, float *item_bias, int d, int 
     EB_ARG(n >= 0, "n < 0");
     if (n == 0) return EB_OK;
     EB_ARG(tu && ti && tj, "null triple arrays");
-    HogwildParams p{};
-    p.U = U; p.V = V; p.b = item_bias; p.ld = ld; p.tu = tu; p.ti = ti; p.tj = tj; p.n = n;
-    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
-    return launch_hogwild<false>(p, ld, flags, (cudaStream_t)stream);
-}
-
-static int set_filter(HogwildParams &p, const uint32_t *filter, int filter_words) {
-    if (!filter) return EB_OK;
-    EB_ARG(filter_words >= 1 && filter_words <= 1024 && (filter_words & (filter_words - 1)) == 0,
-           "filter_words must be a power of two in [1, 1024] (got %d)", filter_words);
-    int lb = 5;
-    while ((1 << (lb - 5)) < filter_words) lb++;
-    p.filter = filter; p.filter_log2bits = lb;
-    return EB_OK;
-}
-
-extern "C" int eb_bloom_build(const int64_t *csr_indptr, const int32_t *csr_indices, int32_t n_users, int filter_words,
-                              uint32_t *out, void *stream) {
-    EB_ARG(csr_indptr && csr_indices && out && n_users >= 1, "bad argument");
-    HogwildParams p{};
-    if (int rc = set_filter(p, out, filter_words)) return rc;
-    int64_t grid = ((int64_t)n_users * 32 + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (grid > cap) grid = cap;
-    bloom_build_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(csr_indptr, csr_indices, n_users, p.filter_log2bits, out);
-    EB_CUDA(cudaGetLastError());
-    return EB_OK;
+    HogwildParams p = step_params(U, V, item_bias, ld, n, {lr, reg_u, reg_b, reg_pos, reg_neg}, loss);
+    p.tu = tu; p.ti = ti; p.tj = tj;
+    return launch_local<false>(p, flags, (cudaStream_t)stream);
 }
 
 extern "C" int eb_bpr_step_sampled_f32(float *U, float *V, float *item_bias, int d, int ld, int32_t n_users,
@@ -1051,17 +724,13 @@ extern "C" int eb_bpr_step_sampled_filter_f32(float *U, float *V, float *item_bi
                                               float reg_neg, double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
                                               void *workspace, size_t workspace_bytes, int flags, void *stream) {
     if (int rc = check_tables(U, V, item_bias, d, ld)) return rc;
-    EB_ARG(n >= 0 && n_users > 0 && n_items > 1, "bad sizes");
-    EB_ARG(csr_indptr && csr_indices, "null CSR");
-    EB_ARG((!out_u && !out_i && !out_j) || (out_u && out_i && out_j), "out_u/out_i/out_j: all or none");
+    EB_ARG(n >= 0, "n < 0");
+    HogwildParams p = step_params(U, V, item_bias, ld, n, {lr, reg_u, reg_b, reg_pos, reg_neg}, loss);
+    if (int rc = sampler_params(p.sampler, n_users, n_items, csr_indptr, csr_indices, filter, filter_words, seed, first_triple))
+        return rc;
+    if (int rc = set_out(p, out_u, out_i, out_j)) return rc;
     if (n == 0) return EB_OK;
-    HogwildParams p{};
-    p.U = U; p.V = V; p.b = item_bias; p.ld = ld; p.n = n;
-    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
-    p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
-    p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
-    if (int rc = set_filter(p, filter, filter_words)) return rc;
-    return launch_hogwild<true>(p, ld, flags, (cudaStream_t)stream, workspace, workspace_bytes);
+    return launch_local<true>(p, flags, (cudaStream_t)stream, workspace, workspace_bytes);
 }
 
 extern "C" int eb_bpr_schedule_sampled(int32_t n_users, int32_t n_items, const int64_t *csr_indptr, int64_t n, uint64_t seed,
@@ -1070,13 +739,15 @@ extern "C" int eb_bpr_schedule_sampled(int32_t n_users, int32_t n_items, const i
     EB_ARG(n >= 1 && n <= GROUP_MAX && n_users > 0 && n_items > 1, "bad sizes (a schedule covers 1..%lld triples)",
            (long long)GROUP_MAX);
     EB_ARG(csr_indptr && order_offset, "null pointer");
+    StepFlags f;
+    if (int rc = decode_flags(flags, f)) return rc;
     const GroupLayout L = group_layout(n, n_users);
     if (!workspace || workspace_bytes < L.total)
         return set_err(EB_ERR_WORKSPACE, "workspace %zu < required %zu", workspace ? workspace_bytes : 0, L.total);
     HogwildParams p{};
-    p.n = n; p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.seed = seed; p.first = first_triple;
+    p.n = n; p.sampler = SamplerParams{n_users, n_items, csr_indptr, nullptr, seed, first_triple, nullptr, 0};
     const int32_t *order = nullptr;
-    if (int rc = schedule_grouped(p, (flags >> 8) & 0xff, (char *)workspace, L, (cudaStream_t)stream, order)) return rc;
+    if (int rc = schedule_grouped(p, f.reserve, (char *)workspace, L, (cudaStream_t)stream, order)) return rc;
     *order_offset = (size_t)((const char *)order - (const char *)workspace);
     return EB_OK;
 }
@@ -1088,33 +759,27 @@ extern "C" int eb_bpr_apply_sampled_filter_f32(float *U, float *V, float *item_b
                                                float reg_neg, double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
                                                const int32_t *order, int flags, void *stream) {
     if (int rc = check_tables(U, V, item_bias, d, ld)) return rc;
-    EB_ARG(n >= 1 && n <= GROUP_MAX && n_users > 0 && n_items > 1, "bad sizes (an apply covers 1..%lld triples)",
-           (long long)GROUP_MAX);
-    EB_ARG(csr_indptr && csr_indices && order, "null CSR or order");
-    EB_ARG((!out_u && !out_i && !out_j) || (out_u && out_i && out_j), "out_u/out_i/out_j: all or none");
-    HogwildParams p{};
-    p.U = U; p.V = V; p.b = item_bias; p.ld = ld; p.n = n;
-    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
-    p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
-    p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
+    EB_ARG(n >= 1 && n <= GROUP_MAX, "bad sizes (an apply covers 1..%lld triples)", (long long)GROUP_MAX);
+    EB_ARG(order, "null order");
+    HogwildParams p = step_params(U, V, item_bias, ld, n, {lr, reg_u, reg_b, reg_pos, reg_neg}, loss);
+    if (int rc = sampler_params(p.sampler, n_users, n_items, csr_indptr, csr_indices, filter, filter_words, seed, first_triple))
+        return rc;
+    if (int rc = set_out(p, out_u, out_i, out_j)) return rc;
     p.order = order;
-    if (int rc = set_filter(p, filter, filter_words)) return rc;
-    return launch_apply(p, ld, flags, (cudaStream_t)stream);
+    return launch_apply(p, flags, (cudaStream_t)stream);
 }
 
 extern "C" int eb_bpr_step_peer_f32(float *U, float *const *V_shards, float *const *b_shards, int n_shards, int32_t shard_rows,
                                     int d, int ld, int32_t n_items, const int32_t *tu, const int32_t *ti, const int32_t *tj, int64_t n,
                                     float lr, float reg_u, float reg_b, float reg_pos, float reg_neg, double *loss, int flags,
                                     void *stream) {
-    EB_ARG(U && d >= 1 && ld >= d && ((uintptr_t)U % 16) == 0, "bad user table");
     EB_ARG(n >= 0, "n < 0");
-    HogwildParams p{};
-    if (int rc = fill_peer(p, V_shards, b_shards, n_shards, shard_rows, n_items)) return rc;
+    HogwildParams p = step_params(U, nullptr, nullptr, ld, n, {lr, reg_u, reg_b, reg_pos, reg_neg}, loss);
+    if (int rc = fill_peer(p, d, V_shards, b_shards, n_shards, shard_rows, n_items)) return rc;
     if (n == 0) return EB_OK;
     EB_ARG(tu && ti && tj, "null triple arrays");
-    p.U = U; p.ld = ld; p.tu = tu; p.ti = ti; p.tj = tj; p.n = n;
-    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
-    return launch_hogwild_peer<false>(p, ld, flags, (cudaStream_t)stream);
+    p.tu = tu; p.ti = ti; p.tj = tj;
+    return launch_peer<false>(p, flags, (cudaStream_t)stream);
 }
 
 extern "C" int eb_bpr_step_sampled_peer_f32(float *U, float *const *V_shards, float *const *b_shards, int n_shards, int32_t shard_rows,
@@ -1123,83 +788,14 @@ extern "C" int eb_bpr_step_sampled_peer_f32(float *U, float *const *V_shards, fl
                                             uint64_t seed, uint64_t first_triple, float lr,
                                             float reg_u, float reg_b, float reg_pos, float reg_neg, double *loss, int32_t *out_u,
                                             int32_t *out_i, int32_t *out_j, int flags, void *stream) {
-    EB_ARG(U && d >= 1 && ld >= d && ((uintptr_t)U % 16) == 0, "bad user table");
-    EB_ARG(n >= 0 && n_users > 0 && n_items > 1, "bad sizes");
-    EB_ARG(csr_indptr && csr_indices, "null CSR");
-    EB_ARG((!out_u && !out_i && !out_j) || (out_u && out_i && out_j), "out_u/out_i/out_j: all or none");
-    HogwildParams p{};
-    if (int rc = fill_peer(p, V_shards, b_shards, n_shards, shard_rows, n_items)) return rc;
-    if (n == 0) return EB_OK;
-    p.U = U; p.ld = ld; p.n = n;
-    p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss;
-    p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
-    p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
-    p.no_item_updates = (flags >> 2) & 1;
-    if (int rc = set_filter(p, filter, filter_words)) return rc;
-    return launch_hogwild_peer<true>(p, ld, flags, (cudaStream_t)stream);
-}
-
-extern "C" int eb_bpr_sample_philox(int32_t n_users, int32_t n_items, const int64_t *csr_indptr,
-                                    const int32_t *csr_indices, int64_t n, uint64_t seed, uint64_t first_triple,
-                                    int32_t *out_u, int32_t *out_i, int32_t *out_j, void *stream) {
-    return eb_bpr_sample_philox_filter(n_users, n_items, csr_indptr, csr_indices, nullptr, 0, n, seed, first_triple, out_u, out_i,
-                                       out_j, stream);
-}
-
-extern "C" int eb_bpr_sample_philox_filter(int32_t n_users, int32_t n_items, const int64_t *csr_indptr,
-                                           const int32_t *csr_indices, const uint32_t *filter, int filter_words, int64_t n,
-                                           uint64_t seed, uint64_t first_triple, int32_t *out_u, int32_t *out_i, int32_t *out_j,
-                                           void *stream) {
-    EB_ARG(n >= 0 && n_users > 0 && n_items > 1, "bad sizes");
-    EB_ARG(csr_indptr && csr_indices && out_u && out_i && out_j, "null pointer");
-    if (n == 0) return EB_OK;
-    HogwildParams p{};
-    p.n = n; p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
-    p.seed = seed; p.first = first_triple; p.out_u = out_u; p.out_i = out_i; p.out_j = out_j;
-    if (int rc = set_filter(p, filter, filter_words)) return rc;
-    int64_t grid = (n + 255) / 256;
-    int64_t cap = (int64_t)sm_count() * 8;
-    if (grid > cap) grid = cap;
-    philox_sample_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(p);
-    EB_CUDA(cudaGetLastError());
-    return EB_OK;
-}
-
-extern "C" int eb_pointwise_sample_philox(int32_t n_users, int32_t n_items, const int64_t *csr_indptr, const int32_t *csr_indices,
-                                          const uint32_t *filter, int filter_words, int64_t n, uint64_t seed, uint64_t first,
-                                          int32_t *out_u, int32_t *out_i, float *out_label, void *stream) {
-    EB_ARG(n >= 0 && n_users > 0 && n_items > 1, "bad sizes");
-    EB_ARG(csr_indptr && csr_indices && out_u && out_i && out_label, "null pointer");
-    if (n == 0) return EB_OK;
-    HogwildParams p{};
-    p.n = n; p.n_users = n_users; p.n_items = n_items; p.indptr = csr_indptr; p.indices = csr_indices;
-    p.seed = seed; p.first = first; p.out_u = out_u; p.out_i = out_i;
-    if (int rc = set_filter(p, filter, filter_words)) return rc;
-    int64_t grid = (n + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (grid > cap) grid = cap;
-    pointwise_sample_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(p, out_label);
-    EB_CUDA(cudaGetLastError());
-    return EB_OK;
-}
-
-extern "C" int eb_bpr_step_host_f32(float *U, float *V, float *item_bias, int d, int ld, const int32_t *tu_host,
-                                    const int32_t *ti_host, const int32_t *tj_host, int64_t n, float lr, float reg_u,
-                                    float reg_b, float reg_pos, float reg_neg, int32_t *staging, double *loss_dev,
-                                    double *loss_host, int flags, void *stream) {
-    EB_ARG(staging && tu_host && ti_host && tj_host, "null host/staging pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    EB_CUDA(cudaMemcpyAsync(staging, tu_host, sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
-    EB_CUDA(cudaMemcpyAsync(staging + n, ti_host, sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
-    EB_CUDA(cudaMemcpyAsync(staging + 2 * n, tj_host, sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
-    if (loss_dev) EB_CUDA(cudaMemsetAsync(loss_dev, 0, sizeof(double), st));
-    if (int rc = eb_bpr_step_f32(U, V, item_bias, d, ld, staging, staging + n, staging + 2 * n, n, lr, reg_u, reg_b,
-                                 reg_pos, reg_neg, loss_dev, flags, stream))
+    EB_ARG(n >= 0, "n < 0");
+    HogwildParams p = step_params(U, nullptr, nullptr, ld, n, {lr, reg_u, reg_b, reg_pos, reg_neg}, loss);
+    if (int rc = sampler_params(p.sampler, n_users, n_items, csr_indptr, csr_indices, filter, filter_words, seed, first_triple))
         return rc;
-    if (loss_dev && loss_host)
-        EB_CUDA(cudaMemcpyAsync(loss_host, loss_dev, sizeof(double), cudaMemcpyDeviceToHost, st));
-    if (!(flags & 2)) EB_CUDA(cudaStreamSynchronize(st));
-    return EB_OK;
+    if (int rc = set_out(p, out_u, out_i, out_j)) return rc;
+    if (int rc = fill_peer(p, d, V_shards, b_shards, n_shards, shard_rows, n_items)) return rc;
+    if (n == 0) return EB_OK;
+    return launch_peer<true>(p, flags, (cudaStream_t)stream);
 }
 
 extern "C" int eb_bpr_step_host_packed_f32(float *U, float *V, float *item_bias, int d, int ld, const uint64_t *packed_host, int64_t n,
@@ -1208,76 +804,17 @@ extern "C" int eb_bpr_step_host_packed_f32(float *U, float *V, float *item_bias,
     if (int rc = check_tables(U, V, item_bias, d, ld)) return rc;
     EB_ARG(staging && packed_host && n >= 0, "null host/staging pointer");
     EB_ARG(bits_u >= 1 && bits_i >= 1 && bits_u + 2 * bits_i <= 64, "need bits_u + 2*bits_i <= 64 (got %d, %d)", bits_u, bits_i);
+    StepFlags f;
+    if (int rc = decode_flags(flags, f)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (loss_dev) EB_CUDA(cudaMemsetAsync(loss_dev, 0, sizeof(double), st));
     if (n > 0) {
         EB_CUDA(cudaMemcpyAsync(staging, packed_host, sizeof(uint64_t) * n, cudaMemcpyHostToDevice, st));   // ONE copy, 8 B / triple
-        HogwildParams p{};
-        p.U = U; p.V = V; p.b = item_bias; p.ld = ld; p.n = n; p.packed = staging; p.bits_u = bits_u; p.bits_i = bits_i;
-        p.hp = {lr, reg_u, reg_b, reg_pos, reg_neg}; p.loss = loss_dev;
-        if (int rc = launch_hogwild<false>(p, ld, flags, st)) return rc;
+        HogwildParams p = step_params(U, V, item_bias, ld, n, {lr, reg_u, reg_b, reg_pos, reg_neg}, loss_dev);
+        p.packed = staging; p.bits_u = bits_u; p.bits_i = bits_i;
+        if (int rc = launch_local<false>(p, flags, st)) return rc;
     }
     if (loss_dev && loss_host) EB_CUDA(cudaMemcpyAsync(loss_host, loss_dev, sizeof(double), cudaMemcpyDeviceToHost, st));
-    if (!(flags & 2)) EB_CUDA(cudaStreamSynchronize(st));
-    return EB_OK;
-}
-
-extern "C" size_t eb_bpr_exact_workspace_bytes(int64_t n, int32_t n_users, int32_t n_items) {
-    if (n <= 0) return 256;
-    return exact_layout(n, n_users, n_items).total;
-}
-
-extern "C" int eb_bpr_exact_f64(double *U, double *V, double *item_bias, int d, int ld, int32_t n_users,
-                                int32_t n_items, const int32_t *tu, const int32_t *ti, const int32_t *tj, int64_t n,
-                                double lr, double reg_u, double reg_b, double reg_pos, double reg_neg, double *loss,
-                                void *workspace, size_t workspace_bytes, void *stream) {
-    if (int rc = check_tables(U, V, item_bias, d, ld)) return rc;
-    EB_ARG(d <= 256, "exact mode supports d <= 256 (d=%d)", d);
-    EB_ARG(n >= 0 && n < (1ll << 30), "n out of range");
-    if (n == 0) return EB_OK;
-    EB_ARG(tu && ti && tj && workspace, "null pointer");
-    const ExactLayout L = exact_layout(n, n_users, n_items);
-    if (workspace_bytes < L.total)
-        return set_err(EB_ERR_WORKSPACE, "workspace %zu < required %zu", workspace_bytes, L.total);
-    cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)workspace;
-    uint64_t *keys_in = (uint64_t *)(ws + L.keys_in), *keys_out = (uint64_t *)(ws + L.keys_out);
-    int32_t *ku = (int32_t *)(ws + L.ku), *ki = (int32_t *)(ws + L.ki), *kj = (int32_t *)(ws + L.kj);
-    int32_t *cnt = (int32_t *)(ws + L.cnt);
-    const int ebits = bits_for((uint64_t)(2 * n));
-    const int rbits_u = bits_for((uint64_t)n_users), rbits_i = bits_for((uint64_t)n_items);
-    const unsigned blocks = (unsigned)((n + 255) / 256);
-    int32_t *status = cnt + (size_t)n_users + (size_t)n_items + 8;
-    EB_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
-    make_keys_kernel<<<blocks, 256, 0, st>>>(tu, ti, tj, n, ebits, keys_in, keys_in + n, n_users, n_items, status);
-    EB_CUDA(cudaGetLastError());
-    {   // exact mode is latency-insensitive (one call per epoch): validate synchronously rather than risk a spin that never ends
-        int32_t bad = 0;
-        EB_CUDA(cudaMemcpyAsync(&bad, status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        EB_CUDA(cudaStreamSynchronize(st));
-        if (bad & 2) return set_err(EB_ERR_ARG, "triple ids out of range (need u < %d, i and j < %d)", n_users, n_items);
-        if (bad & 1) return set_err(EB_ERR_ARG, "a triple has i == j (the reference sampler never emits one, custom_sampler.py:39-41)");
-    }
-    size_t cb = L.cub_bytes;
-    EB_CUDA(cub::DeviceRadixSort::SortKeys(ws + L.cub, cb, keys_in, keys_out, n, 0, ebits + rbits_u, st));
-    ranks_kernel<<<blocks, 256, 0, st>>>(keys_out, n, ebits, 0, ku, nullptr);
-    EB_CUDA(cudaGetLastError());
-    cb = L.cub_bytes;
-    EB_CUDA(cub::DeviceRadixSort::SortKeys(ws + L.cub, cb, keys_in + n, keys_out + n, 2 * n, 0, ebits + rbits_i, st));
-    ranks_kernel<<<(unsigned)((2 * n + 255) / 256), 256, 0, st>>>(keys_out + n, 2 * n, ebits, 1, ki, kj);
-    EB_CUDA(cudaGetLastError());
-    EB_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * ((size_t)n_users + (size_t)n_items + 64), st));
-    ExactParams p{};
-    p.U = U; p.V = V; p.b = item_bias; p.d = d; p.ld = ld; p.tu = tu; p.ti = ti; p.tj = tj;
-    p.ku = ku; p.ki = ki; p.kj = kj; p.cntU = cnt; p.cntI = cnt + n_users; p.ticket = cnt + n_users + n_items;
-    p.n = n; p.lr = lr; p.reg_u = reg_u; p.reg_b = reg_b; p.reg_pos = reg_pos; p.reg_neg = reg_neg; p.loss = loss;
-    const int ne = (d + 31) / 32;
-    int64_t grid = (int64_t)sm_count() * 4;
-    if (grid * 4 > n) grid = (n + 3) / 4;
-    if (ne <= 1) bpr_exact_kernel<1><<<(unsigned)grid, 128, 0, st>>>(p);
-    else if (ne <= 2) bpr_exact_kernel<2><<<(unsigned)grid, 128, 0, st>>>(p);
-    else if (ne <= 4) bpr_exact_kernel<4><<<(unsigned)grid, 128, 0, st>>>(p);
-    else bpr_exact_kernel<8><<<(unsigned)grid, 128, 0, st>>>(p);
-    EB_CUDA(cudaGetLastError());
+    if (!f.no_sync) EB_CUDA(cudaStreamSynchronize(st));
     return EB_OK;
 }

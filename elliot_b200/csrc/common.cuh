@@ -27,6 +27,29 @@ int set_err(int code, const char *fmt, ...);
 
 int sm_count();
 
+// grid of 256-thread CTAs for a grid-stride loop over `threads` threads (>= 1), capped at 8 CTAs per SM on the SMs left
+// after `reserve_sms`
+static inline unsigned capped_grid(int64_t threads, int reserve_sms = 0) {
+    int sms = sm_count() - reserve_sms;
+    if (sms < 1) sms = 1;
+    const int64_t g = (threads + 255) / 256, cap = (int64_t)sms * 8;
+    return (unsigned)(g > cap ? cap : (g < 1 ? 1 : g));
+}
+
+// workspace layouts: every buffer starts on a 256-byte boundary
+static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
+
+// number of bits of v (at least 1): what a radix sort of keys up to v needs
+static inline int bits_for(uint64_t v) { int b = 1; while ((v >> b) != 0) b++; return b; }
+
+// the embedding tables of a BPR step: user rows U, item rows V (row stride ld), item biases b
+static inline int check_tables(const void *U, const void *V, const void *b, int d, int ld) {
+    EB_ARG(U && V && b, "null table pointer");
+    EB_ARG(d >= 1 && ld >= d, "need 1 <= d <= ld (d=%d ld=%d)", d, ld);
+    EB_ARG(((uintptr_t)U % 16) == 0 && ((uintptr_t)V % 16) == 0, "tables must be 16-byte aligned");
+    return EB_OK;
+}
+
 // Philox4x32-10 (Salmon et al. 2011).  key = seed, counter = (triple index, attempt).
 struct Philox {
     static constexpr uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;

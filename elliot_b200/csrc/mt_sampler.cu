@@ -227,20 +227,18 @@ struct SamplerLayout {
     int64_t n_raw_max, n_blocks_max;
 };
 
-static inline size_t align_up_(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
-
 static SamplerLayout sampler_layout(int64_t events) {
     SamplerLayout L;
     L.n_raw_max = 8 * events + 16384;
     L.n_blocks_max = (L.n_raw_max + CHAIN_L - 1) / CHAIN_L;
     size_t off = 0;
-    L.raw = off; off += align_up_(sizeof(uint32_t) * (size_t)L.n_raw_max);
-    L.parsed = off; off += align_up_(sizeof(int4) * (size_t)L.n_raw_max);
-    L.exit_pos = off; off += align_up_(sizeof(int64_t) * (size_t)L.n_raw_max);
-    L.cnt = off; off += align_up_(sizeof(int32_t) * (size_t)L.n_raw_max);
-    L.entry = off; off += align_up_(sizeof(int64_t) * (size_t)L.n_blocks_max);
-    L.base = off; off += align_up_(sizeof(int64_t) * (size_t)L.n_blocks_max);
-    L.status = off; off += align_up_(sizeof(MtStatus));
+    L.raw = off; off += align_up(sizeof(uint32_t) * (size_t)L.n_raw_max);
+    L.parsed = off; off += align_up(sizeof(int4) * (size_t)L.n_raw_max);
+    L.exit_pos = off; off += align_up(sizeof(int64_t) * (size_t)L.n_raw_max);
+    L.cnt = off; off += align_up(sizeof(int32_t) * (size_t)L.n_raw_max);
+    L.entry = off; off += align_up(sizeof(int64_t) * (size_t)L.n_blocks_max);
+    L.base = off; off += align_up(sizeof(int64_t) * (size_t)L.n_blocks_max);
+    L.status = off; off += align_up(sizeof(MtStatus));
     L.total = off;
     return L;
 }

@@ -33,7 +33,7 @@ template <int DP>
 __global__ void __launch_bounds__(256) bpr_rows_kernel(float *U, int64_t ldu, const int32_t *tu, const float *Ri, const float *Rj,
                                                        int64_t ldr, int64_t n, int bias_col, const BprHyper h, float *dRi, float *dRj,
                                                        double *loss) {
-    constexpr int NV = DP / 4, G = NV >= 32 ? 32 : NV, VPL = NV / G;
+    constexpr int G = LaneGroup<DP>::G, VPL = LaneGroup<DP>::VPL;
     const int lane = threadIdx.x & 31, gl = lane % G;
     const int64_t grp = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * (32 / G) + lane / G;
     const int64_t ngrp = (((int64_t)gridDim.x * blockDim.x) >> 5) * (32 / G);
@@ -87,16 +87,7 @@ __global__ void __launch_bounds__(256) bpr_rows_kernel(float *U, int64_t ldu, co
             *reinterpret_cast<float4 *>(dRj + t * ldr + e) = dj;
         }
     }
-    if (loss) {
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, off);
-        if (lane == 0 && loss_acc != 0.f) atomicAdd(loss, (double)loss_acc);
-    }
-}
-
-static inline unsigned sgrid(int64_t threads) {
-    int64_t g = (threads + 255) / 256; const int64_t cap = (int64_t)sm_count() * 8;
-    return (unsigned)(g > cap ? cap : (g < 1 ? 1 : g));
+    flush_loss(loss_acc, loss, lane);
 }
 
 }  // namespace eb
@@ -108,7 +99,7 @@ extern "C" int eb_gather_rows_f32(const float *table, int64_t ld, const int32_t 
     EB_ARG(table && ids && out && n >= 0 && width >= 4 && width % 4 == 0 && ld >= width && ldo >= width && ld % 4 == 0 && ldo % 4 == 0,
            "bad argument (width, ld, ldo must be multiples of 4)");
     if (n == 0) return EB_OK;
-    gather_rows_kernel<<<sgrid(n * (width / 4)), 256, 0, (cudaStream_t)stream>>>(table, ld, ids, n, width, out, ldo);
+    gather_rows_kernel<<<capped_grid(n * (width / 4)), 256, 0, (cudaStream_t)stream>>>(table, ld, ids, n, width, out, ldo);
     EB_CUDA(cudaGetLastError());
     return EB_OK;
 }
@@ -118,7 +109,7 @@ extern "C" int eb_scatter_add_rows_f32(float *table, int64_t ld, const int32_t *
     EB_ARG(table && ids && rows && n >= 0 && width >= 4 && width % 4 == 0 && ld >= width && ldr >= width && ld % 4 == 0 && ldr % 4 == 0,
            "bad argument (width, ld, ldr must be multiples of 4)");
     if (n == 0) return EB_OK;
-    scatter_add_rows_kernel<<<sgrid(n * (width / 4)), 256, 0, (cudaStream_t)stream>>>(table, ld, ids, n, width, rows, ldr);
+    scatter_add_rows_kernel<<<capped_grid(n * (width / 4)), 256, 0, (cudaStream_t)stream>>>(table, ld, ids, n, width, rows, ldr);
     EB_CUDA(cudaGetLastError());
     return EB_OK;
 }
@@ -130,7 +121,7 @@ extern "C" int eb_bpr_step_rows_f32(float *U, int64_t ldu, const int32_t *tu, co
     EB_ARG(ldu == ldr && (bias_col < 0 || bias_col < ldr), "user and item rows must share the row stride; bias_col inside the row");
     if (n == 0) return EB_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    const unsigned grid = sgrid(n * 16);
+    const unsigned grid = capped_grid(n * 16);
     const BprHyper h{lr, reg_u, reg_b, reg_pos, reg_neg};
 #define EB_ROWS(DPV) case DPV: bpr_rows_kernel<DPV><<<grid, 256, 0, st>>>(U, ldu, tu, Ri, Rj, ldr, n, bias_col, h, dRi, dRj, loss); break;
     switch ((int)ldr) {

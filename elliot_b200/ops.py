@@ -95,12 +95,11 @@ def _topk_out(users, n_rows, user_begin, n_sel, k, dtype, device):
             torch.empty((n_sel, k), dtype=dtype, device=device))
 
 
-def _bpr_flags(racy=False, sync=True, no_item_updates=False, variant=0, deterministic=False, reserve_sms=0):
+def _bpr_flags(racy=False, sync=True, variant=0, deterministic=False, reserve_sms=0):
     """The flags word of the eb_bpr_step_* entry points: bit 0 plain stores (racy Hogwild), bit 1 no synchronise (host
-    triples), bit 2 no item-row updates, bits 4-5 kernel variant (16 or 32), bit 6 deterministic rounds, bits 8-15 SMs
-    the grid leaves free."""
-    return ((1 if racy else 0) | (0 if sync else 2) | (4 if no_item_updates else 0) | int(variant)
-            | (64 if deterministic else 0) | ((int(reserve_sms) & 0xff) << 8))
+    triples), bits 4-5 kernel variant (16 or 32), bit 6 deterministic rounds, bits 8-15 SMs the grid leaves free."""
+    return ((1 if racy else 0) | (0 if sync else 2) | int(variant) | (64 if deterministic else 0)
+            | ((int(reserve_sms) & 0xff) << 8))
 
 
 def _out_ptrs(out):
@@ -272,17 +271,6 @@ def bpr_sample_philox(n_users, n_items, indptr, indices, n, seed, first=0, filte
     _call("eb_bpr_sample_philox_filter", indptr, n_users, n_items, _ptr(indptr), _ptr(indices), _ptr(filter),
           0 if filter is None else filter.shape[1], n, seed, first, _ptr(u), _ptr(i), _ptr(j))
     return u, i, j
-
-
-def bpr_step_host_f32(U, V, b, d, tu_host, ti_host, tj_host, lr, reg_u, reg_b, reg_pos, reg_neg, staging, loss_dev,
-                      loss_host, racy=False, sync=True, reserve_sms=0):
-    """End-to-end step from HOST (pinned) int32 triples; returns after the loss is back on the host."""
-    _need_cuda(U, V, b, staging, loss_dev)
-    n = tu_host.numel()
-    assert not tu_host.is_cuda and tu_host.dtype == torch.int32 and staging.numel() >= 3 * n
-    _call("eb_bpr_step_host_f32", U, _ptr(U), _ptr(V), _ptr(b), d, U.stride(0), _ptr(tu_host), _ptr(ti_host), _ptr(tj_host), n,
-          lr, reg_u, reg_b, reg_pos, reg_neg, _ptr(staging), _ptr(loss_dev), _ptr(loss_host),
-          _bpr_flags(racy=racy, sync=sync, reserve_sms=reserve_sms))
 
 
 def pack_bits(n_users, n_items):
@@ -1266,8 +1254,7 @@ def bpr_step_peer_f32(U, V_shards, b_shards, shard_rows, d, n_items, tu, ti, tj,
 
 
 def bpr_step_sampled_peer_f32(U, V_shards, b_shards, shard_rows, d, n_users, n_items, indptr, indices, n, seed, first, lr, reg_u,
-                              reg_b, reg_pos, reg_neg, loss=None, out=None, reserve_sms=0, filter=None, _no_item_updates=False,
-                              _variant=0):
+                              reg_b, reg_pos, reg_neg, loss=None, out=None, reserve_sms=0, filter=None, _variant=0):
     """Fused sample+update step with the item table row-sharded over the GPUs of the box (loads / atomics over NVLink).
     _variant (profiling): 16 forces the register-staged kernel, 32 the shared-memory-staged one (the default)."""
     _need_cuda(U, indptr, indices, loss)
@@ -1277,7 +1264,7 @@ def bpr_step_sampled_peer_f32(U, V_shards, b_shards, shard_rows, d, n_users, n_i
     out = _out_ptrs(out)
     _call("eb_bpr_step_sampled_peer_f32", U, _ptr(U), va, ba, ns, shard_rows, d, U.stride(0), n_users, n_items, _ptr(indptr),
           _ptr(indices), _ptr(filter), 0 if filter is None else filter.shape[1], n, seed, first, lr, reg_u, reg_b, reg_pos, reg_neg,
-          _ptr(loss), *out, _bpr_flags(no_item_updates=_no_item_updates, variant=_variant, reserve_sms=reserve_sms))
+          _ptr(loss), *out, _bpr_flags(variant=_variant, reserve_sms=reserve_sms))
 
 
 def table_reconcile_peer_f32(slice_ptrs, prev_slice, scale, max_ctas=0):

@@ -58,7 +58,8 @@ int eb_device_info(int *sm_count, int *cc);
  * flags: bit0 = plain stores instead of atomics (racy Hogwild); bit6 = deterministic rounds (cooperative launch: every
  * triple reads the values left by the previous rounds of reads-then-atomic-adds, so reruns give the same tables up to
  * fp32 summation order; slower); bits 8..15 = number of SMs the persistent grid leaves free (so a collective kernel on
- * another stream can run beside it).  The same flags apply to the sampled and host-triple variants below. */
+ * another stream can run beside it).  The same flags apply to the sampled and host-triple variants below; bit 2 is
+ * refused with EB_ERR_ARG. */
 int eb_bpr_step_f32(float *U, float *V, float *item_bias, int d, int ld,
                     const int32_t *tu, const int32_t *ti, const int32_t *tj, int64_t n,
                     float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
@@ -123,29 +124,18 @@ int eb_bpr_apply_sampled_filter_f32(float *U, float *V, float *item_bias, int d,
                                     float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
                                     double *loss, int32_t *out_u, int32_t *out_i, int32_t *out_j,
                                     const int32_t *order, int flags, void *stream);
+/* Sample only (no update): same sampler as above (filter may be NULL), for tests and for host
+ * pipelines that want materialised triples. */
 int eb_bpr_sample_philox_filter(int32_t n_users, int32_t n_items, const int64_t *csr_indptr,
                                 const int32_t *csr_indices, const uint32_t *filter, int filter_words, int64_t n,
                                 uint64_t seed, uint64_t first_triple, int32_t *out_u, int32_t *out_i, int32_t *out_j,
                                 void *stream);
 
-/* Sample only (no update): same sampler as above, for tests and for host
- * pipelines that want materialised triples. */
-int eb_bpr_sample_philox(int32_t n_users, int32_t n_items,
-                         const int64_t *csr_indptr, const int32_t *csr_indices,
-                         int64_t n, uint64_t seed, uint64_t first_triple,
-                         int32_t *out_u, int32_t *out_i, int32_t *out_j, void *stream);
-
-/* End-to-end variant of eb_bpr_step_f32 for HOST triples: copies the three
- * host index arrays into `staging` (device, 3*n int32), runs the step, copies
- * the loss back into *loss_host and synchronises the stream (flags bit1 = do NOT synchronise:
- * lets the caller pipeline steps on two streams so the next batch's H2D overlaps this kernel). */
-int eb_bpr_step_host_f32(float *U, float *V, float *item_bias, int d, int ld,
-                         const int32_t *tu_host, const int32_t *ti_host, const int32_t *tj_host, int64_t n,
-                         float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
-                         int32_t *staging, double *loss_dev, double *loss_host, int flags, void *stream);
-/* The same with PACKED host triples: one uint64 per triple, u | i << bits_u | j << (bits_u + bits_i)
- * (bits_u + 2*bits_i <= 64; 20 + 17 + 17 bits cover the C2 shape) — 8 instead of 12 bytes per triple over PCIe and ONE
- * host-to-device copy instead of three; the kernel unpacks.  staging: device, n uint64. */
+/* End-to-end variant of eb_bpr_step_f32 for HOST triples, PACKED one uint64 per triple, u | i << bits_u | j << (bits_u + bits_i)
+ * (bits_u + 2*bits_i <= 64; 20 + 17 + 17 bits cover the C2 shape): ONE host-to-device copy of 8 bytes per triple into
+ * `staging` (device, n uint64), the step (the kernel unpacks), the loss copied back into *loss_host, and the stream
+ * synchronised (flags bit1 = do NOT synchronise: lets the caller pipeline steps on two streams so the next batch's H2D
+ * overlaps this kernel). */
 int eb_bpr_step_host_packed_f32(float *U, float *V, float *item_bias, int d, int ld, const uint64_t *packed_host, int64_t n,
                                 int bits_u, int bits_i, float lr, float reg_u, float reg_b, float reg_pos, float reg_neg,
                                 uint64_t *staging, double *loss_dev, double *loss_host, int flags, void *stream);

@@ -434,6 +434,22 @@ def test_deterministic_rounds_are_refused_where_they_do_not_exist(golden_tiny):
         ops.bpr_step_f32(Ud, Vd, bd, d, t, t, t, 0.05, 0, 0, 0, 0, racy=True, deterministic=True)
 
 
+def test_flags_bit_2_is_refused(golden_tiny):
+    """Flags bit 2 is not a BPR step option: the step refuses it and leaves the tables as they were."""
+    from elliot_b200._lib import EbError
+    g = golden_tiny
+    d = int(g["d"]); ld = ops.padded_dim(d)
+    Ud, Vd = _pad(g["U0"], ld, np.float32), _pad(g["V0"], ld, np.float32)
+    bd = torch.zeros(len(g["items"]), dtype=torch.float32, device=DEV)
+    U0, V0 = Ud.clone(), Vd.clone()
+    t = torch.tensor([0, 1], dtype=torch.int32, device=DEV)
+    with pytest.raises(EbError, match="bit 2"):
+        ops._call("eb_bpr_step_f32", Ud, ops._ptr(Ud), ops._ptr(Vd), ops._ptr(bd), d, ld, ops._ptr(t[:1]), ops._ptr(t[1:]),
+                  ops._ptr(t[:1]), 1, 0.05, 0.0, 0.0, 0.0, 0.0, 0, 4)
+    torch.cuda.synchronize()
+    assert torch.equal(Ud, U0) and torch.equal(Vd, V0) and not bd.any()
+
+
 def test_shared_memory_staged_kernel_is_refused_on_one_table(golden_tiny):
     """The shared-memory-staged kernel (_variant=32) exists for sharded item tables only."""
     from elliot_b200._lib import EbError

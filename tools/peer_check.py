@@ -172,11 +172,6 @@ def _bpr():
         ctr[0] += 1
     ms = timed(step, 10, warm=3)
 
-    def step_reads_only():                                       # profiling: the same kernel without the item-row atomics
-        ops.bpr_step_sampled_peer_f32(U, items.ptrs, bias.ptr_array(), items.shard_rows, d, nu_loc, ni_tot, indptr, indices, B,
-                                      42 + rank, ctr[0] * B, *HP, loss=loss, _no_item_updates=True)
-        ctr[0] += 1
-    res["sharded_step_reads_only_ms"] = timed(step_reads_only, 10, warm=2)
     filt = ops.bloom_build(indptr, indices, nu_loc)
 
     def step_filter():
