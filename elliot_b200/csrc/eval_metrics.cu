@@ -90,16 +90,20 @@ __global__ void __launch_bounds__(EM_THREADS) eval_metrics_user_kernel(
     const int n_list = list_len<G>(lst, k, lane);             // every lane of the warp takes part in the shuffles
     const int n = in_a ? n_list : 0;
 
-    int hits = 0, first_hit = k, hits_sh = 0, n_lt = 0;
+    // ACLT, APLT, PopREO and PopRSP count each listed item once (the reference takes set() of the list): `first`
+    int hits = 0, first_hit = k, hits_sh = 0, hits_lt = 0, n_lt = 0, n_distinct = 0;
     long long sum_r = 0, sum_pop = 0;
     double dcg = 0, map = 0, epc = 0, efd = 0, norm = 0;
     for (int r = lane; r < n; r += G) {
         const int32_t it = lst[r];
         const double d = disc[r];
         const bool lt = long_tail[it] != 0;
+        bool first = true;
+        for (int j = 0; j < r && first; ++j) first = lst[j] != it;
         norm += d;
         sum_pop += pop[it];
-        n_lt += lt;
+        n_lt += lt && first;
+        n_distinct += first;
         atomicAdd(item_count + it, 1);
         if (n_rel > 0) {
             int64_t a = lo, b = hi;
@@ -111,7 +115,8 @@ __global__ void __launch_bounds__(EM_THREADS) eval_metrics_user_kernel(
                 ++hits;
                 sum_r += r;
                 first_hit = min(first_hit, r);
-                hits_sh += !lt;
+                hits_sh += !lt && first;
+                hits_lt += lt && first;
                 dcg += d;
                 map += map_tail[r];
                 epc += d * nov[2 * (int64_t)it];
@@ -120,7 +125,8 @@ __global__ void __launch_bounds__(EM_THREADS) eval_metrics_user_kernel(
         }
     }
     // all 32 lanes shuffle (groups of one warp may belong to users in different sets)
-    hits = group_sum<G>(hits); hits_sh = group_sum<G>(hits_sh); n_lt = group_sum<G>(n_lt);
+    hits = group_sum<G>(hits); hits_sh = group_sum<G>(hits_sh); hits_lt = group_sum<G>(hits_lt); n_lt = group_sum<G>(n_lt);
+    n_distinct = group_sum<G>(n_distinct);
     first_hit = group_min<G>(first_hit);
     sum_r = group_sum<G>(sum_r); sum_pop = group_sum<G>(sum_pop);
     dcg = group_sum<G>(dcg); map = group_sum<G>(map); epc = group_sum<G>(epc); efd = group_sum<G>(efd);
@@ -145,7 +151,7 @@ __global__ void __launch_bounds__(EM_THREADS) eval_metrics_user_kernel(
         v[EM_EPC] = norm > 0 ? epc / norm : 0.0;
         v[EM_EFD] = norm > 0 ? efd / norm : 0.0;
         v[EM_REO_NUM_H] = hits_sh;
-        v[EM_REO_NUM_T] = hits - hits_sh;
+        v[EM_REO_NUM_T] = hits_lt;
         v[EM_REO_DEN_H] = info[2];
         v[EM_REO_DEN_T] = info[3];
     }
@@ -154,7 +160,7 @@ __global__ void __launch_bounds__(EM_THREADS) eval_metrics_user_kernel(
         v[EM_ARP] = n ? (double)sum_pop / (double)n : 0.0;   // an empty list is counted in EM_EMPTY; the caller raises
         v[EM_APLT] = n ? (double)n_lt / (double)n : 0.0;
         v[EM_ACLT] = n_lt;
-        v[EM_RSP_NUM_H] = n - n_lt;
+        v[EM_RSP_NUM_H] = n_distinct - n_lt;
         v[EM_RSP_NUM_T] = n_lt;
         v[EM_RSP_DEN_H] = info[4];
         v[EM_RSP_DEN_T] = info[5];

@@ -116,8 +116,10 @@ def host_metric_sums(tab, cs, priv_users, idx, k, per_user=False):
     den = p + rc
     norm = (valid * disc).sum(1)
     nz = np.where(norm > 0, norm, 1)
-    lt = valid & (tab.long_tail[Li] == 1)
-    n_lt = lt.sum(1)
+    # ACLT, APLT, PopREO and PopRSP count each listed item once (the reference takes set() of the list)
+    first = valid & ~np.tril(Li[:, :, None] == Li[:, None, :], -1).any(2)
+    lt = first & (tab.long_tail[Li] == 1)
+    n_lt, n_distinct = lt.sum(1), first.sum(1)
     n1 = np.maximum(n, 1)
     with np.errstate(divide="ignore", invalid="ignore"):
         user_b = np.stack([
@@ -137,14 +139,14 @@ def host_metric_sums(tab, cs, priv_users, idx, k, per_user=False):
     with np.errstate(divide="ignore"):
         nov_s = -np.log(np.where(valid, counts[Li], 1) / max(free_norm, 1)) / np.log(2)
     s = np.zeros(N_SLOTS)
-    hits_sh = (hit & ~lt).sum(1)
+    hits_sh, hits_lt = (hit & first & ~lt).sum(1), (hit & lt).sum(1)
     s[S_NREL] = B.sum()
     s[S_RENDLE:S_EFD + 1] = user_b[B].sum(0)
-    s[S_REO_NUM_H], s[S_REO_NUM_T] = hits_sh[B].sum(), (h - hits_sh)[B].sum()
+    s[S_REO_NUM_H], s[S_REO_NUM_T] = hits_sh[B].sum(), hits_lt[B].sum()
     s[S_REO_DEN_H], s[S_REO_DEN_T] = info[B, 2].sum(), info[B, 3].sum()
     s[S_NROWS] = A.sum()
     s[S_ARP:S_ACLT + 1] = user_a[A].sum(0)
-    s[S_RSP_NUM_H], s[S_RSP_NUM_T] = (n - n_lt)[A].sum(), n_lt[A].sum()
+    s[S_RSP_NUM_H], s[S_RSP_NUM_T] = (n_distinct - n_lt)[A].sum(), n_lt[A].sum()
     s[S_RSP_DEN_H], s[S_RSP_DEN_T] = info[A, 4].sum(), info[A, 5].sum()
     s[S_UCOV], s[S_UCOV_N] = (n > 0)[A].sum(), (n >= k)[A].sum()
     s[S_FREE_NORM] = free_norm

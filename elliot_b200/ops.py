@@ -5,8 +5,8 @@ CUDA device — there is no CPU path.
 Streams: every op launches on torch's CURRENT stream of the tensors' device.  The C ABI never allocates, so these ops
 keep grow-only scratch per device from call to call (_scratch): bpr_exact_f64, MtSampler.step, score_topk,
 score_topk_tc, bpr_step_sampled_f32 (the schedule prefetch keeps two schedule slots of its own), gram_f64, eval_topk,
-eval_topk_metrics and vae_train_step; mf_pointwise_step_f32 keeps a global-bias accumulator per device.  Those ops must
-not run concurrently on two streams of the same device from one process.
+eval_topk_metrics, vae_train_step and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
+device.  Those ops must not run concurrently on two streams of the same device from one process.
 """
 import ctypes
 import os
@@ -1039,6 +1039,76 @@ def nnmf_row_update_f64(indptr, cols, pos, ratings, est, T, S, reg, out=None):
     _chk_f64_dense(out)
     _call("eb_nnmf_row_update_f64", S, _ptr(indptr), _ptr(cols), _ptr(pos), S.shape[0], _ptr(ratings), _ptr(est), _ptr(T),
           _ptr(S), _ptr(out), S.shape[1], float(reg))
+    return out
+
+
+# ---------------------------------------------------------------- MostPop and Random (unpersonalized.cu)
+def _train_csr(indptr, train):
+    _need_cuda(indptr, train)
+    _chk_idx(train)
+    assert indptr.dtype == torch.int64 and indptr.is_contiguous()
+    return _nonempty(train)
+
+
+def item_pop(indices, n_items):
+    """pop [n_items] int32: the entries of each item among the train indices (eb_item_pop)."""
+    _need_cuda(indices)
+    _chk_idx(indices)
+    pop = torch.empty(n_items, dtype=torch.int32, device=indices.device)
+    _call("eb_item_pop", pop, _ptr(_nonempty(indices)), indices.numel(), n_items, _ptr(pop))
+    return pop
+
+
+def mostpop_topk(order, pop, k, indptr, train, users=None, user_begin=0, n_sel=None):
+    """MostPop lists (eb_mostpop_topk): (idx int32 [n_sel][k], val int32 [n_sel][k] = pop, skipped int32 device scalar)
+    with `order` every item by (pop desc, item asc) and the sorted train CSR as the mask; a user with |train_u| + k >=
+    n_items gets a row of -1 and is counted in `skipped`."""
+    train = _train_csr(indptr, train)
+    _need_cuda(order, pop, users)
+    _chk_idx(order, pop)
+    n_sel, idx, val = _topk_out(users, indptr.numel() - 1, user_begin, n_sel, k, torch.int32, order.device)
+    skipped = torch.empty((), dtype=torch.int32, device=order.device)
+    _call("eb_mostpop_topk", order, _ptr(order), _ptr(pop), order.numel(), _ptr(indptr), _ptr(train), _ptr(users), user_begin,
+          n_sel, k, _ptr(idx), _ptr(val), _ptr(skipped))
+    return idx, val, skipped
+
+
+class RandomStream:
+    """The legacy np.random stream of `np.random.seed(seed)` on the device, drawn the way the reference's Random does
+    (eb_random_draws): the MT19937 state, a buffer of `capacity` generated words and the position in it persist from
+    call to call, as numpy's global state does."""
+
+    def __init__(self, seed, device, capacity=1 << 20):
+        self.state = torch.empty(625, dtype=torch.int32, device=device)
+        self.words = torch.empty(capacity, dtype=torch.int32, device=device)
+        self.pos = (ctypes.c_int64 * 2)(0, 0)
+        self.consumed = 0
+        _call("eb_mt_seed", self.state, _ptr(self.state), seed)
+
+    def draws(self, k, indptr, n_items):
+        """r [n_users][k] int32: each user's draws, -1 past min(k, n_u).  Reads back how far the walk got (one host
+        synchronise per buffer of words)."""
+        _need_cuda(indptr)
+        assert indptr.dtype == torch.int64 and indptr.is_contiguous()
+        n_users = indptr.numel() - 1
+        r = torch.empty((n_users, k), dtype=torch.int32, device=self.state.device)
+        used = ctypes.c_int64(0)
+        ws = _scratch("random_walk", lib().eb_random_workspace_bytes(), r.device)
+        _call("eb_random_draws", r, _ptr(self.state), _ptr(self.words), self.words.numel(), self.pos, n_users, n_items,
+              _ptr(indptr), k, _ptr(r), ctypes.byref(used), _ptr(ws), ws.numel())
+        self.consumed += used.value
+        return r
+
+
+def complement_select(r, indptr, train, users=None, user_begin=0, n_sel=None):
+    """(users x k) int32: the r-th item outside each user's sorted train row for every r of r [n_users][k], -1 where
+    r < 0 (eb_complement_select)."""
+    train = _train_csr(indptr, train)
+    _need_cuda(r, users)
+    _chk_idx(r)
+    k = r.shape[1]
+    n_sel, out, _ = _topk_out(users, indptr.numel() - 1, user_begin, n_sel, k, torch.int32, r.device)
+    _call("eb_complement_select", r, _ptr(r), _ptr(indptr), _ptr(train), _ptr(users), user_begin, n_sel, k, _ptr(out))
     return out
 
 

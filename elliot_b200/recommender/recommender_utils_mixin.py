@@ -18,7 +18,8 @@ class RecMixin:
         if it is not None and (it + 1) % self._validation_rate:
             return
         on_device = (getattr(self._params, "b200_eval", "host") == "device" and hasattr(self, "get_recommendations_tensors")
-                     and hasattr(self.evaluator, "eval_tensors") and not self._save_recs and not self._negative_sampling)
+                     and hasattr(self.evaluator, "eval_tensors") and not self._save_recs and not self._negative_sampling
+                     and getattr(self, "lists_are_tensors", lambda k: True)(self.evaluator.get_needed_recommendations()))
         self._losses.append(loss)
         counts = None
         if self.evaluator.needs_rank:

@@ -41,11 +41,13 @@ def write_tsv(path, seed=SEED):
 
 
 def experiment_yaml(tsv, out_dir, model_key, block, meta=("save_recs: True",), extra="", model_extra="",
-                    metrics=("nDCG", "HR", "Precision", "Recall")):
+                    metrics=("nDCG", "HR", "Precision", "Recall"), cutoffs=None):
     """The reference's YAML layout (sample_hello_world.yml:1-19) over the C1 file above: one `model_key` block with the
     given `meta` lines (without indentation) and parameter lines (`block`, indented, newline-ended), evaluated with
-    `metrics`.  `extra` goes into the experiment section, `model_extra` after the model's parameters."""
+    `metrics` (at `cutoffs` when given, else at top_k).  `extra` goes into the experiment section, `model_extra` after
+    the model's parameters."""
     meta = "".join(f"        {m}\n" for m in meta)
+    cut = f"    cutoffs: [{', '.join(str(c) for c in cutoffs)}]\n" if cutoffs else ""
     return f"""experiment:
   dataset: c1_synth
   data_config:
@@ -58,7 +60,7 @@ def experiment_yaml(tsv, out_dir, model_key, block, meta=("save_recs: True",), e
   top_k: 10
   evaluation:
     simple_metrics: [{', '.join(metrics)}]
-  path_output_rec_result: {out_dir}/recs
+{cut}  path_output_rec_result: {out_dir}/recs
   path_output_rec_weight: {out_dir}/weights
   path_output_rec_performance: {out_dir}/performance
   path_log_folder: {out_dir}/log
@@ -130,3 +132,13 @@ def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra=""
       negative_item_regularization: 0.00025
       seed: {seed}
 """, meta=(f"save_recs: {save_recs}", "verbose: False"), extra=extra, model_extra=model_extra, metrics=metrics)
+
+
+def unpersonalized_yaml(tsv, out_dir, metrics, cutoffs=(5, 10), mostpop_key="MostPop", random_seed=42, extra="",
+                        model_extra=""):
+    """The reference's experiment files list the baselines first: a `mostpop_key` block (MostPop, or external.MostPop
+    with `extra` naming the plugin) and a `Random` block with `random_seed`, both with save_recs, evaluated with
+    `metrics` at `cutoffs`.  `model_extra` goes after each model's parameters."""
+    head = experiment_yaml(tsv, out_dir, mostpop_key, "", extra=extra, model_extra=model_extra, metrics=metrics,
+                           cutoffs=cutoffs)
+    return head + f"    Random:\n      meta:\n        save_recs: True\n      random_seed: {random_seed}\n{model_extra}"

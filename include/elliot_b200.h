@@ -765,6 +765,34 @@ int eb_nnmf_row_update_f64(const int64_t *indptr, const int32_t *cols, const int
                            const double *ratings, const double *est, const double *T, const double *S, double *S_out, int F,
                            double reg, void *stream);
 
+/* ------------------------------------------------------------------------
+ * MostPop and Random (recommender/unpersonalized/most_popular/most_popular.py, random_recommender/Random.py).
+ * The train CSR indptr [n_users + 1] / train (each row sorted ascending) is also the mask: a user's train items are
+ * never listed.  Output row q is user users[q], or user_begin + q when users is NULL.
+ * eb_item_pop: pop[i] = number of entries of item i among the nnz train indices (integer atomics; pop is zeroed first).
+ * eb_mostpop_topk: order = every item by (pop desc, item asc).  Row q gets the first k items of that order outside the
+ *   user's train row, out_val = their pop.  A user with |train_u| + k >= n_items gets a row of -1 (the reference lists
+ *   nothing for it); *skipped (device int32) = the number of such rows.  Slots past the list: -1 / 0.  k >= 1.
+ * eb_random_draws: the reference's np.random.randint(n_u) draws for every user in order (n_u = n_items - |train_u|,
+ *   min(k, n_u) draws each, none when n_u <= 1), from the legacy MT19937 stream of eb_mt_seed / eb_mt_raw.  words
+ *   [capacity] holds generated stream words; pos_host (HOST int64[2]) = (next unread word, words held) and is updated;
+ *   when the held words run out, the buffer is refilled with the next `capacity` words of `state`.  r_out [n_users][k]
+ *   gets the drawn values, -1 past min(k, n_u); *consumed_host (HOST) = the stream words this call used.  Synchronises
+ *   the stream once per buffer's worth of words.  One warp walks the words: the walk is serial.
+ * eb_complement_select: out[q][j] = the r-th (0-based) item outside the user's train row for r = r_in[u][j] (row u of
+ *   [n_users][k]), -1 where r < 0.
+ * ------------------------------------------------------------------------ */
+int eb_item_pop(const int32_t *indices, int64_t nnz, int32_t n_items, int32_t *pop, void *stream);
+int eb_mostpop_topk(const int32_t *order, const int32_t *pop, int32_t n_items, const int64_t *indptr, const int32_t *train,
+                    const int32_t *users, int32_t user_begin, int64_t n_sel, int k, int32_t *out_idx, int32_t *out_val,
+                    int32_t *skipped, void *stream);
+size_t eb_random_workspace_bytes(void);
+int eb_random_draws(uint32_t *state, uint32_t *words, int64_t capacity, int64_t *pos_host, int32_t n_users, int32_t n_items,
+                    const int64_t *indptr, int k, int32_t *r_out, int64_t *consumed_host, void *workspace,
+                    size_t workspace_bytes, void *stream);
+int eb_complement_select(const int32_t *r_in, const int64_t *indptr, const int32_t *train, const int32_t *users,
+                         int32_t user_begin, int64_t n_sel, int k, int32_t *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
