@@ -116,9 +116,10 @@ class DataSet:
             return self._split_dict("val")
         raise AttributeError(name)
 
-    def eval_arrays(self, which):
+    def eval_arrays(self, which, public=False):
         """(private user, private item or -1, rating) of the split's rows whose user is a train user, grouped by user in
-        train-user order, (user, item) duplicates reduced like a dict — the vectorised source of eval_csr_of."""
+        train-user order, (user, item) duplicates reduced like a dict — the vectorised source of eval_csr_of.
+        public=True adds the rows' public item ids, which test-only items keep."""
         if which not in self._eval_frames:
             return None
         df = self._eval_frames[which]
@@ -137,7 +138,7 @@ class DataSet:
             keep = np.sort(first)
             pu, raw_items, r = pu[keep], raw_items[keep], last_r[inv[keep]]
         pi = pd.Index(self.items).get_indexer(raw_items).astype(np.int64)              # -1: test-only item
-        return pu, pi, r
+        return (pu, pi, r, raw_items) if public else (pu, pi, r)
 
     # ---- reference accessors ---------------------------------------------------------------
     def get_test(self):

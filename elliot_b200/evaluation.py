@@ -8,11 +8,17 @@ finish_auc, not from the lists, and are the same at every cutoff (tests/test_ora
 
 `eval_tensors` is the device path (SURVEY.md §8f #1): the top-k index tensor written by the scoring kernels is
 scored against the test set by `eb_eval_topk_f64` (the four above) and `eb_eval_metrics_f64` (the 19 others) without
-ever becoming Python tuples; same definitions, same numbers (fp64; summation order differs, <= 1e-12 relative)."""
+ever becoming Python tuples; same definitions, same numbers (fp64; summation order differs, <= 1e-12 relative).
+
+`evaluation.complex_metrics` entries add the reference's clustered fairness metrics (fairness.py): one pass over the
+lists per pair of clustering files (`eb_eval_fairness_f64` on the device, fairness.host_fairness_sums on the host), their
+keys after the simple metrics in entry order."""
 import math
 
 import numpy as np
+import pandas as pd
 
+from . import fairness
 from .dataset import eval_csr_of, eval_users_of
 
 SUPPORTED = {"ndcg": "nDCG", "hr": "HR", "precision": "Precision", "recall": "Recall"}
@@ -164,6 +170,18 @@ def host_metric_sums(tab, cs, priv_users, idx, k, per_user=False):
     return s, pv
 
 
+def ideal_dcg(cs, k):
+    """Per private user, the DCG@k of its relevant items in descending gain order (the nDCG denominator)."""
+    indptr, idx, gain = cs
+    n = len(indptr) - 1
+    rows = np.repeat(np.arange(n), np.diff(indptr))
+    disc = np.array([math.log(2) / math.log(r + 2) for r in range(k)])      # relevance.py:55
+    by_gain = np.lexsort((-gain, rows))                                      # ideal ranking per user
+    rank = np.arange(len(rows)) - indptr[rows]
+    top = rank < k
+    return np.bincount(rows[top], weights=gain[by_gain][top] * disc[rank[top]], minlength=n)
+
+
 def finish_auc(n_pos, sum_c, n_rel, n_train, n_items, names):
     """AUC and GAUC (auc.py, gauc.py) from the rank pass's per-user counts (ops.score_rank): n_pos relevant items in the
     user's full list and sum_c, the sum over them of the non-relevant entries ahead of each.  With neg_u = n_items -
@@ -242,6 +260,8 @@ class Evaluator:
         self._basic = [m for m in self._metrics if m in SUPPORTED.values()]
         self._extended = [m for m in self._metrics if m in METRICS]
         self._ranked = [m for m in self._metrics if m in RANK]
+        # complex_metrics: the clustered fairness metrics, each entry checked (name, clustering files) here
+        self._complex = [fairness.Entry(e) for e in (getattr(ev, "complex_metrics", None) or [])]
         self._sets = {"test": eval_csr_of(data, "test"), "val": eval_csr_of(data, "val")}
 
     def get_needed_recommendations(self):
@@ -252,6 +272,11 @@ class Evaluator:
         """True when AUC or GAUC is asked for: evaluate() then runs the model's rank pass once per split
         (rank_sets / rank_counts) besides its top-k lists."""
         return bool(self._ranked)
+
+    @property
+    def needs_scores(self):
+        """True when UserMADrating or ItemMADrating is asked for: eval_tensors() then needs the lists' scores (vals)."""
+        return any(e.needs_scores for e in self._complex)
 
     def rank_sets(self, device):
         """{split: (rel indptr int64, item-sorted rel items int32)} on `device` for every split that exists: the
@@ -306,13 +331,9 @@ class Evaluator:
             cache[key] = None
             return None
         indptr, idx, gain = cs
-        n = len(indptr) - 1
-        rows = np.repeat(np.arange(n), np.diff(indptr))
+        rows = np.repeat(np.arange(len(indptr) - 1), np.diff(indptr))
         disc = np.array([math.log(2) / math.log(r + 2) for r in range(k)])      # relevance.py:55
-        by_gain = np.lexsort((-gain, rows))                                      # ideal ranking per user
-        rank = np.arange(len(rows)) - indptr[rows]
-        top = rank < k
-        idcg = np.bincount(rows[top], weights=gain[by_gain][top] * disc[rank[top]], minlength=n)
+        idcg = ideal_dcg(cs, k)
         by_item = np.lexsort((idx, rows))                                        # lookup rows sorted by item id
         t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=device, dtype=dt)
         cache[key] = (t(indptr, torch.int64), t(idx[by_item], torch.int32), t(gain[by_item], torch.float64),
@@ -332,10 +353,23 @@ class Evaluator:
                           *(t(a, torch.float64) for a in position_tables(k)))
         return cache[key]
 
-    def eval_tensors(self, idx, users=None, rank_counts=None):
+    def eval_tensors(self, idx, users=None, rank_counts=None, vals=None):
         """Same result structure as eval(), from a device (rows x top_k) int32 tensor of PRIVATE item ids
-        (-1 = empty), row r = private user r (or users[r])."""
+        (-1 = empty), row r = private user r (or users[r]); vals: the lists' scores (rows x top_k), needed by
+        UserMADrating / ItemMADrating."""
         from . import ops
+        if vals is None and self.needs_scores:
+            raise Exception(f"{', '.join(e.metric for e in self._complex if e.needs_scores)} need the lists' scores: "
+                            f"pass vals= to eval_tensors")
+        scores, rows = (vals if self.needs_scores else None), None
+        if self._complex:
+            rows = users.cpu().numpy().astype(np.int64) if users is not None else np.arange(idx.shape[0])
+
+        def run(which, k, key, ucl, nu, icl, ni):
+            has_rows, ucl_d, icl_d = self._fair_device(which, key, idx.device)
+            c, s = ops.eval_fairness(idx, k, *self._device_set(which, k, idx.device), has_rows, ucl_d, nu, icl_d, ni,
+                                     scores=scores, users=users)
+            return c.cpu().numpy(), s.cpu().numpy()
         out = {}
         ranked = {w: self._rank_values(w, rank_counts) for w in ("val", "test") if self._sets[w] is not None}
         for k in self._k:
@@ -355,6 +389,7 @@ class Evaluator:
                     s, _ = ops.eval_topk_metrics(idx, k, *self._metric_device_set(which, k, idx.device), users=users)
                     vals.update(finish_metrics(s.cpu().numpy(), k, self._tables(which).n_items, self._extended))
                 res[which] = {m: vals[m] for m in self._metrics}
+                res[which].update(self._complex_values(which, k, rows, lambda *a, w=which, k=k: run(w, k, *a)))
             if res["val"] is None:
                 res["val"] = res["test"]
             if res["test"] is None:
@@ -367,9 +402,12 @@ class Evaluator:
         pub_u, pub_i = self._data.public_users, self._data.public_items
         users = [u for u in recs if u in pub_u]
         idx = np.full((len(users), k), -1, np.int64)
+        scores = np.zeros((len(users), k)) if self.needs_scores else None
         for r, u in enumerate(users):
             row = [pub_i.get(it, -1) for it, _ in recs[u][:k]]
             idx[r, :len(row)] = row
+            if scores is not None:
+                scores[r, :len(row)] = [v for _, v in recs[u][:k]]
         priv = np.array([pub_u[u] for u in users], np.int64)
         vals = self.eval_arrays(priv, idx, self._sets[which], k) if self._basic else {}
         if self._extended:
@@ -377,7 +415,88 @@ class Evaluator:
             s, _ = host_metric_sums(tab, self._sets[which], priv, idx, k)
             vals.update(finish_metrics(s, k, tab.n_items, self._extended))
         vals.update(ranked)
-        return {m: vals[m] for m in self._metrics}
+        out = {m: vals[m] for m in self._metrics}
+        if self._complex:
+            cs, idcg, has_rows = self._sets[which], ideal_dcg(self._sets[which], k), self._has_rows(which)
+            out.update(self._complex_values(which, k, priv, lambda key, ucl, nu, icl, ni: fairness.host_fairness_sums(
+                priv, idx, scores, k, cs, idcg, has_rows, ucl, nu, icl, ni)))
+        return out
+
+    # ---- complex metrics (fairness.py) ---------------------------------------------------------
+    def _has_rows(self, which):
+        cache = self.__dict__.setdefault("_has_rows_cache", {})
+        if which not in cache:
+            cache[which] = eval_users_of(self._data, which)
+        return cache[which]
+
+    def _clusterings(self, key):
+        """(user labels int32 per private user, n user clusters, item labels per private item, n item clusters) of a
+        pass key (fairness.Entry.launch), cached."""
+        cache = self.__dict__.setdefault("_cluster_tables", {})
+        if key not in cache:
+            e = next(e for e in self._complex if e.launch == key)
+            cache[key] = (fairness.private_labels(e.users, self._data.users, e.udefault), e.nu,
+                          fairness.private_labels(e.items, self._data.items, e.idefault), e.ni)
+        return cache[key]
+
+    def _fair_device(self, which, key, device):
+        """(has_rows uint8, user labels, item labels) on `device` for a split and pass key (cached)."""
+        import torch
+        cache = self.__dict__.setdefault("_fair_dev", {})
+        ck = (which, key, str(device))
+        if ck not in cache:
+            ucl, _, icl, _ = self._clusterings(key)
+            t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=device, dtype=dt)
+            cache[ck] = (t(self._has_rows(which), torch.uint8), t(ucl, torch.int32), t(icl, torch.int32))
+        return cache[ck]
+
+    def _parity_den(self, e, which, rows):
+        """REO (sum over rows' users with a relevant item of |(c & rel_u) - train_u|) or RSP (sum over rows' users with
+        test rows of |c - train_u|) denominators per item cluster c of the file, ids outside the catalogue included."""
+        if e.items is None:
+            return np.zeros(1)
+        data, cl = self._data, e.items
+        sel = np.zeros(len(data.users), bool)
+        sel[rows] = True
+        sel &= self._has_rows(which)
+        m = data.sp_i_train.tocsr()
+        if e.metric == "REO":
+            sel &= np.diff(self._sets[which][0]) > 0
+            cache = self.__dict__.setdefault("_reo_rel", {})
+            if (which, cl.path) not in cache:
+                pu, pub, pi = fairness.relevant_public(data, which)
+                pos = pd.Index(cl.ids).get_indexer(pub)
+                c = np.where(pos >= 0, cl.labels[np.maximum(pos, 0)], -1)
+                in_train = np.zeros(len(pu), bool)
+                known = pi >= 0
+                in_train[known] = np.asarray(m[pu[known], pi[known]]).ravel() != 0
+                keep = (c >= 0) & ~in_train
+                cache[(which, cl.path)] = (pu[keep], c[keep])
+            pu, c = cache[(which, cl.path)]
+            return np.bincount(c[sel[pu]], minlength=cl.n)
+        icl = self._clusterings(e.launch)[2]
+        rows_t = np.repeat(np.arange(m.shape[0]), np.diff(m.indptr))
+        c = icl[m.indices]
+        ok = sel[rows_t] & (c >= 0)
+        return int(sel.sum()) * cl.sizes - np.bincount(c[ok], minlength=cl.n)
+
+    def _complex_values(self, which, k, rows, run):
+        """{key: value} of every complex entry for a split at cutoff k; run(key, *clusterings) gives a pass's
+        (counts, sums), once per pass key."""
+        out, passes = {}, {}
+        for e in self._complex:
+            if e.launch not in passes:
+                passes[e.launch] = run(e.launch, *self._clusterings(e.launch))
+            extra = {}
+            if e.metric.startswith("BiasDisparity"):
+                ucl, nu, icl, ni = self._clusterings(e.launch)
+                extra["pc"] = e.items.sizes / len(e.items.ids) if e.items is not None else np.ones(1)
+                if e.metric != "BiasDisparityBR":
+                    extra["bs"] = fairness.bias_source(self._data, ucl, nu, icl, ni, extra["pc"])
+            elif e.metric in ("REO", "RSP"):
+                extra["den"] = self._parity_den(e, which, rows)
+            out.update(fairness.finish(e, *passes[e.launch], **extra))
+        return out
 
     def eval_arrays(self, priv_users, idx, cs, k):
         """idx: (n, >=k) private item ids (−1 = empty slot), rows aligned with priv_users."""

@@ -5,7 +5,7 @@ CUDA device — there is no CPU path.
 Streams: every op launches on torch's CURRENT stream of the tensors' device.  The C ABI never allocates, so these ops
 keep grow-only scratch per device from call to call (_scratch): bpr_exact_f64, MtSampler.step, score_topk,
 score_topk_tc, bpr_step_sampled_f32 (the schedule prefetch keeps two schedule slots of its own), gram_f64, eval_topk,
-eval_topk_metrics, vae_train_step and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
+eval_topk_metrics, eval_fairness, vae_train_step and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
 device.  Those ops must not run concurrently on two streams of the same device from one process.
 """
 import ctypes
@@ -1266,6 +1266,42 @@ def eval_topk_metrics(topk_idx, k, rel_indptr, rel_items, user_info, item_pop, i
           _ptr(rel_items), _ptr(user_info), _ptr(item_pop), _ptr(item_long_tail), _ptr(item_novelty), n_items, _ptr(discount),
           _ptr(map_tail), _ptr(inv_binary_idcg), _ptr(pu), _ptr(out), _ptr(ws), ws.numel())
     return out, pu
+
+
+def eval_fairness(topk_idx, k, rel_indptr, rel_items, rel_gains, idcg, discount, has_rows, user_cluster, n_user_clusters,
+                  item_cluster, n_item_clusters, scores=None, users=None):
+    """Counts and sums of the reference's clustered fairness metrics over a (rows x >=k) int32 top-k index tensor
+    (eval_fairness.cu; layout in include/elliot_b200.h).  scores: the lists' (rows x >=k) scores, fp64 or fp32 (cast
+    once, exactly), read only by the rating sums.  Returns (counts int64, sums fp64) device tensors."""
+    _need_cuda(topk_idx, rel_indptr, rel_items, rel_gains, idcg, discount, has_rows, user_cluster, item_cluster, scores,
+               users)
+    assert topk_idx.dtype == torch.int32 and topk_idx.stride(1) == 1 and topk_idx.shape[1] >= k
+    assert rel_indptr.dtype == torch.int64 and rel_items.dtype == torch.int32
+    for t in (rel_gains, idcg, discount):
+        assert t.dtype == torch.float64 and t.is_contiguous()
+    assert discount.numel() >= k
+    n_users = rel_indptr.numel() - 1
+    assert has_rows.dtype == torch.uint8 and has_rows.numel() == n_users
+    _chk_idx(user_cluster, item_cluster)
+    assert user_cluster.numel() == n_users and n_user_clusters >= 1 and n_item_clusters >= 1
+    n = topk_idx.shape[0]
+    if users is not None:
+        _chk_idx(users); assert users.numel() == n
+    if scores is not None:
+        assert scores.shape[0] == n and scores.shape[1] >= k
+        if scores.dtype != torch.float64 or scores.stride() != topk_idx.stride():
+            scores = torch.empty_strided(topk_idx.shape, topk_idx.stride(), dtype=torch.float64,
+                                         device=topk_idx.device).copy_(scores[:, :topk_idx.shape[1]])
+    dev = topk_idx.device
+    nu, ni, n_items = int(n_user_clusters), int(n_item_clusters), item_cluster.numel()
+    counts = torch.empty(nu + nu * ni + 3 * ni, dtype=torch.int64, device=dev)
+    sums = torch.empty(2 * nu + 2 * ni, dtype=torch.float64, device=dev)
+    ws = _scratch("eval_fairness", lib().eb_eval_fairness_workspace_bytes(n, k, n_items, nu, ni), dev)
+    _call("eb_eval_fairness_f64", topk_idx, _ptr(topk_idx), _ptr(scores), n, topk_idx.stride(0), k, _ptr(users),
+          _ptr(rel_indptr), _ptr(rel_items), _ptr(rel_gains), _ptr(idcg), _ptr(discount), _ptr(has_rows),
+          _ptr(user_cluster), nu, _ptr(_nonempty(item_cluster)), ni, n_items, _ptr(counts), _ptr(sums), _ptr(ws),
+          ws.numel())
+    return counts, sums
 
 
 def partition_streams(device, reserve_sms, n_streams=1):

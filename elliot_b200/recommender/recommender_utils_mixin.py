@@ -30,9 +30,11 @@ class RecMixin:
         if on_device:
             # extension: the (users x k) index tensor goes from the scoring kernel straight into the metric
             # kernel; no {user: [(item, score)]} dicts are built (recommender_utils_mixin.py:84-88 / evaluator.py:117-147)
-            idx, _ = self.get_recommendations_tensors(self.evaluator.get_needed_recommendations())
+            idx, val = self.get_recommendations_tensors(self.evaluator.get_needed_recommendations())
             recs = None
-            self._results.append(self.evaluator.eval_tensors(idx, rank_counts=counts))
+            # UserMADrating / ItemMADrating read the lists' scores; no other metric does
+            scores = val if getattr(self.evaluator, "needs_scores", False) else None
+            self._results.append(self.evaluator.eval_tensors(idx, rank_counts=counts, **({"vals": scores} if scores is not None else {})))
         else:
             recs = self.get_recommendations(self.evaluator.get_needed_recommendations())
             self._results.append(self.evaluator.eval(recs, rank_counts=counts))

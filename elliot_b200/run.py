@@ -13,6 +13,7 @@ import importlib.util
 import json
 import math
 import os
+import re
 from types import SimpleNamespace
 
 import numpy as np
@@ -26,6 +27,24 @@ COLS = ["userId", "itemId", "rating", "timestamp"]
 
 def _abs(cfg_dir, p):
     return p if os.path.isabs(p) else os.path.abspath(os.path.join(cfg_dir, p))
+
+
+# a word, a dot and a word somewhere in the value, after a first character that is not a digit: a file name
+_FILE_LIKE = re.compile(r"[\D][\w-]+\.[\w-]+")
+
+
+def resolve_param(cfg_dir, value, dataset):
+    """A complex metric parameter as the reference's namespace builder reads it: strings get `{0}` = the dataset name;
+    an absolute path is kept (normalised), a relative one starting with `.` or looking like a file name is taken from
+    the config file's folder, any other string is a plain value.  Non-strings are returned as they are."""
+    if not isinstance(value, str):
+        return value
+    value = value.format(dataset)
+    if os.path.isabs(value):
+        return os.path.abspath(value)
+    if value.startswith(".") or _FILE_LIKE.search(value):
+        return os.path.abspath(os.path.join(cfg_dir, value))
+    return value
 
 
 def _read(path, binarize):
@@ -71,6 +90,8 @@ def build_base_config(path):
         evaluation=SimpleNamespace(simple_metrics=ev.get("simple_metrics", ["nDCG"]),
                                    relevance_threshold=ev.get("relevance_threshold", 0),
                                    paired_ttest=False, wilcoxon_test=False,
+                                   complex_metrics=[{k: resolve_param(cfg_dir, v, name) for k, v in entry.items()}
+                                                    for entry in ev.get("complex_metrics") or []],
                                    **({"cutoffs": ev["cutoffs"]} if "cutoffs" in ev else {})),
         data_config=SimpleNamespace(**raw["data_config"]),
         splitting=raw.get("splitting"),

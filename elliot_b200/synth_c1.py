@@ -41,13 +41,16 @@ def write_tsv(path, seed=SEED):
 
 
 def experiment_yaml(tsv, out_dir, model_key, block, meta=("save_recs: True",), extra="", model_extra="",
-                    metrics=("nDCG", "HR", "Precision", "Recall"), cutoffs=None):
+                    metrics=("nDCG", "HR", "Precision", "Recall"), cutoffs=None, complex_metrics=None):
     """The reference's YAML layout (sample_hello_world.yml:1-19) over the C1 file above: one `model_key` block with the
     given `meta` lines (without indentation) and parameter lines (`block`, indented, newline-ended), evaluated with
-    `metrics` (at `cutoffs` when given, else at top_k).  `extra` goes into the experiment section, `model_extra` after
-    the model's parameters."""
+    `metrics` (at `cutoffs` when given, else at top_k) and the `complex_metrics` entries (dicts) when given.  `extra`
+    goes into the experiment section, `model_extra` after the model's parameters."""
     meta = "".join(f"        {m}\n" for m in meta)
     cut = f"    cutoffs: [{', '.join(str(c) for c in cutoffs)}]\n" if cutoffs else ""
+    if complex_metrics:
+        cut += "    complex_metrics:\n" + "".join(
+            "".join(f"    {'-' if j == 0 else ' '} {k}: {v}\n" for j, (k, v) in enumerate(e.items())) for e in complex_metrics)
     return f"""experiment:
   dataset: c1_synth
   data_config:
@@ -135,10 +138,11 @@ def yaml_text(tsv, out_dir, model_key, epochs, factors, extra="", model_extra=""
 
 
 def unpersonalized_yaml(tsv, out_dir, metrics, cutoffs=(5, 10), mostpop_key="MostPop", random_seed=42, extra="",
-                        model_extra=""):
+                        model_extra="", complex_metrics=None):
     """The reference's experiment files list the baselines first: a `mostpop_key` block (MostPop, or external.MostPop
     with `extra` naming the plugin) and a `Random` block with `random_seed`, both with save_recs, evaluated with
-    `metrics` at `cutoffs`.  `model_extra` goes after each model's parameters."""
+    `metrics` at `cutoffs` and the `complex_metrics` entries when given.  `model_extra` goes after each model's
+    parameters."""
     head = experiment_yaml(tsv, out_dir, mostpop_key, "", extra=extra, model_extra=model_extra, metrics=metrics,
-                           cutoffs=cutoffs)
+                           cutoffs=cutoffs, complex_metrics=complex_metrics)
     return head + f"    Random:\n      meta:\n        save_recs: True\n      random_seed: {random_seed}\n{model_extra}"

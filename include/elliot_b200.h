@@ -399,6 +399,30 @@ int eb_eval_metrics_f64(const int32_t *topk_idx, int64_t n_rows, int ld, int k, 
                         const double *inv_binary_idcg, double *per_user, double *out, void *workspace,
                         size_t workspace_bytes, void *stream);
 
+/* ------------------------------------------------------------------------
+ * The reference's clustered fairness metrics, on the device (elliot/evaluation/metrics/fairness: BiasDisparityBR / BD,
+ * User/ItemMADrating, User/ItemMADranking, REO, RSP).  topk_idx / ld / k / users and the relevant CSR with its gains,
+ * per-user IDCG@k and discounts as for eb_eval_topk_f64; a row's list is its entries before the first -1.  scores
+ * (optional, fp64, same ld as topk_idx): the lists' scores, read only for the rating sums.  has_rows[n_users]: the user
+ * has any test row.  user_cluster[n_users] / item_cluster[n_items]: the cluster of each private id in 0..n-1, -1 = not
+ * clustered.  A row counts when its user has test rows (A); the per-user and per-item sums also need >= 1 relevant
+ * item (B).
+ * counts (int64, n_user_clusters + n_user_clusters * n_item_clusters + 3 * n_item_clusters):
+ *   [nu] B users per user cluster | [nu][ni] list entries of A users per (user cluster, item cluster), repeated items
+ *   every time | [ni] distinct listed relevant items of B users (REO numerators) | [ni] distinct listed items of A users
+ *   (RSP numerators) | [ni] listed items of B users per item cluster.
+ * sums (fp64, 2 * nu + 2 * ni, deterministic): [nu] sum of nDCG over B users (each the bits eb_eval_topk_f64 gives) |
+ *   [nu] sum of the mean list score (NaN for an empty list) | [ni] sum over listed items of their summed gains / count |
+ *   [ni] sum over listed items of their summed relevant scores / count; an item's sums run in row, then list order.
+ * ------------------------------------------------------------------------ */
+size_t eb_eval_fairness_workspace_bytes(int64_t n_rows, int k, int n_items, int n_user_clusters, int n_item_clusters);
+int eb_eval_fairness_f64(const int32_t *topk_idx, const double *scores, int64_t n_rows, int ld, int k,
+                         const int32_t *users, const int64_t *rel_indptr, const int32_t *rel_items,
+                         const double *rel_gains, const double *idcg, const double *discount, const uint8_t *has_rows,
+                         const int32_t *user_cluster, int n_user_clusters, const int32_t *item_cluster,
+                         int n_item_clusters, int n_items, int64_t *counts, double *sums, void *workspace,
+                         size_t workspace_bytes, void *stream);
+
 /* SM partition for compute/collective overlap (no reference counterpart): creates a green context holding
  * all but >= reserve_sms SMs of the current device (rounded to the driver's 8-SM granularity) and n_streams
  * CUDA streams bound to it.  Kernels launched on those streams run only inside the partition, so a collective
