@@ -16,23 +16,26 @@ __global__ void __launch_bounds__(256) gemm_f32_ref_kernel(const float *__restri
                                                            const float *__restrict__ bias, float alpha, int act) {
     __shared__ float sa[16][17], sb[16][17];
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    const int m = blockIdx.y * 16 + ty, n = blockIdx.x * 16 + tx;
-    float acc = 0.f;
-    for (int k0 = 0; k0 < K; k0 += 16) {
-        const int ka = k0 + tx, ma = blockIdx.y * 16 + ty;             // A tile element (ma, ka)
-        sa[ty][tx] = (ma < M && ka < K) ? (a_mn ? A[(int64_t)ka * lda + ma] : A[(int64_t)ma * lda + ka]) : 0.f;
-        const int kb = k0 + ty, nb = blockIdx.x * 16 + tx;             // B tile element (nb, kb)
-        sb[ty][tx] = (nb < N && kb < K) ? (b_mn ? B[(int64_t)kb * ldb + nb] : B[(int64_t)nb * ldb + kb]) : 0.f;
-        __syncthreads();
+    const int n = blockIdx.x * 16 + tx;
+    for (int mt = blockIdx.y; mt * 16 < M; mt += gridDim.y) {          // row tiles beyond the 65535 of grid.y: loop
+        const int m = mt * 16 + ty;
+        float acc = 0.f;
+        for (int k0 = 0; k0 < K; k0 += 16) {
+            const int ka = k0 + tx;                                     // A tile element (m, ka)
+            sa[ty][tx] = (m < M && ka < K) ? (a_mn ? A[(int64_t)ka * lda + m] : A[(int64_t)m * lda + ka]) : 0.f;
+            const int kb = k0 + ty, nb = blockIdx.x * 16 + tx;         // B tile element (nb, kb)
+            sb[ty][tx] = (nb < N && kb < K) ? (b_mn ? B[(int64_t)kb * ldb + nb] : B[(int64_t)nb * ldb + kb]) : 0.f;
+            __syncthreads();
 #pragma unroll
-        for (int k = 0; k < 16; k++) acc = fmaf(sa[ty][k], sb[k][tx], acc);
-        __syncthreads();
-    }
-    if (m < M && n < N) {
-        float x = alpha * acc + (bias ? bias[n] : 0.f);
-        if (act == 1) x = tanhf(x);
-        else if (act == 2) x = fmaxf(x, 0.f);
-        C[(int64_t)m * ldc + n] = x;
+            for (int k = 0; k < 16; k++) acc = fmaf(sa[ty][k], sb[k][tx], acc);
+            __syncthreads();
+        }
+        if (m < M && n < N) {
+            float x = alpha * acc + (bias ? bias[n] : 0.f);
+            if (act == 1) x = tanhf(x);
+            else if (act == 2) x = fmaxf(x, 0.f);
+            C[(int64_t)m * ldc + n] = x;
+        }
     }
 }
 
@@ -43,8 +46,8 @@ extern "C" int eb_gemm_f32_ref(const float *A, int64_t lda, int a_rows_are_k, co
     using namespace eb;
     EB_ARG(A && B && C && M >= 1 && N >= 1 && K >= 1 && ldc >= N && act >= 0 && act <= 2, "bad argument");
     EB_ARG(lda >= (a_rows_are_k ? M : K) && ldb >= (b_rows_are_k ? N : K), "leading dimensions too small");
-    dim3 grid((unsigned)((N + 15) / 16), (unsigned)((M + 15) / 16));
-    EB_ARG(grid.y <= 65535, "M too large for the checking kernel");
+    const int m_tiles = (M + 15) / 16;
+    dim3 grid((unsigned)((N + 15) / 16), (unsigned)(m_tiles < 65535 ? m_tiles : 65535));
     gemm_f32_ref_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(A, lda, a_rows_are_k, B, ldb, b_rows_are_k, C, ldc, M, N, K, bias, alpha, act);
     EB_CUDA(cudaGetLastError());
     return EB_OK;

@@ -30,7 +30,8 @@ struct GemmParams {
     int M, N, K;
     int act;             // 0 none, 1 tanh, 2 relu
     float alpha;         // C = alpha * (A B^T) + bias, then activation
-    int splits;          // split-K factor: > 1 -> each work item covers a K range and ADDS into a zeroed C (no bias/act)
+    int splits;          // split-K factor: > 1 -> each work item covers a K range and STORES its partial tile into ws
+    float *ws;           // split-K partials [splits][M][N], summed into C in split order by splitk_reduce_kernel
     __nv_bfloat16 *Cb;   // optional second output: the same values as bf16 rows (row stride ldcb) — the next layer's operand copy
     int64_t ldcb;
 };
@@ -136,8 +137,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     float x0 = p.alpha * acc[4 * j + 2 * half], x1 = p.alpha * acc[4 * j + 2 * half + 1];
                     const bool two = col + 1 < p.N;
                     if (p.splits > 1) {
-                        red_add_f32(crow + col, x0);
-                        if (two) red_add_f32(crow + col + 1, x1);
+                        float *wrow = p.ws + ((int64_t)split * p.M + row) * p.N;
+                        wrow[col] = x0;
+                        if (two) wrow[col + 1] = x1;
                         continue;
                     }
                     if (p.bias) { x0 += __ldg(p.bias + col); if (two) x1 += __ldg(p.bias + col + 1); }
@@ -152,6 +154,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         }
+    }
+}
+
+// C[r][c] = sum_s ws[s][r][c], s = 0, 1, ... in order: the split-K sum is the same bits on every run
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(const float *__restrict__ ws, int splits, int M, int N, float *__restrict__ C,
+                                                            int64_t ldc) {
+    const int64_t total = (int64_t)M * N;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        float t = ws[e];
+        for (int s = 1; s < splits; s++) t += ws[(int64_t)s * total + e];
+        const int64_t r = e / N;
+        C[r * ldc + (e - r * N)] = t;
     }
 }
 
@@ -228,8 +242,8 @@ extern "C" int eb_convert_bf16(const float *src, int rows, int cols, int64_t ld,
 }
 
 static int gemm_bf16(const void *A_bf16, int64_t lda, bool a_mn, const void *B_bf16, int64_t ldb, bool b_mn, float *C, int64_t ldc,
-                     int M, int N, int K, const float *bias, float alpha, int act, void *stream, void *C_bf16 = nullptr,
-                     int64_t ldcb = 0) {
+                     int M, int N, int K, const float *bias, float alpha, int act, void *ws, size_t ws_bytes, void *stream,
+                     void *C_bf16 = nullptr, int64_t ldcb = 0) {
     EB_ARG(A_bf16 && B_bf16 && C, "null pointer");
     EB_ARG(M >= 1 && N >= 1 && K >= 1 && lda >= (a_mn ? M : K) && ldb >= (b_mn ? N : K) && ldc >= N, "bad shape M=%d N=%d K=%d", M, N, K);
     EB_ARG(lda % 8 == 0 && ldb % 8 == 0, "lda/ldb must be multiples of 8 bf16 (16-byte TMA strides)");
@@ -242,23 +256,21 @@ static int gemm_bf16(const void *A_bf16, int64_t lda, bool a_mn, const void *B_b
     const int n_out_tiles = ((M + G_BM - 1) / G_BM) * ((N + G_BN - 1) / G_BN);
     const int k_blocks = (K + G_BK - 1) / G_BK;
     // split-K: few output tiles with a long K (dh2 = dlogits . W4: 20 tiles, K = 26 744) leave most SMs idle and each
-    // busy CTA load-latency bound; split the K range over the idle SMs and add the partial tiles into a zeroed C
-    // (the partial tiles are ADDED with atomics: the summation order, hence the last bits, vary from run to run;
-    // EB_GEMM_SPLITK=0 keeps every GEMM single-pass and bit-reproducible at the cost of idle SMs on these shapes)
+    // busy CTA load-latency bound; split the K range over the idle SMs, store the partial tiles into the caller's workspace
+    // and sum them in split order (bit-reproducible: a run-to-run change in the last bits would move bf16 operand copies
+    // of the result by a whole bf16 ulp).  No workspace, or EB_GEMM_SPLITK=0: every GEMM single-pass.
     static const bool splitk_off = [] { const char *e = getenv("EB_GEMM_SPLITK"); return e && e[0] == '0'; }();
     int splits = 1;
-    if (!splitk_off && !bias && act == 0 && !C_bf16 && n_out_tiles * 2 <= sm_count() && k_blocks >= 16) {
+    if (!splitk_off && ws && !bias && act == 0 && !C_bf16 && n_out_tiles * 2 <= sm_count() && k_blocks >= 16) {
         splits = sm_count() / n_out_tiles;
         if (splits > k_blocks / 8) splits = k_blocks / 8;           // at least 8 k-blocks per work item
         if (splits < 1) splits = 1;
         const int per = (k_blocks + splits - 1) / splits;
         splits = (k_blocks + per - 1) / per;                         // no empty trailing splits
     }
-    GemmParams p{C, ldc, bias, M, N, K, act, alpha, splits, (__nv_bfloat16 *)C_bf16, ldcb};
-    if (splits > 1) {
-        if (ldc == N) EB_CUDA(cudaMemsetAsync(C, 0, (size_t)M * N * sizeof(float), (cudaStream_t)stream));
-        else EB_CUDA(cudaMemset2DAsync(C, (size_t)ldc * sizeof(float), 0, (size_t)N * sizeof(float), (size_t)M, (cudaStream_t)stream));
-    }
+    if (splits > 1 && ws_bytes < (size_t)splits * M * N * sizeof(float))   // splits * M * N <= sm_count * G_BM * G_BN always
+        return set_err(EB_ERR_WORKSPACE, "split-K workspace too small: need %zu bytes", (size_t)splits * M * N * sizeof(float));
+    GemmParams p{C, ldc, bias, M, N, K, act, alpha, splits, (float *)ws, (__nv_bfloat16 *)C_bf16, ldcb};
     const int n_tiles = n_out_tiles * splits;
     int grid = sm_count();
     if (grid > n_tiles) grid = n_tiles;
@@ -273,21 +285,32 @@ static int gemm_bf16(const void *A_bf16, int64_t lda, bool a_mn, const void *B_b
     else EB_GEMM_LAUNCH(false, false);
 #undef EB_GEMM_LAUNCH
     EB_CUDA(cudaGetLastError());
+    if (splits > 1) {
+        int64_t g = ((int64_t)M * N + 255) / 256; const int64_t cap = (int64_t)sm_count() * 8; if (g > cap) g = cap;
+        splitk_reduce_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>((const float *)ws, splits, M, N, C, ldc);
+        EB_CUDA(cudaGetLastError());
+    }
     return EB_OK;
 }
 
+extern "C" size_t eb_gemm_workspace_bytes(void) { return (size_t)sm_count() * G_BM * G_BN * sizeof(float); }
+
 extern "C" int eb_gemm_bf16_tn(const void *A_bf16, int64_t lda, const void *B_bf16, int64_t ldb, float *C, int64_t ldc,
-                               int M, int N, int K, const float *bias, float alpha, int act, void *stream) {
-    return gemm_bf16(A_bf16, lda, false, B_bf16, ldb, false, C, ldc, M, N, K, bias, alpha, act, stream);
+                               int M, int N, int K, const float *bias, float alpha, int act, void *workspace, size_t workspace_bytes,
+                               void *stream) {
+    return gemm_bf16(A_bf16, lda, false, B_bf16, ldb, false, C, ldc, M, N, K, bias, alpha, act, workspace, workspace_bytes, stream);
 }
 
 extern "C" int eb_gemm_bf16(const void *A_bf16, int64_t lda, int a_rows_are_k, const void *B_bf16, int64_t ldb, int b_rows_are_k,
-                            float *C, int64_t ldc, int M, int N, int K, const float *bias, float alpha, int act, void *stream) {
-    return gemm_bf16(A_bf16, lda, a_rows_are_k != 0, B_bf16, ldb, b_rows_are_k != 0, C, ldc, M, N, K, bias, alpha, act, stream);
+                            float *C, int64_t ldc, int M, int N, int K, const float *bias, float alpha, int act, void *workspace,
+                            size_t workspace_bytes, void *stream) {
+    return gemm_bf16(A_bf16, lda, a_rows_are_k != 0, B_bf16, ldb, b_rows_are_k != 0, C, ldc, M, N, K, bias, alpha, act, workspace,
+                     workspace_bytes, stream);
 }
 
 extern "C" int eb_gemm_bf16_out(const void *A_bf16, int64_t lda, int a_rows_are_k, const void *B_bf16, int64_t ldb, int b_rows_are_k,
                                 float *C, int64_t ldc, void *C_bf16, int64_t ldcb, int M, int N, int K, const float *bias, float alpha,
                                 int act, void *stream) {
-    return gemm_bf16(A_bf16, lda, a_rows_are_k != 0, B_bf16, ldb, b_rows_are_k != 0, C, ldc, M, N, K, bias, alpha, act, stream, C_bf16, ldcb);
+    return gemm_bf16(A_bf16, lda, a_rows_are_k != 0, B_bf16, ldb, b_rows_are_k != 0, C, ldc, M, N, K, bias, alpha, act, nullptr, 0, stream,
+                     C_bf16, ldcb);
 }

@@ -75,6 +75,7 @@ __global__ void __launch_bounds__(256) vae_embed_bwd_kernel(float *__restrict__ 
     }
 }
 
+// counter = (step, element): distinct (step, e) never share a draw, whatever B is from step to step (e < B L < 2^32)
 __device__ __forceinline__ float philox_normal(uint64_t seed, uint64_t ctr, uint32_t sub) {
     uint32_t r[4];
     Philox::gen(seed, ctr, sub, r);
@@ -91,7 +92,7 @@ __global__ void __launch_bounds__(256) vae_reparam_fwd_kernel(const float *__res
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
         const int b = (int)(e / L), l = (int)(e - (int64_t)b * L);
         const float mu = ml[(int64_t)b * ldml + l], lv = ml[(int64_t)b * ldml + L + l];
-        const float eps = philox_normal(seed, step * (uint64_t)n + (uint64_t)e, 0u);
+        const float eps = philox_normal(seed, step, (uint32_t)e);
         z[(int64_t)b * ldz + l] = mu + __expf(0.5f * lv) * eps;
         acc += lv - mu * mu - __expf(lv) + 1.f;
     }
@@ -109,7 +110,7 @@ __global__ void __launch_bounds__(256) vae_reparam_bwd_kernel(const float *__res
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
         const int b = (int)(e / L), l = (int)(e - (int64_t)b * L);
         const float mu = ml[(int64_t)b * ldml + l], lv = ml[(int64_t)b * ldml + L + l];
-        const float eps = philox_normal(seed, step * (uint64_t)n + (uint64_t)e, 0u);
+        const float eps = philox_normal(seed, step, (uint32_t)e);
         const float g = dz[(int64_t)b * lddz + l];
         dml[(int64_t)b * lddml + l] = g + c * mu;
         dml[(int64_t)b * lddml + L + l] = g * 0.5f * __expf(0.5f * lv) * eps + c * 0.5f * (__expf(lv) - 1.f);
@@ -336,6 +337,7 @@ extern "C" int eb_vae_embed_bwd(float *dW1, int H, const int64_t *indptr, const 
 extern "C" int eb_vae_reparam_fwd(const float *ml, int64_t ldml, int B, int L, float *z, int64_t ldz, uint64_t seed, uint64_t step,
                                   double *kl_sum, void *stream) {
     EB_ARG(ml && z && B >= 1 && L >= 1, "bad argument");
+    EB_ARG((int64_t)B * L < (1ll << 32), "B * L must be below 2^32 (the noise counter's element word)");
     vae_reparam_fwd_kernel<<<grid_for((int64_t)B * L), 256, 0, (cudaStream_t)stream>>>(ml, ldml, B, L, z, ldz, seed, step, kl_sum);
     EB_CUDA(cudaGetLastError());
     return EB_OK;
@@ -344,6 +346,7 @@ extern "C" int eb_vae_reparam_fwd(const float *ml, int64_t ldml, int B, int L, f
 extern "C" int eb_vae_reparam_bwd(const float *ml, int64_t ldml, int B, int L, const float *dz, int64_t lddz, float *dml,
                                   int64_t lddml, uint64_t seed, uint64_t step, float anneal, void *stream) {
     EB_ARG(ml && dz && dml && B >= 1 && L >= 1, "bad argument");
+    EB_ARG((int64_t)B * L < (1ll << 32), "B * L must be below 2^32 (the noise counter's element word)");
     vae_reparam_bwd_kernel<<<grid_for((int64_t)B * L), 256, 0, (cudaStream_t)stream>>>(ml, ldml, B, L, dz, lddz, dml, lddml, seed,
                                                                                         step, anneal);
     EB_CUDA(cudaGetLastError());
@@ -354,7 +357,9 @@ extern "C" int eb_vae_softmax_bf16(float *logits, int64_t ld, int n_items, const
                                    const int32_t *rows, int B, double *nll_sum, float *lse_out, int write_grad, void *grad_bf16,
                                    int64_t ld_bf16, void *stream) {
     EB_ARG(logits && indptr && indices && rows && B >= 1 && n_items >= 1 && ld >= n_items, "bad argument");
-    EB_ARG(!grad_bf16 || (write_grad && ld_bf16 >= n_items && ld_bf16 % 2 == 0 && ((uintptr_t)grad_bf16 % 4) == 0), "bad bf16 gradient buffer");
+    // the bf16 copy is a GEMM operand: 16-byte rows on both paths (the unstaged one converts through eb_convert_bf16)
+    EB_ARG(!grad_bf16 || (write_grad && ld_bf16 >= n_items && ld_bf16 % 8 == 0 && ((uintptr_t)grad_bf16 % 16) == 0),
+           "bad bf16 gradient buffer (ld_bf16 must be a multiple of 8 covering the row, 16-byte aligned)");
     const size_t smem = (size_t)n_items * sizeof(float);
     const bool staged = smem <= 200 * 1024 && ld % 4 == 0 && ((uintptr_t)logits % 16) == 0;
     if (staged) {

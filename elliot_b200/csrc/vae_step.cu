@@ -20,7 +20,8 @@ inline int64_t pad4(int64_t x) { return (x + 3) / 4 * 4; }
 struct VaeWs {
     float *h1, *ml, *z, *h2, *logits, *dh2, *dpre2, *dz, *dml, *dh1, *dpre1;
     void *h1b, *zb, *h2b, *dlb, *dpre2b, *dmlb;
-    size_t total;
+    void *gws;                                 // split-K workspace of the GEMMs (one at a time)
+    size_t gws_bytes, total;
 };
 
 VaeWs carve(char *base, int64_t I, int64_t H, int64_t L, int64_t B) {
@@ -32,6 +33,8 @@ VaeWs carve(char *base, int64_t I, int64_t H, int64_t L, int64_t B) {
     w.dh2 = f32(B * H); w.dpre2 = f32(B * H); w.dz = f32(B * L); w.dml = f32(B * 2 * L); w.dh1 = f32(B * H); w.dpre1 = f32(B * H);
     w.h1b = b16(B * pad8(H)); w.zb = b16(B * pad8(L)); w.h2b = b16(B * pad8(H));
     w.dlb = b16(B * pad8(I)); w.dpre2b = b16(B * pad8(H)); w.dmlb = b16(B * pad8(2 * L));
+    w.gws_bytes = eb_gemm_workspace_bytes();
+    w.gws = (void *)(base + off); off += up256(w.gws_bytes);
     w.total = off;
     return w;
 }
@@ -65,29 +68,29 @@ extern "C" int eb_vae_train_step(const eb_vae_model *m, const int32_t *rows, int
         // ---- forward (multi_vae_model.py:56-64, 80-83)
         EB_TRY(eb_vae_embed_fwd(m->W1, m->b1, (int)H, m->indptr, m->indices, rows, B, w.h1, H, drop_rate, drop_seed, stream));
         EB_TRY(eb_convert_bf16(w.h1, B, (int)H, H, w.h1b, H8, 0, stream));
-        EB_TRY(eb_gemm_bf16_tn(w.h1b, H8, m->W2b, H8, w.ml, LL, B, (int)LL, (int)H, m->b2, 1.f, 0, stream));
+        EB_TRY(eb_gemm_bf16_tn(w.h1b, H8, m->W2b, H8, w.ml, LL, B, (int)LL, (int)H, m->b2, 1.f, 0, w.gws, w.gws_bytes, stream));
         EB_TRY(eb_vae_reparam_fwd(w.ml, LL, B, (int)L, w.z, L, noise_seed, step, acc + 0, stream));
         EB_TRY(eb_convert_bf16(w.z, B, (int)L, L, w.zb, L8, 0, stream));
-        EB_TRY(eb_gemm_bf16_tn(w.zb, L8, m->W3b, L8, w.h2, H, B, (int)H, (int)L, m->b3, 1.f, 1, stream));
+        EB_TRY(eb_gemm_bf16_tn(w.zb, L8, m->W3b, L8, w.h2, H, B, (int)H, (int)L, m->b3, 1.f, 1, w.gws, w.gws_bytes, stream));
         EB_TRY(eb_convert_bf16(w.h2, B, (int)H, H, w.h2b, H8, 0, stream));
-        EB_TRY(eb_gemm_bf16_tn(w.h2b, H8, m->W4b, H8, w.logits, I, B, (int)I, (int)H, m->b4, 1.f, 0, stream));
+        EB_TRY(eb_gemm_bf16_tn(w.h2b, H8, m->W4b, H8, w.logits, I, B, (int)I, (int)H, m->b4, 1.f, 0, w.gws, w.gws_bytes, stream));
         // ---- loss + backward (multi_vae_model.py:114-142); dlogits overwrite the logits.  Every backward GEMM reads the row-major
         // bf16 copies as they lie: "rows are K" operands (eb_gemm_bf16) instead of transposed copies — dW = dY^T . X contracts over
         // the batch rows of both operands, dX = dY . W takes the [out][in] weight as a [K][N] matrix.
         EB_TRY(eb_vae_softmax_bf16(w.logits, I, (int)I, m->indptr, m->indices, rows, B, acc + 1, nullptr, 1, w.dlb, I8, stream));
-        EB_TRY(eb_gemm_bf16(w.dlb, I8, 1, w.h2b, H8, 1, m->gW4, H, (int)I, (int)H, B, nullptr, 1.f, 0, stream));
+        EB_TRY(eb_gemm_bf16(w.dlb, I8, 1, w.h2b, H8, 1, m->gW4, H, (int)I, (int)H, B, nullptr, 1.f, 0, w.gws, w.gws_bytes, stream));
         EB_TRY(eb_colsum(w.logits, B, (int)I, I, m->gb4, stream));
-        EB_TRY(eb_gemm_bf16(w.dlb, I8, 0, m->W4b, H8, 1, w.dh2, H, B, (int)H, (int)I, nullptr, 1.f, 0, stream));
+        EB_TRY(eb_gemm_bf16(w.dlb, I8, 0, m->W4b, H8, 1, w.dh2, H, B, (int)H, (int)I, nullptr, 1.f, 0, w.gws, w.gws_bytes, stream));
         EB_TRY(eb_tanh_bwd(w.dh2, w.h2, w.dpre2, B * H, stream));
         EB_TRY(eb_convert_bf16(w.dpre2, B, (int)H, H, w.dpre2b, H8, 0, stream));
-        EB_TRY(eb_gemm_bf16(w.dpre2b, H8, 1, w.zb, L8, 1, m->gW3, L, (int)H, (int)L, B, nullptr, 1.f, 0, stream));
+        EB_TRY(eb_gemm_bf16(w.dpre2b, H8, 1, w.zb, L8, 1, m->gW3, L, (int)H, (int)L, B, nullptr, 1.f, 0, w.gws, w.gws_bytes, stream));
         EB_TRY(eb_colsum(w.dpre2, B, (int)H, H, m->gb3, stream));
-        EB_TRY(eb_gemm_bf16(w.dpre2b, H8, 0, m->W3b, L8, 1, w.dz, L, B, (int)L, (int)H, nullptr, 1.f, 0, stream));
+        EB_TRY(eb_gemm_bf16(w.dpre2b, H8, 0, m->W3b, L8, 1, w.dz, L, B, (int)L, (int)H, nullptr, 1.f, 0, w.gws, w.gws_bytes, stream));
         EB_TRY(eb_vae_reparam_bwd(w.ml, LL, B, (int)L, w.dz, L, w.dml, LL, noise_seed, step, anneal, stream));
         EB_TRY(eb_convert_bf16(w.dml, B, (int)LL, LL, w.dmlb, LL8, 0, stream));
-        EB_TRY(eb_gemm_bf16(w.dmlb, LL8, 1, w.h1b, H8, 1, m->gW2, H, (int)LL, (int)H, B, nullptr, 1.f, 0, stream));
+        EB_TRY(eb_gemm_bf16(w.dmlb, LL8, 1, w.h1b, H8, 1, m->gW2, H, (int)LL, (int)H, B, nullptr, 1.f, 0, w.gws, w.gws_bytes, stream));
         EB_TRY(eb_colsum(w.dml, B, (int)LL, LL, m->gb2, stream));
-        EB_TRY(eb_gemm_bf16(w.dmlb, LL8, 0, m->W2b, H8, 1, w.dh1, H, B, (int)H, (int)LL, nullptr, 1.f, 0, stream));
+        EB_TRY(eb_gemm_bf16(w.dmlb, LL8, 0, m->W2b, H8, 1, w.dh1, H, B, (int)H, (int)LL, nullptr, 1.f, 0, w.gws, w.gws_bytes, stream));
         EB_TRY(eb_tanh_bwd(w.dh1, w.h1, w.dpre1, B * H, stream));
         EB_TRY(eb_colsum(w.dpre1, B, (int)H, H, m->gb1, stream));
         EB_TRY(eb_vae_embed_bwd(m->gW1, (int)H, m->indptr, m->indices, rows, B, w.dpre1, H, drop_rate, drop_seed, stream));

@@ -5,7 +5,7 @@ CUDA device — there is no CPU path.
 Streams: every op launches on torch's CURRENT stream of the tensors' device.  The C ABI never allocates, so these ops
 keep grow-only scratch per device from call to call (_scratch): bpr_exact_f64, MtSampler.step, score_topk,
 score_topk_tc, bpr_step_sampled_f32 (the schedule prefetch keeps two schedule slots of its own), gram_f64, eval_topk,
-eval_topk_metrics, eval_fairness, vae_train_step and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
+eval_topk_metrics, eval_fairness, vae_train_step, gemm_bf16_tn / gemm_bf16 (split-K partials) and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
 device.  Those ops must not run concurrently on two streams of the same device from one process.
 """
 import ctypes
@@ -471,6 +471,11 @@ def to_bf16(src, transpose=False, out=None):
     return out
 
 
+def _gemm_ws(device):
+    """The split-K workspace of the tensor-core GEMMs on `device` (partial tiles summed in a fixed order)."""
+    return _scratch("gemm_splitk", lib().eb_gemm_workspace_bytes(), device)
+
+
 def gemm_bf16_tn(A, B, M, N, K, bias=None, alpha=1.0, act=0, out=None, out_bf16=False):
     """C[M][N] fp32 = act(alpha * A[M][:K] @ B[N][:K]^T + bias) on the tensor cores (A, B bf16, K-major).
     out_bf16=True: returns (C, C_bf16) — the bf16 operand copy of C written by the epilogue itself (no conversion pass)."""
@@ -490,8 +495,9 @@ def gemm_bf16_tn(A, B, M, N, K, bias=None, alpha=1.0, act=0, out=None, out_bf16=
     assert A.dtype == torch.bfloat16 and B.dtype == torch.bfloat16
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=A.device)
+    ws = _gemm_ws(A.device)
     _call("eb_gemm_bf16_tn", A, _ptr(A), A.stride(0), _ptr(B), B.stride(0), _ptr(out), out.stride(0), M, N, K, _ptr(bias), alpha,
-          act)
+          act, _ptr(ws), ws.numel())
     return out
 
 
@@ -504,8 +510,9 @@ def gemm_bf16(A, B, M, N, K, a_rows_are_k=False, b_rows_are_k=False, bias=None, 
     assert A.dtype == torch.bfloat16 and B.dtype == torch.bfloat16
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=A.device)
+    ws = _gemm_ws(A.device)
     _call("eb_gemm_bf16", A, _ptr(A), A.stride(0), 1 if a_rows_are_k else 0, _ptr(B), B.stride(0), 1 if b_rows_are_k else 0,
-          _ptr(out), out.stride(0), M, N, K, _ptr(bias), alpha, act)
+          _ptr(out), out.stride(0), M, N, K, _ptr(bias), alpha, act, _ptr(ws), ws.numel())
     return out
 
 
@@ -572,10 +579,13 @@ def vae_reparam_bwd(ml, L, dz, dml, seed, step, anneal):
           seed, step, anneal)
 
 
-def vae_softmax(logits, indptr, indices, rows, nll_sum=None, lse_out=None, write_grad=True):
-    _need_cuda(logits, indptr, indices, rows, nll_sum, lse_out)
-    _call("eb_vae_softmax", logits, _ptr(logits), logits.stride(0), logits.shape[1], _ptr(indptr), _ptr(indices), _ptr(rows),
-          logits.shape[0], _ptr(nll_sum), _ptr(lse_out), 1 if write_grad else 0)
+def vae_softmax(logits, indptr, indices, rows, nll_sum=None, lse_out=None, write_grad=True, grad_bf16=None):
+    """grad_bf16: optional bf16 [B][ld] (ld a multiple of 8) that also receives the gradient, padding columns zeroed."""
+    _need_cuda(logits, indptr, indices, rows, nll_sum, lse_out, grad_bf16)
+    assert grad_bf16 is None or (grad_bf16.dtype == torch.bfloat16 and grad_bf16.stride(1) == 1)
+    _call("eb_vae_softmax_bf16", logits, _ptr(logits), logits.stride(0), logits.shape[1], _ptr(indptr), _ptr(indices), _ptr(rows),
+          logits.shape[0], _ptr(nll_sum), _ptr(lse_out), 1 if write_grad else 0, _ptr(grad_bf16),
+          grad_bf16.stride(0) if grad_bf16 is not None else 0)
 
 
 def tanh_bwd(dout, out, dpre=None):

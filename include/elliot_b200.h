@@ -245,14 +245,17 @@ int eb_vae_embed_fwd(const float *W1, const float *b1, int H, const int64_t *ind
                      const int32_t *rows, int B, float *h1, int64_t ldh, float drop_rate, uint64_t seed, void *stream);
 int eb_vae_embed_bwd(float *dW1, int H, const int64_t *indptr, const int32_t *indices, const int32_t *rows, int B,
                      const float *dpre1, int64_t ldd, float drop_rate, uint64_t seed, void *stream);
+/* eps of element e = b L + l at step `step` is the Philox draw (key seed, counter (step, e)): no two steps share a draw
+ * whatever their batch sizes; B L < 2^32 */
 int eb_vae_reparam_fwd(const float *ml, int64_t ldml, int B, int L, float *z, int64_t ldz, uint64_t seed, uint64_t step,
                        double *kl_sum, void *stream);
 int eb_vae_reparam_bwd(const float *ml, int64_t ldml, int B, int L, const float *dz, int64_t lddz, float *dml,
                        int64_t lddml, uint64_t seed, uint64_t step, float anneal, void *stream);
 int eb_vae_softmax(float *logits, int64_t ld, int n_items, const int64_t *indptr, const int32_t *indices,
                    const int32_t *rows, int B, double *nll_sum, float *lse_out, int write_grad, void *stream);
-/* the same, additionally writing the gradient as bf16 rows (row stride ld_bf16 >= n_items, padding columns zeroed): the operand
- * copy the backward GEMMs read.  Rows up to 200 KB are staged in shared memory (one pass over the B x I block). */
+/* the same, additionally writing the gradient as bf16 rows (row stride ld_bf16 >= n_items and a multiple of 8, grad_bf16
+ * 16-byte aligned, padding columns zeroed): the operand copy the backward GEMMs read.  Rows up to 200 KB are staged in shared
+ * memory (one pass over the B x I block). */
 int eb_vae_softmax_bf16(float *logits, int64_t ld, int n_items, const int64_t *indptr, const int32_t *indices,
                         const int32_t *rows, int B, double *nll_sum, float *lse_out, int write_grad, void *grad_bf16,
                         int64_t ld_bf16, void *stream);
@@ -441,13 +444,19 @@ int eb_partition_streams_create(int reserve_sms, int n_streams, void **streams, 
  * ------------------------------------------------------------------------ */
 int eb_convert_bf16(const float *src, int rows, int cols, int64_t ld, void *dst_bf16, int64_t dst_ld, int transpose,
                     void *stream);
+/* workspace (may be NULL): eb_gemm_workspace_bytes() bytes that let a GEMM with few output tiles and a long K (no bias, no
+ * activation) split K over the idle SMs; the partial tiles are summed in a fixed order, so the result is the same bits on
+ * every run.  Without it the GEMM runs single-pass.  One GEMM at a time may use a workspace. */
+size_t eb_gemm_workspace_bytes(void);
 int eb_gemm_bf16_tn(const void *A_bf16, int64_t lda, const void *B_bf16, int64_t ldb, float *C, int64_t ldc,
-                    int M, int N, int K, const float *bias, float alpha, int act, void *stream);
+                    int M, int N, int K, const float *bias, float alpha, int act, void *workspace, size_t workspace_bytes,
+                    void *stream);
 /* The same contraction with either operand given "rows are K": a_rows_are_k != 0 means A is a [K][M] row-major matrix
  * (M contiguous, lda >= M), likewise B as [K][N].  The tensor cores read such tiles directly (MN-major shared-memory
  * descriptors), so the backward GEMMs dW = dY^T . X (K = batch) and dX = dY . W with W kept [K][N] need no transposed copies. */
 int eb_gemm_bf16(const void *A_bf16, int64_t lda, int a_rows_are_k, const void *B_bf16, int64_t ldb, int b_rows_are_k,
-                 float *C, int64_t ldc, int M, int N, int K, const float *bias, float alpha, int act, void *stream);
+                 float *C, int64_t ldc, int M, int N, int K, const float *bias, float alpha, int act, void *workspace,
+                 size_t workspace_bytes, void *stream);
 /* ... and with a second output: C_bf16 (row stride ldcb >= N) receives the same values as bf16 — the next layer's operand copy,
  * written from the epilogue's registers instead of by a conversion pass (not combined with split-K). */
 int eb_gemm_bf16_out(const void *A_bf16, int64_t lda, int a_rows_are_k, const void *B_bf16, int64_t ldb, int b_rows_are_k,

@@ -70,16 +70,24 @@ def glorot_uniform(rng, shape):
 
 
 # ---------------------------------------------------------------- MultiVAE (parity unpinned)
-def multivae_forward_backward(P, X, eps, anneal):
+def _dropout_input(X, keep, rate):
+    """l2_normalize (multi_vae_model.py:42) then Keras Dropout (:43): kept entries scaled by 1/(1-rate), `keep` the 0/1 mask
+    (None: no dropout)."""
+    nrm = np.sqrt((X ** 2).sum(1, keepdims=True)); nrm[nrm == 0] = 1.0
+    xh = X / nrm
+    return xh if keep is None else xh * keep / (1.0 - rate)
+
+
+def multivae_forward_backward(P, X, eps, anneal, keep=None, rate=0.0):
     """VariationalAutoEncoder.call/train_step, multi_vae_model.py:114-142, for a dense binary batch X
     (B x I) and given reparametrisation noise eps (B x L).  P holds Keras-layout weights:
     W1 (I x H), b1, W2 (H x 2L: dense_mean | dense_log_var), b2, W3 (L x H), b3, W4 (H x I), b4.
+    keep (B x I, 0/1) with rate: the input dropout mask, applied after l2_normalize with the 1/(1-rate) scale.
     kernel_regularizer losses are declared but never added to the loss in the reference
     (multi_vae_model.py:47-53,75-78 vs :136) -> reg_lambda is inert, as here.
     Returns loss, grads dict, (logits, mu, lv, z)."""
     B, L = eps.shape
-    nrm = np.sqrt((X ** 2).sum(1, keepdims=True)); nrm[nrm == 0] = 1.0
-    xh = X / nrm                                                  # l2_normalize, :42
+    xh = _dropout_input(X, keep, rate)
     h1 = np.tanh(xh @ P["W1"] + P["b1"])
     ml = h1 @ P["W2"] + P["b2"]
     mu, lv = ml[:, :L], ml[:, L:]
@@ -106,12 +114,23 @@ def multivae_forward_backward(P, X, eps, anneal):
     return loss, G, (logits, mu, lv, z, neg_ll, kl)
 
 
+# Keras BinaryCrossentropy clips fp32 probabilities to [epsilon, 1 - epsilon] with epsilon = 1e-7 as fp32 constants: the
+# upper bound is 1 - 2^-23 (0.99999988), which sets the loss of a saturated sample (-log(1.19e-7), not -log(1e-7))
+CLIP_LO, CLIP_HI = float(np.float32(1e-7)), float(np.float32(1.0) - np.float32(1e-7))
+
+
+def _bce_clip(p, y):
+    """(mean-reduction numerator terms, d loss / d logit numerators) of Keras BinaryCrossentropy on probabilities p"""
+    pc = np.clip(p, CLIP_LO, CLIP_HI)
+    return -(y * np.log(pc) + (1 - y) * np.log(1 - pc)), np.where((p > CLIP_LO) & (p < CLIP_HI), p - y, 0.0)
+
+
 # ---------------------------------------------------------------- NeuMF (parity unpinned)
 def neumf_forward_backward(P, u, i, y):
     """NeuralMatrixFactorizationModel.call/train_step (neural_matrix_factorization_model.py:74-106), dropout 0,
     is_mf_train = is_mlp_train = True.  P: U_mf, I_mf, U_mlp, I_mlp (tables), W1 (2f x 4f), b1, W2 (4f x 2f), b2,
     W3 (2f x f), b3, wp (2f), bp (scalar) in Keras layout.  Keras BinaryCrossentropy: mean over the batch of
-    -(y log p + (1-y) log(1-p)) with p clipped to [1e-7, 1-1e-7]."""
+    -(y log p + (1-y) log(1-p)) with p clipped to [CLIP_LO, CLIP_HI]."""
     B = len(u)
     x0 = np.concatenate([P["U_mlp"][u], P["I_mlp"][i]], 1)
     pm = P["U_mf"][u] * P["I_mf"][i]
@@ -120,9 +139,9 @@ def neumf_forward_backward(P, u, i, y):
     feat = np.concatenate([pm, h3], 1)
     logit = feat @ P["wp"] + P["bp"]
     p = 1 / (1 + np.exp(-logit))
-    pc = np.clip(p, 1e-7, 1 - 1e-7)
-    loss = np.mean(-(y * np.log(pc) + (1 - y) * np.log(1 - pc)))
-    dl = np.where((p > 1e-7) & (p < 1 - 1e-7), p - y, 0.0) / B
+    bce, g = _bce_clip(p, y)
+    loss = np.mean(bce)
+    dl = g / B
     f = pm.shape[1]
     G = {"wp": feat.T @ dl, "bp": dl.sum()}
     dpm = dl[:, None] * P["wp"][None, :f]
@@ -141,13 +160,13 @@ def neumf_forward_backward(P, u, i, y):
 
 
 # ---------------------------------------------------------------- MultiDAE (parity unpinned)
-def multidae_forward_backward(P, X):
-    """DenoisingAutoEncoder.call/train_step (autoencoders/dae/multi_dae_model.py:20-125), dropout 0: l2-normalised rows ->
-    tanh Dense(I->H) -> tanh Dense(H->L) -> tanh Dense(L->H) -> Dense(H->I); loss = -mean_u sum_i log_softmax * x.
+def multidae_forward_backward(P, X, keep=None, rate=0.0):
+    """DenoisingAutoEncoder.call/train_step (autoencoders/dae/multi_dae_model.py:20-125): l2-normalised rows -> input
+    dropout (keep mask with rate, as multivae_forward_backward; None: dropout 0) -> tanh Dense(I->H) -> tanh Dense(H->L)
+    -> tanh Dense(L->H) -> Dense(H->I); loss = -mean_u sum_i log_softmax * x.
     P in Keras layout: W1 (I x H), b1, W2 (H x L), b2, W3 (L x H), b3, W4 (H x I), b4.  Returns loss, grads, logits."""
     B = X.shape[0]
-    nrm = np.sqrt((X ** 2).sum(1, keepdims=True)); nrm[nrm == 0] = 1.0
-    xh = X / nrm
+    xh = _dropout_input(X, keep, rate)
     h1 = np.tanh(xh @ P["W1"] + P["b1"])
     zm = np.tanh(h1 @ P["W2"] + P["b2"])
     h2 = np.tanh(zm @ P["W3"] + P["b3"])
@@ -170,13 +189,13 @@ def multidae_forward_backward(P, X):
 def gmf_forward_backward(P, u, i, y):
     """GeneralizedMatrixFactorizationModel.call/train_step (generalized_matrix_factorization_model.py:56-75),
     is_edge_weight_train = True: p = sigmoid((U[u]*I[i]) @ h), Keras BinaryCrossentropy (batch mean, p clipped to
-    [1e-7, 1-1e-7]).  P: U, I (tables), h (f).  Returns loss, grads, p."""
+    [CLIP_LO, CLIP_HI]).  P: U, I (tables), h (f).  Returns loss, grads, p."""
     B = len(u)
     pm = P["U"][u] * P["I"][i]
     p = 1 / (1 + np.exp(-(pm @ P["h"])))
-    pc = np.clip(p, 1e-7, 1 - 1e-7)
-    loss = np.mean(-(y * np.log(pc) + (1 - y) * np.log(1 - pc)))
-    dl = np.where((p > 1e-7) & (p < 1 - 1e-7), p - y, 0.0) / B
+    bce, g = _bce_clip(p, y)
+    loss = np.mean(bce)
+    dl = g / B
     G = {"h": pm.T @ dl, "U": np.zeros_like(P["U"]), "I": np.zeros_like(P["I"])}
     dpm = dl[:, None] * P["h"][None, :]
     np.add.at(G["U"], u, dpm * P["I"][i]); np.add.at(G["I"], i, dpm * P["U"][u])

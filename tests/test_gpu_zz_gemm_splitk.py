@@ -1,5 +1,5 @@
-"""Split-K path of the wgmma GEMM (no bias / activation, few output tiles, long K: partial tiles are added into a
-zeroed C with vector atomics) vs a bf16-rounded fp64 matmul.  The path is also exercised through the MultiVAE tests
+"""Split-K path of the wgmma GEMM (no bias / activation, few output tiles, long K: partial tiles are stored in a
+workspace and summed in split order) vs a bf16-rounded fp64 matmul.  The path is also exercised through the MultiVAE tests
 (dh2 = dlogits . W4); this file sorts last on purpose."""
 import pytest
 import torch
@@ -21,7 +21,7 @@ def test_split_k_matches_bf16_matmul(M, N, K):
 
 
 def test_split_k_respects_row_stride_padding():
-    """C with ldc > N: the zero-fill and the atomics must stay inside the N columns."""
+    """C with ldc > N: the split-K sums must stay inside the N columns."""
     M, N, K, pad = 100, 200, 4096, 12
     g = torch.Generator(device=DEV); g.manual_seed(3)
     A = torch.randn(M, K, device=DEV, generator=g) / K ** 0.5

@@ -29,17 +29,36 @@ def test_bprmf_batch_gradients_match_autograd():
         assert np.abs(a - b.numpy()).max() < 1e-12
 
 
+def _dropout_mask(rs, shape, rate):
+    """(keep mask, rate) of Keras Dropout at `rate`, or (None, 0) for no dropout."""
+    return (None, 0.0) if rate == 0 else ((rs.rand(*shape) >= rate).astype(np.float64), rate)
+
+
+def _dropped(xh, keep, rate):
+    return xh if keep is None else xh * torch.tensor(keep) / (1.0 - rate)
+
+
 def test_multivae_gradients_match_autograd():
+    _check_multivae(0.0)
+
+
+def test_multivae_dropout_gradients_match_autograd():
+    """The same with the input dropout of dropout_pkeep = 0.5 (a fixed keep mask, Keras 1/(1-rate) scale)."""
+    _check_multivae(0.5)
+
+
+def _check_multivae(rate):
     rs = np.random.RandomState(1)
     B, I, H, L = 12, 50, 16, 8
     P = {"W1": rs.normal(0, 0.2, (I, H)), "b1": rs.normal(0, 0.05, H), "W2": rs.normal(0, 0.2, (H, 2 * L)), "b2": rs.normal(0, 0.05, 2 * L),
          "W3": rs.normal(0, 0.2, (L, H)), "b3": rs.normal(0, 0.05, H), "W4": rs.normal(0, 0.2, (H, I)), "b4": rs.normal(0, 0.05, I)}
     X = (rs.rand(B, I) < 0.2).astype(np.float64); X[0] = 0; X[0, 3] = 1
     eps = rs.normal(size=(B, L)); anneal = 0.17
-    loss, G, _ = tfm.multivae_forward_backward(P, X, eps, anneal)
+    keep, rate = _dropout_mask(rs, (B, I), rate)
+    loss, G, _ = tfm.multivae_forward_backward(P, X, eps, anneal, keep=keep, rate=rate)
     tp = {k: T(v) for k, v in P.items()}
     tx, te = torch.tensor(X), torch.tensor(eps)
-    xh = torch.nn.functional.normalize(tx, p=2, dim=1)                               # tf.nn.l2_normalize
+    xh = _dropped(torch.nn.functional.normalize(tx, p=2, dim=1), keep, rate)       # tf.nn.l2_normalize, then Dropout
     h1 = torch.tanh(xh @ tp["W1"] + tp["b1"])
     ml = h1 @ tp["W2"] + tp["b2"]
     mu, lv = ml[:, :L], ml[:, L:]
@@ -78,15 +97,24 @@ def test_neumf_gradients_match_autograd():
 
 
 def test_multidae_gradients_match_autograd():
+    _check_multidae(0.0)
+
+
+def test_multidae_dropout_gradients_match_autograd():
+    _check_multidae(0.2)
+
+
+def _check_multidae(rate):
     rs = np.random.RandomState(3)
     B, I, H, L = 10, 40, 16, 8
     P = {"W1": rs.normal(0, 0.2, (I, H)), "b1": rs.normal(0, 0.05, H), "W2": rs.normal(0, 0.2, (H, L)), "b2": rs.normal(0, 0.05, L),
          "W3": rs.normal(0, 0.2, (L, H)), "b3": rs.normal(0, 0.05, H), "W4": rs.normal(0, 0.2, (H, I)), "b4": rs.normal(0, 0.05, I)}
     X = (rs.rand(B, I) < 0.2).astype(np.float64); X[0] = 0; X[0, 3] = 1
-    loss, G, _ = tfm.multidae_forward_backward(P, X)
+    keep, rate = _dropout_mask(rs, (B, I), rate)
+    loss, G, _ = tfm.multidae_forward_backward(P, X, keep=keep, rate=rate)
     tp = {k: T(v) for k, v in P.items()}
     tx = torch.tensor(X)
-    xh = torch.nn.functional.normalize(tx, p=2, dim=1)
+    xh = _dropped(torch.nn.functional.normalize(tx, p=2, dim=1), keep, rate)
     h = torch.tanh(xh @ tp["W1"] + tp["b1"]); h = torch.tanh(h @ tp["W2"] + tp["b2"]); h = torch.tanh(h @ tp["W3"] + tp["b3"])
     tl = -torch.mean((torch.log_softmax(h @ tp["W4"] + tp["b4"], 1) * tx).sum(1))
     tl.backward()
