@@ -1,5 +1,5 @@
 // bpr_sample.cu — the samplers on their own: membership signatures for the sampler's rejection test, BPR triples and
-// pointwise samples drawn from the Philox stream of bpr_sampler.cuh (the same triples the fused steps draw).
+// pointwise and rated samples drawn from the Philox stream of bpr_sampler.cuh (the same triples the fused steps draw).
 #include "bpr_sampler.cuh"
 
 namespace eb {
@@ -53,6 +53,22 @@ __global__ void __launch_bounds__(256) pointwise_sample_kernel(const SamplerPara
     }
 }
 
+// custom_pointwise_sparse_sampler.py:24-39: u uniform, i uniform over u's train items, label = u's train rating of i.  The
+// user and item are the BPR sampler's draws; `ratings` is aligned with the sorted train CSR.
+__global__ void __launch_bounds__(256) rated_sample_kernel(const SamplerParams p, const float *__restrict__ ratings, int64_t n,
+                                                           int32_t *out_u, int32_t *out_i, float *__restrict__ out_r) {
+    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; t < n; t += stride) {
+        uint32_t r[4];
+        int u, len;
+        int64_t beg;
+        sample_user(p, t, r, u, beg, len);
+        const int64_t e = beg + bounded(r[1], (uint32_t)len);
+        out_u[t] = u; out_i[t] = __ldg(p.indices + e); out_r[t] = __ldg(ratings + e);
+    }
+}
+
 }  // namespace eb
 
 using namespace eb;
@@ -89,6 +105,18 @@ extern "C" int eb_pointwise_sample_philox(int32_t n_users, int32_t n_items, cons
     EB_ARG(n >= 0 && out_u && out_i && out_label, "n < 0 or null output");
     if (n == 0) return EB_OK;
     pointwise_sample_kernel<<<capped_grid(n), 256, 0, (cudaStream_t)stream>>>(p, n, out_u, out_i, out_label);
+    EB_CUDA(cudaGetLastError());
+    return EB_OK;
+}
+
+extern "C" int eb_rated_sample_philox(int32_t n_users, int32_t n_items, const int64_t *csr_indptr, const int32_t *csr_indices,
+                                      const float *csr_ratings, int64_t n, uint64_t seed, uint64_t first, int32_t *out_u,
+                                      int32_t *out_i, float *out_rating, void *stream) {
+    SamplerParams p;
+    if (int rc = sampler_params(p, n_users, n_items, csr_indptr, csr_indices, nullptr, 0, seed, first)) return rc;
+    EB_ARG(csr_ratings && n >= 0 && out_u && out_i && out_rating, "n < 0 or null ratings / output");
+    if (n == 0) return EB_OK;
+    rated_sample_kernel<<<capped_grid(n), 256, 0, (cudaStream_t)stream>>>(p, csr_ratings, n, out_u, out_i, out_rating);
     EB_CUDA(cudaGetLastError());
     return EB_OK;
 }

@@ -217,6 +217,24 @@ def train_csr_of(data, device, set_order=True):
 def eval_csr_of(data, which="test"):
     """Host CSR (indptr, private item ids, gains) of the relevant items per private user (evaluator.py:117-147,
     relevance.py:80-82); None when the split does not exist."""
+    rel = _relevant_rows(data, which)
+    if rel is None:
+        return None
+    indptr, idx, r = rel
+    thr = data.config.evaluation.relevance_threshold
+    return indptr, idx, (2.0 ** (r - thr + 1) - 1).astype(np.float64)
+
+
+def eval_ratings_of(data, which="test"):
+    """The test rating (float64) of every entry of eval_csr_of(data, which), in its order; None when the split does not
+    exist."""
+    rel = _relevant_rows(data, which)
+    return None if rel is None else rel[2]
+
+
+def _relevant_rows(data, which):
+    """(indptr over private users, private item ids or -1, float64 ratings) of the split's rows rated at least the
+    relevance threshold, grouped by user; None when the split does not exist."""
     thr = data.config.evaluation.relevance_threshold
     if hasattr(data, "eval_arrays"):                                  # the mirror: no dicts, no per-user Python
         arr = data.eval_arrays(which)
@@ -227,20 +245,20 @@ def eval_csr_of(data, which="test"):
         pu, pi, r = pu[keep], pi[keep], r[keep]
         indptr = np.zeros(len(data.users) + 1, np.int64)
         np.cumsum(np.bincount(pu, minlength=len(data.users)), out=indptr[1:])
-        return indptr, pi.astype(np.int64), (2.0 ** (r.astype(np.float64) - thr + 1) - 1).astype(np.float64)
+        return indptr, pi.astype(np.int64), r.astype(np.float64)
     d = data.test_dict if which == "test" else getattr(data, "val_dict", None)
     if d is None:
         return None
     n_users = len(data.users)
     indptr = np.zeros(n_users + 1, np.int64)
-    idx, gain = [], []
+    idx, rating = [], []
     for pu, u in enumerate(data.users):
         for it, score in d.get(u, {}).items():
             if score >= thr:
                 idx.append(data.public_items.get(it, -1))            # test-only items can never be recommended
-                gain.append(2 ** (score - thr + 1) - 1)              # relevance.py:80-82
+                rating.append(score)
         indptr[pu + 1] = len(idx)
-    return indptr, np.array(idx, np.int64), np.array(gain, np.float64)
+    return indptr, np.array(idx, np.int64), np.array(rating, np.float64)
 
 
 def eval_users_of(data, which="test"):

@@ -4,7 +4,10 @@ and 19 more of the reference's list metrics (METRICS below: ranking accuracy, no
 diversity), vectorised over (users x k) index arrays.  tests/test_host_parity.py and tests/test_metrics_host.py check
 them against numbers the reference's own Evaluator produced on the same lists (tests/golden).  AUC and GAUC rank every
 relevant item in the whole catalogue: they come from the model's rank pass (ops.score_rank, counts per user) through
-finish_auc, not from the lists, and are the same at every cutoff (tests/test_oracle_auc.py).
+finish_auc, not from the lists, and are the same at every cutoff (tests/test_oracle_auc.py).  MAE, MSE and RMSE read the
+score each user's full list gives every relevant item: they come from the model's pair pass (ops.score_pairs_f32, one
+score per relevant-item CSR entry) through finish_rating, and are the same at every cutoff too
+(tests/test_oracle_rating.py).
 
 `eval_tensors` is the device path (SURVEY.md §8f #1): the top-k index tensor written by the scoring kernels is
 scored against the test set by `eb_eval_topk_f64` (the four above) and `eb_eval_metrics_f64` (the 19 others) without
@@ -19,7 +22,7 @@ import numpy as np
 import pandas as pd
 
 from . import fairness
-from .dataset import eval_csr_of, eval_users_of
+from .dataset import eval_csr_of, eval_ratings_of, eval_users_of
 
 SUPPORTED = {"ndcg": "nDCG", "hr": "HR", "precision": "Precision", "recall": "Recall"}
 # result keys are the reference's name() values; each kernel runs only when one of its metrics is asked for
@@ -30,10 +33,16 @@ _EXTENDED = {m.lower(): m for m in METRICS}
 # the top-k lists, and the same at every cutoff; available to an evaluator built with rank_pass=True
 RANK = ("AUC", "GAUC")
 _RANKED = {m.lower(): m for m in RANK}
+# metrics of the score of each relevant item in the user's full list: from the model's pair pass, not from the top-k lists,
+# and the same at every cutoff; available to an evaluator built with score_pass=True
+RATING = ("MAE", "MSE", "RMSE")
+_RATED = {m.lower(): m for m in RATING}
 _WHY_NOT = {
     **dict.fromkeys(("auc", "gauc"), "it ranks every relevant item in the whole catalogue, which takes a model's rank pass "
                                      "(build the Evaluator with rank_pass=True and give eval() its rank_counts)"),
-    **dict.fromkeys(("mae", "mse", "rmse"), "it needs the predicted scores and the test ratings, not a top-k list"),
+    **dict.fromkeys(("mae", "mse", "rmse"), "it reads the score every relevant item has in the user's full list, which "
+                                            "takes a model's pair pass (build the Evaluator with score_pass=True and give "
+                                            "eval() its pair_scores)"),
     **dict.fromkeys(("dsc", "extendedf1", "extendedepc", "extendedefd", "extendedpopreo", "extendedpoprsp"),
                     "it is a complex metric with parameters"),
     **dict.fromkeys(("srecall", "biasdisparitybr", "biasdisparitybs", "biasdisparitybd", "usermadrating", "itemmadrating",
@@ -202,6 +211,18 @@ def finish_auc(n_pos, sum_c, n_rel, n_train, n_items, names):
     return {m: out[m] for m in names}
 
 
+def finish_rating(abs_sum, sq_sum, n_rel, names):
+    """MAE, MSE and RMSE (mae.py, mse.py, rmse.py) from the pair pass's sums over every relevant item of the users with
+    test rows that is in the user's full list: sum |v - r| and sum (v - r)^2, v the list's score (-inf for a train item,
+    which the reference's full lists end with: such an item makes the sums inf).  n_rel counts every relevant item of
+    those users, test-only items included; n_rel = 0 raises ZeroDivisionError, as the reference's int / int does."""
+    if n_rel == 0:
+        raise ZeroDivisionError("MAE/MSE/RMSE: the users with test rows have no relevant item")
+    out = {"MAE": float(abs_sum) / n_rel, "MSE": float(sq_sum) / n_rel}
+    out["RMSE"] = float(np.sqrt(out["MSE"]))
+    return {m: out[m] for m in names}
+
+
 def finish_metrics(s, k, n_items, names):
     """Metric values from the slot vector: means over the users each metric averages over (0.0 when there are none,
     like the four accuracy metrics), the ratios of PopREO / PopRSP and the closed forms of Gini and SEntropy."""
@@ -240,9 +261,10 @@ def finish_metrics(s, k, n_items, names):
 
 
 class Evaluator:
-    def __init__(self, data, params, rank_pass=False):
+    def __init__(self, data, params, rank_pass=False, score_pass=False):
         """rank_pass: the caller supplies rank_counts (a model's ops.score_rank counts) to eval() / eval_tensors(), so
-        AUC and GAUC are available; without it they raise here, like every other name this evaluator cannot compute."""
+        AUC and GAUC are available; without it they raise here, like every other name this evaluator cannot compute.
+        score_pass: the same for MAE, MSE and RMSE, with pair_scores (a model's pair pass over pair_sets())."""
         self._data, self._params = data, params
         ev = data.config.evaluation
         self._k = getattr(ev, "cutoffs", [data.config.top_k])
@@ -251,7 +273,8 @@ class Evaluator:
             raise Exception("Cutoff values must be smaller than recommendation list length (top_k)")
         self._metrics = []
         for m in ev.simple_metrics:
-            name = SUPPORTED.get(m.lower()) or _EXTENDED.get(m.lower()) or (_RANKED.get(m.lower()) if rank_pass else None)
+            name = (SUPPORTED.get(m.lower()) or _EXTENDED.get(m.lower()) or (_RANKED.get(m.lower()) if rank_pass else None)
+                    or (_RATED.get(m.lower()) if score_pass else None))
             if name is None:
                 why = _WHY_NOT.get(m.lower(), "the reference does not know this name")
                 raise Exception(f"metric {m} is not available in elliot_b200's evaluator: {why} "
@@ -260,6 +283,7 @@ class Evaluator:
         self._basic = [m for m in self._metrics if m in SUPPORTED.values()]
         self._extended = [m for m in self._metrics if m in METRICS]
         self._ranked = [m for m in self._metrics if m in RANK]
+        self._rated = [m for m in self._metrics if m in RATING]
         # complex_metrics: the clustered fairness metrics, each entry checked (name, clustering files) here
         self._complex = [fairness.Entry(e) for e in (getattr(ev, "complex_metrics", None) or [])]
         self._sets = {"test": eval_csr_of(data, "test"), "val": eval_csr_of(data, "val")}
@@ -274,6 +298,12 @@ class Evaluator:
         return bool(self._ranked)
 
     @property
+    def needs_pairs(self):
+        """True when MAE, MSE or RMSE is asked for: evaluate() then runs the model's pair pass once per split
+        (pair_sets / pair_scores) besides its top-k lists."""
+        return bool(self._rated)
+
+    @property
     def needs_scores(self):
         """True when UserMADrating or ItemMADrating is asked for: eval_tensors() then needs the lists' scores (vals)."""
         return any(e.needs_scores for e in self._complex)
@@ -282,6 +312,50 @@ class Evaluator:
         """{split: (rel indptr int64, item-sorted rel items int32)} on `device` for every split that exists: the
         arguments of a model's rank pass."""
         return {w: self._device_set(w, self._k[0], device)[:2] for w in ("val", "test") if self._sets[w] is not None}
+
+    def pair_sets(self, device):
+        """{split: (rel indptr int64, item-sorted rel items int32, their test ratings float64)} on `device` for every
+        split that exists: the CSR of the rank pass, with the rating of each entry.  A model's pair pass scores each
+        entry; eval() / eval_tensors() take those scores as pair_scores."""
+        import torch
+        cache = self.__dict__.setdefault("_pair_dev_sets", {})
+        for w in ("val", "test"):
+            if self._sets[w] is not None and (w, str(device)) not in cache:
+                ds = self._device_set(w, self._k[0], device)
+                cache[(w, str(device))] = (ds[0], ds[1], torch.from_numpy(self._pair_host(w)[1]).to(device))
+        return {w: cache[(w, str(device))] for w in ("val", "test") if self._sets[w] is not None}
+
+    def _pair_host(self, which):
+        """(items, ratings) of the split's relevant entries in the order of the device CSR (item-sorted per user), cached."""
+        cache = self.__dict__.setdefault("_pair_host_cache", {})
+        if which not in cache:
+            indptr, idx, _ = self._sets[which]
+            rows = np.repeat(np.arange(len(indptr) - 1), np.diff(indptr))
+            by_item = np.lexsort((idx, rows))                                    # the order of _device_set's items
+            cache[which] = (idx[by_item], eval_ratings_of(self._data, which)[by_item])
+        return cache[which]
+
+    def _rating_values(self, which, pair_scores):
+        """MAE / MSE / RMSE of a split from the host scores of its pair pass (aligned with pair_sets()), fp64."""
+        if not self._rated:
+            return {}
+        if pair_scores is None:
+            raise Exception(f"{'/'.join(self._rated)} need the model's pair pass scores (pair_scores)")
+        items, ratings = self._pair_host(which)
+        keep = items >= 0
+        d = np.asarray(pair_scores[which], np.float64)[keep] - ratings[keep]
+        return finish_rating(np.abs(d).sum(), (d * d).sum(), len(items), self._rated)
+
+    def _rating_values_device(self, which, pair_scores, device):
+        """The same from the device scores: ops.rating_error_sums finishes the sums in fp64 on the device."""
+        if not self._rated:
+            return {}
+        if pair_scores is None:
+            raise Exception(f"{'/'.join(self._rated)} need the model's pair pass scores (pair_scores)")
+        from . import ops
+        _, items, ratings = self.pair_sets(device)[which]
+        s = ops.rating_error_sums(pair_scores[which], ratings, items).cpu().numpy()
+        return finish_rating(s[0], s[1], items.numel(), self._rated)
 
     def _rank_values(self, which, rank_counts):
         """AUC / GAUC of a split from the host (n_pos, sum_c) arrays of its rank pass (rows = private users)."""
@@ -294,9 +368,11 @@ class Evaluator:
 
     # recommendations: (val, test) pair of {public_user: [(public_item, score), ...]}
     # rank_counts: {split: (n_pos, sum_c)} host arrays of the model's rank pass, when AUC or GAUC is asked for
-    def eval(self, recommendations, rank_counts=None):
+    # pair_scores: {split: host scores aligned with pair_sets()}, the model's pair pass, when MAE, MSE or RMSE is asked for
+    def eval(self, recommendations, rank_counts=None, pair_scores=None):
         out = {}
-        ranked = {w: self._rank_values(w, rank_counts) for w in ("val", "test") if self._sets[w] is not None}
+        ranked = {w: {**self._rank_values(w, rank_counts), **self._rating_values(w, pair_scores)}
+                  for w in ("val", "test") if self._sets[w] is not None}
         for k in self._k:
             res = {}
             for slot, which in ((0, "val"), (1, "test")):
@@ -353,10 +429,10 @@ class Evaluator:
                           *(t(a, torch.float64) for a in position_tables(k)))
         return cache[key]
 
-    def eval_tensors(self, idx, users=None, rank_counts=None, vals=None):
+    def eval_tensors(self, idx, users=None, rank_counts=None, vals=None, pair_scores=None):
         """Same result structure as eval(), from a device (rows x top_k) int32 tensor of PRIVATE item ids
         (-1 = empty), row r = private user r (or users[r]); vals: the lists' scores (rows x top_k), needed by
-        UserMADrating / ItemMADrating."""
+        UserMADrating / ItemMADrating; pair_scores: {split: device scores aligned with pair_sets()}."""
         from . import ops
         if vals is None and self.needs_scores:
             raise Exception(f"{', '.join(e.metric for e in self._complex if e.needs_scores)} need the lists' scores: "
@@ -371,7 +447,8 @@ class Evaluator:
                                      scores=scores, users=users)
             return c.cpu().numpy(), s.cpu().numpy()
         out = {}
-        ranked = {w: self._rank_values(w, rank_counts) for w in ("val", "test") if self._sets[w] is not None}
+        ranked = {w: {**self._rank_values(w, rank_counts), **self._rating_values_device(w, pair_scores, idx.device)}
+                  for w in ("val", "test") if self._sets[w] is not None}
         for k in self._k:
             res = {}
             for which in ("val", "test"):

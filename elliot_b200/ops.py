@@ -1460,3 +1460,80 @@ def sigmoid_(x):
     assert x.is_contiguous() and x.dtype == torch.float32
     _call("eb_sigmoid_inplace", x, _ptr(x), x.numel())
     return x
+
+
+# ---------------------------------------------------------------- SVD++ / FunkSVD (csrc/rating_mf.cu)
+def rated_sample_philox(n_users, n_items, indptr, indices, ratings, n, seed, first=0):
+    """(u, item, rating) samples of custom_pointwise_sparse_sampler.py:24-39 (Philox stream): u uniform, item uniform over
+    u's train row, its train rating; `ratings` float32 aligned with the sorted train CSR `indices`."""
+    _need_cuda(indptr, indices, ratings)
+    assert ratings.dtype == torch.float32 and ratings.numel() == indices.numel()
+    dev = indptr.device
+    u = torch.empty(n, dtype=torch.int32, device=dev); i = torch.empty_like(u); r = torch.empty(n, dtype=torch.float32, device=dev)
+    _call("eb_rated_sample_philox", indptr, n_users, n_items, _ptr(indptr), _ptr(indices), _ptr(ratings), n, seed, first,
+          _ptr(u), _ptr(i), _ptr(r))
+    return u, i, r
+
+
+def implicit_mean_f32(P, Y, f, indptr, indices, users=None, out=None):
+    """Z[r] = P[u] + mean over u's train row of Y (u = users[r], or r for every row of P when users is None)."""
+    _need_cuda(P, Y, indptr, indices, users, out)
+    assert P.stride(0) == Y.stride(0) and P.stride(1) == 1 and Y.stride(1) == 1
+    n = P.shape[0] if users is None else users.numel()
+    if users is not None:
+        _chk_idx(users)
+    if out is None:
+        out = torch.zeros((n, P.stride(0)), dtype=torch.float32, device=P.device)
+    assert out.shape[0] >= n and out.stride(1) == 1
+    _call("eb_implicit_mean_f32", P, _ptr(P), _ptr(Y), P.stride(0), f, _ptr(indptr), _ptr(indices), _ptr(users), n, _ptr(out),
+          out.stride(0))
+    return out
+
+
+def rating_mf_step_f32(P, Q, bu, bi, g, f, u, it, label, dP, dQ, dbu, dbi, dg, Z=None, indptr=None, indices=None, dY=None,
+                       loss=None, mean_over=None):
+    """Gradient of the batch's mean squared error of z.q + b_u + b_i (+ g) into the dense gradient tables: z = Z[s] with
+    dY over the train rows (SVD++), or P[u] (FunkSVD: Z, dY, g and dg None).  `loss` (fp64) gets the batch loss added."""
+    _need_cuda(P, Q, bu, bi, g, u, it, label, dP, dQ, dbu, dbi, dg, Z, indptr, indices, dY, loss)
+    _chk_idx(u, it)
+    assert P.stride(0) == Q.stride(0) == dP.stride(0) == dQ.stride(0)
+    if dY is not None:
+        assert dY.stride(0) == P.stride(0)
+    _call("eb_rating_mf_step_f32", P, _ptr(P), _ptr(Q), P.stride(0), f, _ptr(bu), _ptr(bi), _ptr(g), _ptr(Z),
+          0 if Z is None else Z.stride(0), _ptr(indptr), _ptr(indices), _ptr(u), _ptr(it), _ptr(label), u.numel(),
+          int(mean_over) if mean_over else max(int(u.numel()), 1), _ptr(dP), _ptr(dQ), _ptr(dY), _ptr(dbu), _ptr(dbi), _ptr(dg),
+          _ptr(loss))
+
+
+def score_pairs_f32(U, V, f, rel_indptr, rel_items, item_bias=None, user_off=None, global_off=None, mask_indptr=None,
+                    mask_indices=None):
+    """Per entry of the relevant-item CSR (rows = users 0 .. n-1 of U): (U[u].V[item] + item_bias) + (user_off[u] +
+    global_off[0]) as the user's full list carries it; -inf for an item of the user's mask row, NaN for item -1."""
+    _need_cuda(U, V, rel_indptr, rel_items, item_bias, user_off, global_off, mask_indptr, mask_indices)
+    assert U.dtype == torch.float32 and V.dtype == torch.float32 and U.stride(0) == V.stride(0)
+    assert rel_indptr.dtype == torch.int64 and rel_items.dtype == torch.int32 and rel_items.is_contiguous()
+    n_users = rel_indptr.numel() - 1
+    assert n_users <= U.shape[0]
+    out = torch.empty(rel_items.numel(), dtype=torch.float32, device=U.device)
+    _call("eb_score_pairs_f32", U, _ptr(U), _ptr(V), U.stride(0), f, _ptr(item_bias), _ptr(user_off), _ptr(global_off),
+          _ptr(rel_indptr), _ptr(_nonempty(rel_items)), n_users, _ptr(mask_indptr), _ptr(mask_indices), _ptr(out))
+    return out
+
+
+def add_row_offset_(x, row_off, scalar_off=None):
+    """x[r][:] += row_off[r] (+ scalar_off[0]) in place, for a 2-D fp32 x with unit column stride."""
+    _need_cuda(x, row_off, scalar_off)
+    assert x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1 and row_off.numel() >= x.shape[0]
+    _call("eb_add_row_offset_f32", x, _ptr(x), x.shape[0], x.shape[1], x.stride(0), _ptr(row_off), _ptr(scalar_off))
+    return x
+
+
+def rating_error_sums(scores, ratings, items):
+    """Device fp64 [sum |v - r|, sum (v - r)^2] over the entries with items >= 0 (fixed summation order)."""
+    _need_cuda(scores, ratings, items)
+    assert scores.dtype == torch.float32 and ratings.dtype == torch.float64 and items.dtype == torch.int32
+    n = scores.numel()
+    assert ratings.numel() == n and items.numel() == n
+    out = torch.empty(2, dtype=torch.float64, device=scores.device)
+    _call("eb_rating_error_sums_f64", scores, _ptr(_nonempty(scores)), _ptr(_nonempty(ratings)), _ptr(_nonempty(items)), n, _ptr(out))
+    return out

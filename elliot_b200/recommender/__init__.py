@@ -16,3 +16,4 @@ from .pure_svd import PureSVD, PureSVDModel  # noqa: F401
 from .slope_one import SlopeOne, SlopeOneModel  # noqa: F401
 from .nonneg_mf import NonNegMF, NonNegMFModel  # noqa: F401
 from .unpersonalized import MostPop, Random, MostPopLists, RandomLists  # noqa: F401
+from .rating_mf import SVDpp, FunkSVD, RatingMFModel  # noqa: F401

@@ -50,6 +50,16 @@ class RankRecs:
         return self._model.rank(rel_indptr, rel_items, self._indptr, self._sorted_idx)
 
 
+class PairScoreRecs:
+    """The MAE / MSE / RMSE pair pass of a model whose `_model.pair_scores(rel_indptr, rel_items, mask_indptr,
+    mask_indices)` scores every relevant item as the full lists its `_model.topk` takes the top k of would (ops.score_pairs_f32
+    on the same tables; -inf for a train item)."""
+
+    def get_pair_score_tensors(self, rel_indptr, rel_items):
+        """float32 device tensor, one score per entry of the relevant-item CSR."""
+        return self._model.pair_scores(rel_indptr, rel_items, self._indptr, self._sorted_idx)
+
+
 def upload(a, device, dtype):
     """A numpy array on the device as a contiguous tensor of `dtype`, in its stored order."""
     return torch.from_numpy(np.ascontiguousarray(a)).to(device, dtype)

@@ -102,15 +102,22 @@ def init_charger(init):
         random.seed(self._seed)
         self._nprandom, self._random = np.random, random
         self._num_items, self._num_users = self._data.num_items, self._data.num_users
-        from ..evaluation import RANK, Evaluator
+        from ..evaluation import RANK, RATING, Evaluator
         asked = [m for m in self._data.config.evaluation.simple_metrics if m.upper() in RANK]
         if asked and not hasattr(self, "get_rank_tensors"):
             raise Exception(f"{self.__class__.__name__} cannot evaluate {'/'.join(asked)}: these rank every relevant "
                             f"item in the whole catalogue, and only the factor models that list with score_topk have "
                             f"that rank pass; this model's scores come from a different scorer, which would need its own")
+        rated = [m for m in self._data.config.evaluation.simple_metrics if m.upper() in RATING]
+        if rated and not hasattr(self, "get_pair_score_tensors"):
+            raise Exception(f"{self.__class__.__name__} cannot evaluate {'/'.join(rated)}: these read the score every "
+                            f"relevant test item has in the user's full list, and only the rating-prediction models "
+                            f"(SVDpp, FunkSVD) have that pair pass")
         init(self, *args, **kwargs)
-        # AUC / GAUC come from this model's rank pass (checked above); other configs build the evaluator as before
-        self.evaluator = Evaluator(self._data, self._params, rank_pass=True) if asked else Evaluator(self._data, self._params)
+        # AUC / GAUC come from this model's rank pass, MAE / MSE / RMSE from its pair pass (both checked above); other
+        # configs build the evaluator as before
+        passes = {**({"rank_pass": True} if asked else {}), **({"score_pass": True} if rated else {})}
+        self.evaluator = Evaluator(self._data, self._params, **passes)
         self._params.name = self.name
         wdir = os.path.abspath(os.sep.join([self._config.path_output_rec_weight, self.name]))
         os.makedirs(wdir, exist_ok=True)

@@ -27,6 +27,12 @@ class RecMixin:
             # the lists stay top_k
             counts = {w: tuple(t.cpu().numpy() for t in self.get_rank_tensors(*rel))
                       for w, rel in self.evaluator.rank_sets(self._device).items()}
+        pairs = {}
+        if getattr(self.evaluator, "needs_pairs", False):
+            # MAE / MSE / RMSE: the score every relevant item has in the user's full list, from the model's pair pass
+            # once per split; the lists stay top_k
+            pairs = {"pair_scores": {w: self.get_pair_score_tensors(*rel[:2])
+                                     for w, rel in self.evaluator.pair_sets(self._device).items()}}
         if on_device:
             # extension: the (users x k) index tensor goes from the scoring kernel straight into the metric
             # kernel; no {user: [(item, score)]} dicts are built (recommender_utils_mixin.py:84-88 / evaluator.py:117-147)
@@ -34,10 +40,13 @@ class RecMixin:
             recs = None
             # UserMADrating / ItemMADrating read the lists' scores; no other metric does
             scores = val if getattr(self.evaluator, "needs_scores", False) else None
-            self._results.append(self.evaluator.eval_tensors(idx, rank_counts=counts, **({"vals": scores} if scores is not None else {})))
+            self._results.append(self.evaluator.eval_tensors(idx, rank_counts=counts, **({"vals": scores} if scores is not None else {}),
+                                                             **pairs))
         else:
             recs = self.get_recommendations(self.evaluator.get_needed_recommendations())
-            self._results.append(self.evaluator.eval(recs, rank_counts=counts))
+            if pairs:
+                pairs = {"pair_scores": {w: t.cpu().numpy() for w, t in pairs["pair_scores"].items()}}
+            self._results.append(self.evaluator.eval(recs, rank_counts=counts, **pairs))
         if it is not None:
             self.logger.info(f"Epoch {it + 1}/{self._epochs} loss {loss / (it + 1):.5f}")
         else:

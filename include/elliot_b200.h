@@ -799,6 +799,42 @@ int eb_nnmf_row_update_f64(const int64_t *indptr, const int32_t *cols, const int
                            double reg, void *stream);
 
 /* ------------------------------------------------------------------------
+ * SVD++ and FunkSVD (latent_factor_models/SVDpp/svdpp_model.py, FunkSVD/funk_svd_model.py) and the pair pass of the rating
+ * metrics (evaluation/metrics/rating/{mae,mse,rmse}).  fp32 tables, row stride ld (multiple of 4), f % 4 == 0, f <= 128.
+ * eb_rated_sample_philox: dataset/samplers/custom_pointwise_sparse_sampler.py:24-39 (u uniform, i uniform over u's train
+ *   row, label = the train rating), the user and item draws of eb_bpr_sample_philox_filter's stream (counter first + t);
+ *   csr_ratings [nnz] is aligned with the sorted train CSR.
+ * eb_implicit_mean_f32: Z[r] (row stride ldz) = P[u] + (1/|N(u)|) sum_{j in N(u)} Y[j], N(u) = train row of u = users[r]
+ *   (users NULL: u = r), fp32 sums of 128-bit row loads.
+ * eb_rating_mf_step_f32: per sample s, out = z.q_i + b_u + b_i + g with z = Z[s] (SVD++) or P[u] (Z NULL: FunkSVD), g NULL
+ *   for no global bias; loss += (out - y)^2 / mean_over (fp64 accumulator); the gradient e = 2 (out - y) / mean_over is
+ *   added (vector atomics) to dQ[i] (e z), dP[u] (e q_i), dbu[u], dbi[i], dg[0] and, when dY is given (with Z and the train
+ *   CSR), to dY[j] (e q_i / |N(u)|) for every j of u's train row.  The tables the dense Keras Adam then applies.
+ * eb_score_pairs_f32: for every user w < n_users and relevant entry k of its row (rel CSR, rel_items -1 outside the
+ *   catalogue): out[k] = (U[w].V[item] + item_bias[item]) + (user_off[w] + global_off[0]) (each term optional), -inf when
+ *   item is in w's mask row (sorted), NaN when item = -1.  One warp per user.
+ * eb_add_row_offset_f32: x[r][c] += row_off[r] + scalar_off[0] (scalar_off optional) for c < cols.
+ * eb_rating_error_sums_f64: out[0] = sum |scores[e] - ratings[e]|, out[1] = sum (scores[e] - ratings[e])^2 over the
+ *   entries with items[e] >= 0, in fp64, one CTA in a fixed order (the same bits every run).
+ * ------------------------------------------------------------------------ */
+int eb_rated_sample_philox(int32_t n_users, int32_t n_items, const int64_t *csr_indptr, const int32_t *csr_indices,
+                           const float *csr_ratings, int64_t n, uint64_t seed, uint64_t first, int32_t *out_u, int32_t *out_i,
+                           float *out_rating, void *stream);
+int eb_implicit_mean_f32(const float *P, const float *Y, int64_t ld, int f, const int64_t *indptr, const int32_t *indices,
+                         const int32_t *users, int64_t n, float *Z, int64_t ldz, void *stream);
+int eb_rating_mf_step_f32(const float *P, const float *Q, int64_t ld, int f, const float *bu, const float *bi, const float *g,
+                          const float *Z, int64_t ldz, const int64_t *indptr, const int32_t *indices, const int32_t *u,
+                          const int32_t *it, const float *label, int64_t n, int64_t mean_over, float *dP, float *dQ, float *dY,
+                          float *dbu, float *dbi, float *dg, double *loss, void *stream);
+int eb_score_pairs_f32(const float *U, const float *V, int64_t ld, int f, const float *item_bias, const float *user_off,
+                       const float *global_off, const int64_t *rel_indptr, const int32_t *rel_items, int32_t n_users,
+                       const int64_t *mask_indptr, const int32_t *mask_indices, float *out, void *stream);
+int eb_add_row_offset_f32(float *x, int64_t rows, int cols, int64_t ldx, const float *row_off, const float *scalar_off,
+                          void *stream);
+int eb_rating_error_sums_f64(const float *scores, const double *ratings, const int32_t *items, int64_t n, double *out,
+                             void *stream);
+
+/* ------------------------------------------------------------------------
  * MostPop and Random (recommender/unpersonalized/most_popular/most_popular.py, random_recommender/Random.py).
  * The train CSR indptr [n_users + 1] / train (each row sorted ascending) is also the mask: a user's train items are
  * never listed.  Output row q is user users[q], or user_begin + q when users is NULL.
