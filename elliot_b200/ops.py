@@ -5,7 +5,7 @@ CUDA device — there is no CPU path.
 Streams: every op launches on torch's CURRENT stream of the tensors' device.  The C ABI never allocates, so these ops
 keep grow-only scratch per device from call to call (_scratch): bpr_exact_f64, MtSampler.step, score_topk,
 score_topk_tc, bpr_step_sampled_f32 (the schedule prefetch keeps two schedule slots of its own), gram_f64, eval_topk,
-eval_topk_metrics, eval_fairness, vae_train_step, gemm_bf16_tn / gemm_bf16 (split-K partials) and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
+eval_topk_metrics, eval_fairness, vae_train_step, gemm_bf16_tn / gemm_bf16 (split-K partials), cml_grad_f32 and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
 device.  Those ops must not run concurrently on two streams of the same device from one process.
 """
 import ctypes
@@ -1537,3 +1537,35 @@ def rating_error_sums(scores, ratings, items):
     out = torch.empty(2, dtype=torch.float64, device=scores.device)
     _call("eb_rating_error_sums_f64", scores, _ptr(_nonempty(scores)), _ptr(_nonempty(ratings)), _ptr(_nonempty(items)), n, _ptr(out))
     return out
+
+
+# ---------------------------------------------------------------- CML (csrc/cml.cu)
+def cml_grad_f32(Gu, Gi, Bi, dGu, dGi, dBi, d, tu, ti, tj, l_w, l_b, margin, loss=None, terms=None):
+    """Batch gradient of the CML loss (CML_model.py:59-98, the reference's B x B broadcast, counted by sorting) into dense
+    gradient tables; `loss` (fp64) gets the batch loss added.  terms (float32, 2n): receives D then E in triple order
+    (None: device scratch)."""
+    _need_cuda(Gu, Gi, Bi, dGu, dGi, dBi, tu, ti, tj, loss, terms)
+    _chk_idx(tu, ti, tj)
+    assert Gu.stride(0) == Gi.stride(0) == dGu.stride(0) == dGi.stride(0)
+    n = tu.numel()
+    if terms is None:
+        terms = _scratch("cml_terms", 8 * n, Gu.device)
+    else:
+        assert terms.dtype == torch.float32 and terms.is_contiguous() and terms.numel() >= 2 * n
+    ws = _scratch("cml", lib().eb_cml_workspace_bytes(n), Gu.device)
+    _call("eb_cml_grad_f32", Gu, _ptr(Gu), _ptr(Gi), _ptr(Bi), _ptr(dGu), _ptr(dGi), _ptr(dBi), d, Gu.stride(0), _ptr(tu),
+          _ptr(ti), _ptr(tj), n, l_w, l_b, margin, _ptr(terms), _ptr(loss), _ptr(ws), ws.numel())
+
+
+def cml_score_operands_f32(Gu, Gi, Bi, n_users, n_items):
+    """(U2, item_off, user_off): 2 Gu, Bi - |Gi|^2 and -|Gu|^2 per row, so that the dot-product scorers on
+    (U2, Gi, item_off) plus user_off give CML's Bi - |Gu - Gi|^2 (CML_model.py:101-106)."""
+    _need_cuda(Gu, Gi, Bi)
+    assert Gu.dtype == Gi.dtype == Bi.dtype == torch.float32 and Gu.is_contiguous() and Gi.is_contiguous()
+    assert Gu.stride(0) == Gi.stride(0) and Gu.shape[0] >= n_users and Gi.shape[0] >= n_items and Bi.numel() >= n_items
+    U2 = torch.empty((n_users, Gu.shape[1]), dtype=torch.float32, device=Gu.device)
+    item_off = torch.empty(n_items, dtype=torch.float32, device=Gu.device)
+    user_off = torch.empty(n_users, dtype=torch.float32, device=Gu.device)
+    _call("eb_cml_score_operands_f32", Gu, _ptr(Gu), _ptr(Gi), _ptr(Bi), Gu.stride(0), n_users, n_items, _ptr(U2), _ptr(item_off),
+          _ptr(user_off))
+    return U2, item_off, user_off

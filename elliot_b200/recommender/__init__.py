@@ -17,3 +17,4 @@ from .slope_one import SlopeOne, SlopeOneModel  # noqa: F401
 from .nonneg_mf import NonNegMF, NonNegMFModel  # noqa: F401
 from .unpersonalized import MostPop, Random, MostPopLists, RandomLists  # noqa: F401
 from .rating_mf import SVDpp, FunkSVD, RatingMFModel  # noqa: F401
+from .cml import CML, CMLModel  # noqa: F401

@@ -835,6 +835,24 @@ int eb_rating_error_sums_f64(const float *scores, const double *ratings, const i
                              void *stream);
 
 /* ------------------------------------------------------------------------
+ * CML (latent_factor_models/CML/CML_model.py:59-106), fp32 tables Gu, Gi (row stride ld, one of 8..256), Bi.
+ * eb_cml_grad_f32 accumulates the gradient of the reference's broadcast B x B loss over n triples (see csrc/cml.cu):
+ *   L = sum_a sum_b max(m - clip(D_a + E_b, -80, 1e8), 0) + l_w (|gu_a|^2 + |gi_a|^2 + |gj_a|^2)/2 + l_b bpos^2/2
+ *       + l_b bneg^2/20,   D_a = |gu_a - gj_a|^2 - |gu_a - gi_a|^2,  E_b = Bi[pos_b] - Bi[neg_b]
+ *   into dense gradient tables (duplicates summed), counting the active pairs (-80 < D_a + E_b <= m, fp64 sum of the fp32
+ *   terms) by sorting instead of forming them.  loss (optional, device double[1]) += L.  terms [2n] receives D then E in
+ *   triple order.  -80 < margin < 1e8; n < 2^31.  workspace: eb_cml_workspace_bytes(n) bytes, else EB_ERR_WORKSPACE.
+ * eb_cml_score_operands_f32: U2 = 2 Gu (row stride ld), item_off[i] = Bi[i] - |Gi[i]|^2, user_off[u] = -|Gu[u]|^2, so
+ *   that U2[u].Gi[i] + item_off[i] + user_off[u] = Bi[i] - |Gu[u] - Gi[i]|^2, the reference's predict.
+ * ------------------------------------------------------------------------ */
+size_t eb_cml_workspace_bytes(int64_t n);
+int eb_cml_grad_f32(const float *Gu, const float *Gi, const float *Bi, float *dGu, float *dGi, float *dBi, int d, int ld,
+                    const int32_t *tu, const int32_t *ti, const int32_t *tj, int64_t n, float l_w, float l_b, float margin,
+                    float *terms, double *loss, void *workspace, size_t workspace_bytes, void *stream);
+int eb_cml_score_operands_f32(const float *Gu, const float *Gi, const float *Bi, int ld, int32_t n_users, int32_t n_items,
+                              float *U2, float *item_off, float *user_off, void *stream);
+
+/* ------------------------------------------------------------------------
  * MostPop and Random (recommender/unpersonalized/most_popular/most_popular.py, random_recommender/Random.py).
  * The train CSR indptr [n_users + 1] / train (each row sorted ascending) is also the mask: a user's train items are
  * never listed.  Output row q is user users[q], or user_begin + q when users is NULL.
