@@ -3,9 +3,9 @@ all arithmetic happens in elliot_b200/csrc/*.cu.  Every op raises if its tensors
 CUDA device — there is no CPU path.
 
 Streams: every op launches on torch's CURRENT stream of the tensors' device.  The C ABI never allocates, so these ops
-keep grow-only scratch per device from call to call (_scratch): bpr_exact_f64, MtSampler.step, score_topk,
+keep grow-only scratch per device from call to call (_scratch): bpr_exact_f64, MtSampler.step, MtPointwiseRatioSampler.step, score_topk,
 score_topk_tc, bpr_step_sampled_f32 (the schedule prefetch keeps two schedule slots of its own), gram_f64, eval_topk,
-eval_topk_metrics, eval_fairness, vae_train_step, gemm_bf16_tn / gemm_bf16 (split-K partials), cml_grad_f32 and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
+eval_topk_metrics, eval_fairness, vae_train_step, gemm_bf16_tn / gemm_bf16 (split-K partials), cml_grad_f32, dmf_head_f32 and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
 device.  Those ops must not run concurrently on two streams of the same device from one process.
 """
 import ctypes
@@ -339,6 +339,49 @@ class MtSampler:
         _call("eb_mt_sampler_step", u, _ptr(self.state), self.n_users, self.n_items, _ptr(self.indptr), _ptr(self.set_indices),
               _ptr(self.sorted_indices), events, _ptr(u), _ptr(i), _ptr(j), _ptr(ws), ws.numel())
         return u, i, j
+
+
+class MtPointwiseRatioSampler:
+    """Device replay of the reference's pointwise ratio sampler (samplers/pointwise_pos_neg_ratio_ratings_sampler.py,
+    DMF's): (user, item, rating) samples, `neg_ratio` negatives (rating 0) per positive on average, from one MT19937 stream
+    seeded at construction.  indptr/set_indices/set_ratings: the reference's `_ui_dict` in list(set(...)) order with each
+    entry's train rating; sorted_indices: the same CSR with rows sorted.  The MT state persists across calls; the list
+    permutation persists within an epoch, and epoch() resets it as each Sampler.step() call does.  step(events) draws
+    the next `events` samples of the current epoch in windows of at most `window` samples (scratch ~2.3 KB per window
+    sample at neg_ratio 5); the samples do not depend on the window."""
+
+    WINDOW = 1 << 17
+
+    def __init__(self, n_users, n_items, indptr, set_indices, set_ratings, sorted_indices, neg_ratio, seed=42):
+        _need_cuda(indptr, set_indices, set_ratings, sorted_indices)
+        assert indptr.dtype == torch.int64 and set_indices.dtype == torch.int32 and sorted_indices.dtype == torch.int32
+        assert set_ratings.dtype == torch.float32 and set_ratings.numel() == set_indices.numel()
+        if not 0 <= int(neg_ratio) <= 15:
+            raise ValueError(f"neg_ratio={neg_ratio}: the device sampler replays lists of at most 16 slots (0 <= neg_ratio <= 15)")
+        self.n_users, self.n_items, self.neg_ratio = n_users, n_items, int(neg_ratio)
+        self.indptr, self.set_indices, self.set_ratings, self.sorted_indices = indptr, set_indices, set_ratings, sorted_indices
+        self.state = torch.empty(625, dtype=torch.int32, device=indptr.device)
+        self.list_pos = torch.empty(1, dtype=torch.int32, device=indptr.device)
+        _call("eb_mt_seed", indptr, _ptr(self.state), seed)
+        self.epoch()
+
+    def epoch(self):
+        """Start an epoch: the list is [0] * neg_ratio + [1] again."""
+        self.list_pos.fill_(self.neg_ratio)
+
+    def step(self, events, window=None):
+        dev = self.state.device
+        window = int(window or self.WINDOW)
+        u = torch.empty(events, dtype=torch.int32, device=dev); i = torch.empty_like(u)
+        r = torch.empty(events, dtype=torch.float32, device=dev)
+        ws = _scratch("mt_pointwise", lib().eb_mt_pointwise_ratio_workspace_bytes(min(events, window), self.n_users,
+                                                                                   self.neg_ratio), dev)
+        for s in range(0, events, window):
+            n = min(window, events - s)
+            _call("eb_mt_pointwise_ratio_step", u, _ptr(self.state), _ptr(self.list_pos), self.n_users, self.n_items,
+                  _ptr(self.indptr), _ptr(self.set_indices), _ptr(self.set_ratings), _ptr(self.sorted_indices),
+                  self.neg_ratio, n, _ptr(u[s:]), _ptr(i[s:]), _ptr(r[s:]), _ptr(ws), ws.numel())
+        return u, i, r
 
 
 def score_topk(U, V, bias, d, k, mask_indptr=None, mask_indices=None, users=None, user_begin=0, n_sel=None):
@@ -1569,3 +1612,50 @@ def cml_score_operands_f32(Gu, Gi, Bi, n_users, n_items):
     _call("eb_cml_score_operands_f32", Gu, _ptr(Gu), _ptr(Gi), _ptr(Bi), Gu.stride(0), n_users, n_items, _ptr(U2), _ptr(item_off),
           _ptr(user_off))
     return U2, item_off, user_off
+
+
+# ---------------------------------------------------------------- DMF (csrc/dmf.cu)
+def dmf_sparse_fwd(W1, b1, indptr, indices, values, rows, h1, relu):
+    """h1[b] = act(X[rows[b]] . W1 + b1), X the CSR (indptr, indices, values); W1 [n_cols][H] fp32."""
+    _need_cuda(W1, b1, indptr, indices, values, rows, h1)
+    _chk_idx(rows)
+    assert W1.is_contiguous() and h1.stride(1) == 1 and values.dtype == torch.float32
+    _call("eb_dmf_sparse_fwd_f32", W1, _ptr(W1), _ptr(b1), W1.shape[1], _ptr(indptr), _ptr(indices), _ptr(values), _ptr(rows),
+          rows.numel(), 1 if relu else 0, _ptr(h1), h1.stride(0))
+    return h1
+
+
+def dmf_sparse_bwd(dW1, indptr, indices, values, rows, dpre1):
+    """dW1 += X[rows]^T . dpre1."""
+    _need_cuda(dW1, indptr, indices, values, rows, dpre1)
+    _chk_idx(rows)
+    assert dW1.is_contiguous() and dpre1.stride(1) == 1
+    _call("eb_dmf_sparse_bwd_f32", dW1, _ptr(dW1), dW1.shape[1], _ptr(indptr), _ptr(indices), _ptr(values), _ptr(rows),
+          rows.numel(), _ptr(dpre1), dpre1.stride(0))
+
+
+def dmf_head_f32(U, V, F, label, max_rating, cosine, loss, dU, dV, prob=None):
+    """One batch of DMF's head (model.py:76-77, 93-105): batch-axis cosine (or dot), clipped BCE against label /
+    max_rating; `loss` (fp64 [1]) gets the batch mean added, dU / dV the gradients.  U, V, dU, dV [B][ld] fp32."""
+    _need_cuda(U, V, label, loss, dU, dV, prob)
+    assert U.stride(0) == V.stride(0) and dU.stride(0) == dV.stride(0) and U.stride(1) == 1 and dU.stride(1) == 1
+    B = U.shape[0]
+    ws = _scratch("dmf_head", lib().eb_dmf_head_workspace_bytes(B, F), U.device)
+    _call("eb_dmf_head_f32", U, _ptr(U), _ptr(V), U.stride(0), F, B, _ptr(label), float(max_rating), 1 if cosine else 0,
+          _ptr(loss), _ptr(dU), _ptr(dV), dU.stride(0), _ptr(prob), _ptr(ws), ws.numel())
+
+
+def dmf_score_operands_f32(Uo, Vo, F, block, cosine):
+    """(Uh, Vh, Vh_last) of get_recs (model.py:106-121) for user blocks of `block`: each block's users scaled by the block's
+    column norms, items by 1 / sqrt(block V^2) (Vh_last: the short last block's size; None when there is none), row
+    stride padded_dim(F).  The dot-product scorers on (Uh rows of a block, Vh of that block) give the reference's scores."""
+    _need_cuda(Uo, Vo)
+    n_users, n_items = Uo.shape[0], Vo.shape[0]
+    ld = padded_dim(F)
+    Uh = torch.empty((n_users, ld), dtype=torch.float32, device=Uo.device)
+    Vh = torch.empty((n_items, ld), dtype=torch.float32, device=Uo.device)
+    bl = min(int(block), n_users)
+    Vl = torch.empty_like(Vh) if cosine and n_users % bl else None
+    _call("eb_dmf_score_operands_f32", Uo, _ptr(Uo), Uo.stride(0), _ptr(Vo), Vo.stride(0), F, n_users, n_items, bl,
+          1 if cosine else 0, _ptr(Uh), _ptr(Vh), _ptr(Vl), ld)
+    return Uh, Vh, Vl

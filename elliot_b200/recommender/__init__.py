@@ -18,3 +18,4 @@ from .nonneg_mf import NonNegMF, NonNegMFModel  # noqa: F401
 from .unpersonalized import MostPop, Random, MostPopLists, RandomLists  # noqa: F401
 from .rating_mf import SVDpp, FunkSVD, RatingMFModel  # noqa: F401
 from .cml import CML, CMLModel  # noqa: F401
+from .dmf import DMF, DMFModel  # noqa: F401

@@ -169,6 +169,20 @@ int eb_mt_sampler_step(uint32_t *state, int32_t n_users, int32_t n_items,
                        const int64_t *indptr, const int32_t *set_indices, const int32_t *sorted_indices,
                        int64_t events, int32_t *out_u, int32_t *out_i, int32_t *out_j,
                        void *workspace, size_t workspace_bytes, void *stream);
+/* Pointwise ratio sampler (dataset/samplers/pointwise_pos_neg_ratio_ratings_sampler.py, DMF): the same MT19937
+ * stream.  Each sample: u = randint(n_users); np.random.shuffle of the list [0]*neg_ratio + [1]; if the list's
+ * first slot holds the 1, a positive set_indices[randint(lui)] of u's row with its set_ratings value, else a
+ * negative randint(n_items) redrawn while it is a train item, rating 0.  *list_pos (device int32) is the position
+ * of the 1 in the list: the caller sets it to neg_ratio at each epoch's start (the reference rebuilds the list per
+ * step() call) and the call leaves it where the last sample left it, as it advances the MT state by the draws
+ * consumed.  0 <= neg_ratio <= 15.  Returns EB_ERR_DATA if a sampled user owns every item or none.
+ * workspace: eb_mt_pointwise_ratio_workspace_bytes(events, n_users, neg_ratio) bytes, about 2.3 KB per event at
+ * neg_ratio 5: call in windows (the stream does not depend on how it is windowed). */
+size_t eb_mt_pointwise_ratio_workspace_bytes(int64_t events, int32_t n_users, int32_t neg_ratio);
+int eb_mt_pointwise_ratio_step(uint32_t *state, int32_t *list_pos, int32_t n_users, int32_t n_items,
+                               const int64_t *indptr, const int32_t *set_indices, const float *set_ratings,
+                               const int32_t *sorted_indices, int32_t neg_ratio, int64_t events, int32_t *out_u,
+                               int32_t *out_i, float *out_r, void *workspace, size_t workspace_bytes, void *stream);
 /* raw tempered 32-bit outputs (testing the generator against numpy) */
 int eb_mt_raw(uint32_t *state, uint32_t *out, int64_t n, void *stream);
 
@@ -851,6 +865,35 @@ int eb_cml_grad_f32(const float *Gu, const float *Gi, const float *Bi, float *dG
                     float *terms, double *loss, void *workspace, size_t workspace_bytes, void *stream);
 int eb_cml_score_operands_f32(const float *Gu, const float *Gi, const float *Bi, int ld, int32_t n_users, int32_t n_items,
                               float *U2, float *item_off, float *user_off, void *stream);
+
+/* ------------------------------------------------------------------------
+ * DMF (neural/DMF/deep_matrix_factorization_model.py), fp32.
+ * eb_dmf_sparse_fwd_f32: h1[b][:H] = act(sum_p values[p] W1[indices[p]][:] + b1) over the CSR row rows[b] (act = ReLU
+ *   if relu, else none); W1 [n_cols][H], H a multiple of 4 up to 1024, 16-byte aligned; row stride ldh; B < 2^31.
+ * eb_dmf_sparse_bwd_f32: dW1[indices[p]][:] += values[p] dpre1[b][:] over the same rows (vector atomics).
+ * eb_dmf_head_f32: one batch of B (user, item) tower outputs U, V [B][ld] (F columns) and ratings label[B].
+ *   cosine: u^ = l2_normalize(U, axis 0) (each column over the batch: x / sqrt(max(sum_b x^2, 1e-12))), same for V;
+ *   else u^ = U, v^ = V.  o_b = sum_f u^ v^, p_b = clip(o_b, 1e-7, 1 - 1e-7) (float32 bounds, as Keras), y_b = label_b / max_rating;
+ *   loss (device double[1]) += mean_b -(y log(p + 1e-7) + (1 - y) log(1 - p + 1e-7)) (fp64, fixed order);
+ *   dU, dV [B][ldg] = d mean / d(U, V) (clip passes the gradient on the closed interval; a column below the 1e-12
+ *   floor gets only the direct term).  prob (optional) [B] = o.  F <= 256.  workspace: eb_dmf_head_workspace_bytes(B, F).
+ * eb_dmf_score_operands_f32: tower outputs Uo [n_users] (stride ldu), Vo [n_items] (stride ldv) -> Uh [n_users][ld]
+ *   with each user block [k block, (k+1) block) normalised by its own column norms, Vh [n_items][ld] = V / sqrt(max(
+ *   block V^2, 1e-12)) and, when n_users % block != 0, Vh_last the same for the short last block (get_recs).  cosine = 0:
+ *   Uh, Vh are Uo, Vo.  Padding columns [F, ld) are zero.  block > n_users means one block of every user.
+ * ------------------------------------------------------------------------ */
+int eb_dmf_sparse_fwd_f32(const float *W1, const float *b1, int H, const int64_t *indptr, const int32_t *indices,
+                          const float *values, const int32_t *rows, int64_t B, int relu, float *h1, int64_t ldh,
+                          void *stream);
+int eb_dmf_sparse_bwd_f32(float *dW1, int H, const int64_t *indptr, const int32_t *indices, const float *values,
+                          const int32_t *rows, int64_t B, const float *dpre1, int64_t ldd, void *stream);
+size_t eb_dmf_head_workspace_bytes(int64_t B, int F);
+int eb_dmf_head_f32(const float *U, const float *V, int64_t ld, int F, int64_t B, const float *label, float max_rating,
+                    int cosine, double *loss, float *dU, float *dV, int64_t ldg, float *prob, void *workspace,
+                    size_t workspace_bytes, void *stream);
+int eb_dmf_score_operands_f32(const float *Uo, int64_t ldu, const float *Vo, int64_t ldv, int F, int32_t n_users,
+                              int32_t n_items, int64_t block, int cosine, float *Uh, float *Vh, float *Vh_last, int64_t ld,
+                              void *stream);
 
 /* ------------------------------------------------------------------------
  * MostPop and Random (recommender/unpersonalized/most_popular/most_popular.py, random_recommender/Random.py).
