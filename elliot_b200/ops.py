@@ -5,7 +5,7 @@ CUDA device — there is no CPU path.
 Streams: every op launches on torch's CURRENT stream of the tensors' device.  The C ABI never allocates, so these ops
 keep grow-only scratch per device from call to call (_scratch): bpr_exact_f64, MtSampler.step, MtPointwiseRatioSampler.step, score_topk,
 score_topk_tc, bpr_step_sampled_f32 (the schedule prefetch keeps two schedule slots of its own), gram_f64, eval_topk,
-eval_topk_metrics, eval_fairness, vae_train_step, gemm_bf16_tn / gemm_bf16 (split-K partials), cml_grad_f32, dmf_head_f32 and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
+eval_topk_metrics, eval_fairness, vae_train_step, gemm_bf16_tn / gemm_bf16 (split-K partials), cml_grad_f32, dmf_head_f32, autorec_decoder_f32 and RandomStream.draws; mf_pointwise_step_f32 keeps a global-bias accumulator per
 device.  Those ops must not run concurrently on two streams of the same device from one process.
 """
 import ctypes
@@ -1659,3 +1659,22 @@ def dmf_score_operands_f32(Uo, Vo, F, block, cosine):
     _call("eb_dmf_score_operands_f32", Uo, _ptr(Uo), Uo.stride(0), _ptr(Vo), Vo.stride(0), F, n_users, n_items, bl,
           1 if cosine else 0, _ptr(Uh), _ptr(Vh), _ptr(Vl), ld)
     return Uh, Vh, Vl
+
+
+# ---------------------------------------------------------------- UserAutoRec / ItemAutoRec (csrc/autorec.cu)
+def autorec_decoder_f32(indptr, indices, values, rows, h, W2, b2, act, loss, dW2, db2, dpre1, scale=None, max_entries=None):
+    """One training step's decoder and its backward over the observed entries of the CSR rows `rows`
+    (userautorec_model.py:92-107): `loss` (fp64 [1]) gets scale sum e^2 added, dW2 / db2 the decoder gradients (added),
+    dpre1 [B][H] the gradient at the encoder's pre-activation (written).  act 0 = linear, 1 = sigmoid; scale defaults to
+    1 / B; max_entries (the most entries the rows can hold) defaults to the CSR's nnz, which distinct rows never pass."""
+    _need_cuda(indptr, indices, values, rows, h, W2, b2, loss, dW2, db2, dpre1)
+    _chk_idx(rows, indices)
+    assert W2.is_contiguous() and dW2.is_contiguous() and h.stride(1) == 1 and dpre1.stride(1) == 1
+    assert values.dtype == torch.float32 and loss.dtype == torch.float64
+    B, H = rows.numel(), W2.shape[1]
+    if max_entries is None:
+        max_entries = indices.numel()
+    ws = _scratch("autorec", lib().eb_autorec_decoder_workspace_bytes(B, H, max_entries), W2.device)
+    _call("eb_autorec_decoder_f32", W2, _ptr(indptr), _ptr(indices), _ptr(values), _ptr(rows), B, max_entries, _ptr(h),
+          h.stride(0), _ptr(W2), _ptr(b2), H, int(act), float(1.0 / max(B, 1) if scale is None else scale), _ptr(dW2),
+          _ptr(db2), _ptr(dpre1), dpre1.stride(0), _ptr(loss), _ptr(ws), ws.numel())

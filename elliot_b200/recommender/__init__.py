@@ -19,3 +19,4 @@ from .unpersonalized import MostPop, Random, MostPopLists, RandomLists  # noqa: 
 from .rating_mf import SVDpp, FunkSVD, RatingMFModel  # noqa: F401
 from .cml import CML, CMLModel  # noqa: F401
 from .dmf import DMF, DMFModel  # noqa: F401
+from .autorec import UserAutoRec, ItemAutoRec, AutoRecModel  # noqa: F401

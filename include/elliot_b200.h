@@ -896,6 +896,25 @@ int eb_dmf_score_operands_f32(const float *Uo, int64_t ldu, const float *Vo, int
                               void *stream);
 
 /* ------------------------------------------------------------------------
+ * UserAutoRec / ItemAutoRec (neural/UserAutoRec/userautorec_model.py, neural/ItemAutoRec/itemautorec_model.py), fp32.
+ * eb_autorec_decoder_f32: one training step's decoder and its backward over the OBSERVED entries of the batch rows
+ *   rows[B] of the CSR (indptr, indices, values).  h [B][ldh] is the encoder output after its sigmoid, W2 [n_out][H] the
+ *   decoder kernel stored output-major (Keras's [H][n_out] transposed), b2 [n_out]; act 0 = linear, 1 = sigmoid; scale =
+ *   1 / B.  For every entry p of row rows[b], i = indices[p], x = values[p]:
+ *     o = h_b . W2[i] + b2[i], r = act(o), e = x - r;  loss (device double[1]) += scale e^2 (fp64);
+ *     g = -2 scale e act'(o);  dW2[i] += g h_b, db2[i] += g (vector / scalar reductions);  dh_b += g W2[i];
+ *   then dpre1 [B][ldd] = dh ⊙ h ⊙ (1 - h) (an empty row gets 0).  dpre1 and the loss are combined in a fixed order (they
+ *   do not depend on scheduling); dW2 / db2 may differ in the last bits from run to run.  H a multiple of 4 in [4, 1024];
+ *   h, W2, dW2, dpre1 16-byte aligned.  The rows' entries must total at most max_entries (distinct rows of the CSR: its
+ *   nnz).  workspace: eb_autorec_decoder_workspace_bytes(B, H, max_entries).  No host synchronisation.
+ * ------------------------------------------------------------------------ */
+size_t eb_autorec_decoder_workspace_bytes(int64_t B, int H, int64_t max_entries);
+int eb_autorec_decoder_f32(const int64_t *indptr, const int32_t *indices, const float *values, const int32_t *rows, int64_t B,
+                           int64_t max_entries, const float *h, int64_t ldh, const float *W2, const float *b2, int H, int act,
+                           float scale, float *dW2, float *db2, float *dpre1, int64_t ldd, double *loss, void *workspace,
+                           size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------
  * MostPop and Random (recommender/unpersonalized/most_popular/most_popular.py, random_recommender/Random.py).
  * The train CSR indptr [n_users + 1] / train (each row sorted ascending) is also the mask: a user's train items are
  * never listed.  Output row q is user users[q], or user_begin + q when users is NULL.
