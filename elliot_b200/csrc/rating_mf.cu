@@ -5,7 +5,8 @@
 //                            SVD++ user vector, for a training batch or for every user before scoring
 //   eb_rating_mf_step_f32    ONE fused kernel per batch: gather -> predict (z.q + b_u + b_i [+ g]) -> squared error -> loss ->
 //                            vector-atomic scatter of dQ, dP, db_u, db_i, dg and, for SVD++, dY_j += e q / |N(u)| over the
-//                            user's train row; the dense Keras Adam (eb_adam_dense_f32) follows
+//                            user's train row; the dense Keras Adam (eb_adam_dense_f32) follows.  b_u / b_i are
+//                            optional (MF has neither)
 //   eb_score_pairs_f32       the score of every (user, relevant item) entry of a CSR: the values the user's full list
 //                            gives those items (-inf for a train item), for the rating metrics
 //   eb_add_row_offset_f32    adds b_u (+ g) to the top-k values: a per-user constant changes no ranking, so the scoring
@@ -83,12 +84,12 @@ __global__ void __launch_bounds__(256) step_kernel(const float *__restrict__ P, 
         float part = f4_dot(z, q);
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
-        const float d = part + __ldg(bu + uu) + __ldg(bi + ii) + gv - label[w];
+        const float d = part + (bu ? __ldg(bu + uu) : 0.f) + (bi ? __ldg(bi + ii) : 0.f) + gv - label[w];
         const float e = 2.f * d * invn;                                   // d (mean_B (out - y)^2) / d out
         if (lane == 0) {
             acc_loss += (double)d * (double)d;
-            red_add_f32(dbu + uu, e);
-            red_add_f32(dbi + ii, e);
+            if (dbu) red_add_f32(dbu + uu, e);
+            if (dbi) red_add_f32(dbi + ii, e);
             acc_g += e;
         }
         if (on) {
@@ -219,7 +220,8 @@ extern "C" int eb_rating_mf_step_f32(const float *P, const float *Q, int64_t ld,
                                      const float *Z, int64_t ldz, const int64_t *indptr, const int32_t *indices, const int32_t *u,
                                      const int32_t *it, const float *label, int64_t n, int64_t mean_over, float *dP, float *dQ,
                                      float *dY, float *dbu, float *dbi, float *dg, double *loss, void *stream) {
-    EB_ARG(P && Q && bu && bi && u && it && label && dP && dQ && dbu && dbi, "null pointer");
+    EB_ARG(P && Q && u && it && label && dP && dQ, "null pointer");
+    EB_ARG((bu == nullptr) == (dbu == nullptr) && (bi == nullptr) == (dbi == nullptr), "bu and dbu, bi and dbi go together");
     EB_ARG(rows_ok(f, ld) && mean_over >= 1 && n >= 0, "f must be a multiple of 4, <= 128, with ld >= f a multiple of 4");
     EB_ARG((g == nullptr) == (dg == nullptr), "g and dg go together");
     EB_ARG((Z == nullptr) == (dY == nullptr), "Z (the batch's implicit means) and dY go together");

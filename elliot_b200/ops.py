@@ -1582,6 +1582,52 @@ def rating_error_sums(scores, ratings, items):
     return out
 
 
+# ---------------------------------------------------------------- PMF / LMF / FM labels (csrc/pointwise_mf.cu)
+PMF_MSE, LMF_LOGPOST = 0, 1
+
+
+def pointwise_mf_step_f32(P, Q, f, u, it, label, dQ, kind, dP=None, bu=None, bi=None, dbi=None, alpha=0.0, lam=0.0, loss=None,
+                          mean_over=None):
+    """Batch gradient of PMF's mean squared error of sigmoid(p.q) (kind PMF_MSE: into dP, dQ) or of LMF's summed log
+    posterior of p.q + b_u + b_i with lam (|p|^2 + |q|^2) / 2 (kind LMF_LOGPOST: item side only, into dQ, dbi); `loss`
+    (fp64) gets the batch loss added."""
+    _need_cuda(P, Q, u, it, label, dQ, dP, bu, bi, dbi, loss)
+    _chk_idx(u, it)
+    assert P.stride(0) == Q.stride(0) == dQ.stride(0) and (dP is None or dP.stride(0) == P.stride(0))
+    _call("eb_pointwise_mf_step_f32", P, _ptr(P), _ptr(Q), P.stride(0), f, _ptr(bu), _ptr(bi), _ptr(u), _ptr(it), _ptr(label),
+          u.numel(), int(kind), int(mean_over) if mean_over else max(int(u.numel()), 1), float(alpha), float(lam), _ptr(dP),
+          _ptr(dQ), _ptr(dbi), _ptr(loss))
+
+
+def adagrad_rows_f32(var, acc, grad, rows, stamp, step, lr, width=None, bvar=None, bacc=None, bgrad=None, eps=1e-7):
+    """TF's sparse Adagrad on every distinct row listed in `rows` (int32, repeats allowed), once, then those gradient rows
+    (and bias entries) cleared.  stamp: int64 [n_rows] zeros at the start, kept with the tables; step: > every step this
+    stamp table has seen."""
+    _need_cuda(var, acc, grad, rows, stamp, bvar, bacc, bgrad)
+    _chk_idx(rows)
+    assert var.stride(0) == acc.stride(0) == grad.stride(0) and var.stride(1) == 1 and stamp.dtype == torch.int64
+    _call("eb_adagrad_rows_f32", var, _ptr(var), _ptr(acc), _ptr(grad), var.stride(0), var.shape[1] if width is None else width,
+          _ptr(bvar), _ptr(bacc), _ptr(bgrad), _ptr(rows), rows.numel(), _ptr(stamp), int(step), float(lr), float(eps))
+
+
+def rating_labels_(indptr, indices, ratings, u, it, label):
+    """label[s] <- the train rating of (u[s], it[s]) for every positive (label != 0) sample, in place; `ratings` float32
+    aligned with the sorted train CSR `indices`."""
+    _need_cuda(indptr, indices, ratings, u, it, label)
+    _chk_idx(u, it)
+    assert ratings.dtype == torch.float32 and ratings.numel() == indices.numel() and label.dtype == torch.float32
+    _call("eb_rating_labels_f32", indptr, _ptr(indptr), _ptr(indices), _ptr(ratings), _ptr(u), _ptr(it), _ptr(label), u.numel())
+    return label
+
+
+def sigmoid_scores_(x):
+    """sigmoid of every score of x in place; -inf (a masked item) and NaN (outside the catalogue) stay as they are."""
+    _need_cuda(x)
+    assert x.is_contiguous() and x.dtype == torch.float32
+    _call("eb_sigmoid_scores_f32", x, _ptr(x), x.numel())
+    return x
+
+
 # ---------------------------------------------------------------- CML (csrc/cml.cu)
 def cml_grad_f32(Gu, Gi, Bi, dGu, dGi, dBi, d, tu, ti, tj, l_w, l_b, margin, loss=None, terms=None):
     """Batch gradient of the CML loss (CML_model.py:59-98, the reference's B x B broadcast, counted by sorting) into dense

@@ -16,7 +16,8 @@ from .pure_svd import PureSVD, PureSVDModel  # noqa: F401
 from .slope_one import SlopeOne, SlopeOneModel  # noqa: F401
 from .nonneg_mf import NonNegMF, NonNegMFModel  # noqa: F401
 from .unpersonalized import MostPop, Random, MostPopLists, RandomLists  # noqa: F401
-from .rating_mf import SVDpp, FunkSVD, RatingMFModel  # noqa: F401
+from .rating_mf import SVDpp, FunkSVD, MF, PMF, FM, RatingMFModel  # noqa: F401
 from .cml import CML, CMLModel  # noqa: F401
 from .dmf import DMF, DMFModel  # noqa: F401
 from .autorec import UserAutoRec, ItemAutoRec, AutoRecModel  # noqa: F401
+from .logistic_mf import LMF, LMFModel  # noqa: F401

@@ -824,6 +824,7 @@ int eb_nnmf_row_update_f64(const int64_t *indptr, const int32_t *cols, const int
  *   for no global bias; loss += (out - y)^2 / mean_over (fp64 accumulator); the gradient e = 2 (out - y) / mean_over is
  *   added (vector atomics) to dQ[i] (e z), dP[u] (e q_i), dbu[u], dbi[i], dg[0] and, when dY is given (with Z and the train
  *   CSR), to dY[j] (e q_i / |N(u)|) for every j of u's train row.  The tables the dense Keras Adam then applies.
+ *   bu / dbu (and bi / dbi) may both be NULL: no such bias term (MF, out = p_u.q_i).
  * eb_score_pairs_f32: for every user w < n_users and relevant entry k of its row (rel CSR, rel_items -1 outside the
  *   catalogue): out[k] = (U[w].V[item] + item_bias[item]) + (user_off[w] + global_off[0]) (each term optional), -inf when
  *   item is in w's mask row (sorted), NaN when item = -1.  One warp per user.
@@ -847,6 +848,38 @@ int eb_add_row_offset_f32(float *x, int64_t rows, int cols, int64_t ldx, const f
                           void *stream);
 int eb_rating_error_sums_f64(const float *scores, const double *ratings, const int32_t *items, int64_t n, double *out,
                              void *stream);
+
+/* ------------------------------------------------------------------------
+ * PMF and LMF (latent_factor_models/PMF/probabilistic_matrix_factorization_model.py,
+ * LogisticMF/logistic_matrix_factorization_model.py) and FM's labels (FM/factorization_machine.py without side
+ * information; MF and FM otherwise train on eb_rating_mf_step_f32).  fp32 tables, row stride ld (multiple of 4),
+ * f % 4 == 0, f <= 128.
+ * eb_pointwise_mf_step_f32: one fused kernel per batch; per sample s with p = P[u], q = Q[i]:
+ *   kind 0 (PMF): o = sigmoid(p.q); loss += (o - y)^2 / mean_over; e = 2 (o - y) o (1 - o) / mean_over is added as e p to
+ *     dQ[i] and e q to dP[u] (bu, bi, dbi unused).
+ *   kind 1 (LMF): x = p.q + bu[u] + bi[i]; loss += -(alpha y x - (1 + alpha y) softplus(x)) + lambda (|p|^2 + |q|^2) / 2;
+ *     c = sigmoid(x) (1 + alpha y) - alpha y is added as c p + lambda q to dQ[i] and c to dbi[i]; dP must be NULL (no user
+ *     row is ever updated).  softplus and sigmoid are evaluated in overflow-free forms (finite for any finite x).
+ *   loss (fp64, optional) gets the batch's sum added.  Vector atomics: dQ / dP / dbi may differ in the last bits from run to
+ *   run.  No host synchronisation.
+ * eb_adagrad_rows_f32: TF's sparse Adagrad on the rows listed in rows[n] (repeats allowed): every distinct row r is updated
+ *   exactly once, acc += g^2; var -= g lr / (sqrt(acc) + eps) on columns 0 .. width-1 of var / acc / grad (row stride ld),
+ *   and the same on element r of bvar / bacc / bgrad (all three NULL: no bias), then its gradient is cleared.  A row is
+ *   claimed by swapping `step` into stamp[r] (uint64 per row, zero-initialised, step >= 1 strictly increasing from call to
+ *   call on the same stamp table).
+ * eb_rating_labels_f32: for every s with label[s] != 0, label[s] = ratings[p], p the position of it[s] in u[s]'s sorted
+ *   train row (indptr, indices; ratings aligned with indices); the item must be in the row.  Labels equal to 0 stay 0.
+ * eb_sigmoid_scores_f32: x = 1 / (1 + exp(-x)) (eb_sigmoid_inplace's map) for every x except -inf, which stays -inf; NaN
+ *   stays NaN.
+ * ------------------------------------------------------------------------ */
+int eb_pointwise_mf_step_f32(const float *P, const float *Q, int64_t ld, int f, const float *bu, const float *bi, const int32_t *u,
+                             const int32_t *it, const float *label, int64_t n, int kind, int64_t mean_over, float alpha,
+                             float lambda, float *dP, float *dQ, float *dbi, double *loss, void *stream);
+int eb_adagrad_rows_f32(float *var, float *acc, float *grad, int64_t ld, int width, float *bvar, float *bacc, float *bgrad,
+                        const int32_t *rows, int64_t n, uint64_t *stamp, uint64_t step, float lr, float eps, void *stream);
+int eb_rating_labels_f32(const int64_t *indptr, const int32_t *indices, const float *ratings, const int32_t *u, const int32_t *it,
+                         float *label, int64_t n, void *stream);
+int eb_sigmoid_scores_f32(float *x, int64_t n, void *stream);
 
 /* ------------------------------------------------------------------------
  * CML (latent_factor_models/CML/CML_model.py:59-106), fp32 tables Gu, Gi (row stride ld, one of 8..256), Bi.
