@@ -1724,3 +1724,76 @@ def autorec_decoder_f32(indptr, indices, values, rows, h, W2, b2, act, loss, dW2
     _call("eb_autorec_decoder_f32", W2, _ptr(indptr), _ptr(indices), _ptr(values), _ptr(rows), B, max_entries, _ptr(h),
           h.stride(0), _ptr(W2), _ptr(b2), H, int(act), float(1.0 / max(B, 1) if scale is None else scale), _ptr(dW2),
           _ptr(db2), _ptr(dpre1), dpre1.stride(0), _ptr(loss), _ptr(ws), ws.numel())
+
+
+# ---------------------------------------------------------------- ConvNeuMF (csrc/convneumf.cu)
+def convneumf_widths(channels):
+    """The scorer's packed channel widths: byte l - 1 = c_l."""
+    w = 0
+    for l, c in enumerate(channels):
+        w |= int(c) << (8 * l)
+    return w
+
+
+def convneumf_l1_fwd(U, I, f, pu, pi, L, HL, W1, b1, c1, out):
+    """Level-1 outputs of the pairs (U[pu[p]], I[pi[p]]) into out [n_pairs R_1][c1], Z-order rows; out bf16, or fp32 in
+    the exact_gemm checking mode."""
+    _need_cuda(U, I, pu, pi, W1, b1, out)
+    _chk_idx(pu, pi)
+    assert U.stride(0) == I.stride(0) and out.is_contiguous() and out.dtype in (torch.bfloat16, torch.float32)
+    _call("eb_convneumf_l1_fwd", U, _ptr(U), _ptr(I), U.stride(0), f, _ptr(pu), _ptr(pi), pu.numel(), L, HL, c1, _ptr(W1),
+          _ptr(b1), _ptr(out), 1 if out.dtype == torch.bfloat16 else 0)
+    return out
+
+
+def convneumf_l1_bwd(U, I, f, pu, pi, n_user_reg, L, HL, W1, b1, c1, dx1, l_w, dU, dI, dW1, db1):
+    """Adds the level-1 gradients of the pairs (dW1, db1, dU / dI rows, plus l_w times the rows) from dx1, the gradient at
+    the level-1 outputs."""
+    _need_cuda(U, I, pu, pi, W1, b1, dx1, dU, dI, dW1, db1)
+    _chk_idx(pu, pi)
+    assert U.stride(0) == I.stride(0) == dU.stride(0) == dI.stride(0) and dx1.dtype == torch.float32 and dx1.is_contiguous()
+    _call("eb_convneumf_l1_bwd", U, _ptr(U), _ptr(I), U.stride(0), f, _ptr(pu), _ptr(pi), pu.numel(), int(n_user_reg), L, HL,
+          c1, _ptr(W1), _ptr(b1), _ptr(dx1), float(l_w), _ptr(dU), _ptr(dI), _ptr(dW1), _ptr(db1))
+
+
+def convneumf_head(hL, RL, cL, Wd1, bd1, wd2, bd2, U, I, f, tu, ti, tj, first, n_total, p_drop, seed, l_w, loss, dWd1, dbd1,
+                   dwd2, dbd2, dpre, y_out=None, mask_out=None):
+    """Head, clipped BPR loss and their gradients for the triples (tu, ti, tj), triples first .. first + n of a batch of
+    n_total: see include/elliot_b200.h."""
+    _need_cuda(hL, Wd1, bd1, wd2, bd2, U, I, tu, ti, tj, loss, dWd1, dbd1, dwd2, dbd2, dpre, y_out, mask_out)
+    _chk_idx(tu, ti, tj)
+    assert hL.dtype == torch.float32 and hL.is_contiguous() and dpre.is_contiguous() and loss.dtype == torch.float64
+    _call("eb_convneumf_head", hL, _ptr(hL), int(RL), cL, _ptr(Wd1), _ptr(bd1), _ptr(wd2), _ptr(bd2), _ptr(U), _ptr(I),
+          U.stride(0), f, _ptr(tu), _ptr(ti), _ptr(tj), tu.numel(), int(first), int(n_total), float(p_drop), int(seed),
+          float(l_w), _ptr(loss), _ptr(dWd1), _ptr(dbd1), _ptr(dwd2), _ptr(dbd2), _ptr(dpre), _ptr(y_out), _ptr(mask_out))
+
+
+def convneumf_score_smem_bytes(f, L, HL, channels):
+    return int(lib().eb_convneumf_score_smem_bytes(f, L, HL, convneumf_widths(channels)))
+
+
+def convneumf_score(U, I, f, L, HL, channels, W1, b1, Wp, bp, Wd1, bd1, wd2, bd2, u0, n_ub, n_items, out=None):
+    """Dense fp32 scores [n_ub][n_items] of users u0 .. u0 + n_ub - 1 against every item (dropout off), one fused kernel.
+    Wp: bf16 W_l [c_l][4 c_(l-1)] for l = 2..L back to back (None at L = 1), bp: fp32 b_l back to back."""
+    _need_cuda(U, I, W1, b1, Wp, bp, Wd1, bd1, wd2, bd2, out)
+    assert U.stride(0) == I.stride(0) and (Wp is None or Wp.dtype == torch.bfloat16)
+    if out is None:
+        out = torch.empty((n_ub, n_items), dtype=torch.float32, device=U.device)
+    _call("eb_convneumf_score", U, _ptr(U), _ptr(I), U.stride(0), f, L, HL, convneumf_widths(channels), _ptr(W1), _ptr(b1),
+          _ptr(Wp), _ptr(bp), _ptr(Wd1), _ptr(bd1), _ptr(wd2), _ptr(bd2), int(u0), int(n_ub), int(n_items), _ptr(out),
+          out.stride(0))
+    return out
+
+
+def dense_rank(scores, rel_indptr, rel_items, mask_indptr=None, mask_indices=None, rows=None, row_begin=0):
+    """(n_pos, sum_c) of score_rank for the rows of a dense fp32 score block: row q is user rows[q] (or row_begin + q)."""
+    _need_cuda(scores, rel_indptr, rel_items, mask_indptr, mask_indices, rows)
+    assert scores.dtype == torch.float32 and scores.stride(1) == 1
+    assert rel_indptr.dtype == torch.int64 and rel_items.dtype == torch.int32 and rel_items.is_contiguous()
+    if rows is not None:
+        _chk_idx(rows)
+    n = scores.shape[0]
+    n_pos, sum_c = (torch.empty(n, dtype=torch.int64, device=scores.device) for _ in range(2))
+    _call("eb_dense_rank_f32", scores, _ptr(scores), scores.stride(0), n, scores.shape[1], _ptr(rows), int(row_begin),
+          _ptr(mask_indptr), _ptr(mask_indices), _ptr(rel_indptr), _ptr(_nonempty(rel_items)), _ptr(n_pos), _ptr(sum_c))
+    return n_pos, sum_c

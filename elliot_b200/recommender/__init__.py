@@ -21,3 +21,4 @@ from .cml import CML, CMLModel  # noqa: F401
 from .dmf import DMF, DMFModel  # noqa: F401
 from .autorec import UserAutoRec, ItemAutoRec, AutoRecModel  # noqa: F401
 from .logistic_mf import LMF, LMFModel  # noqa: F401
+from .convneumf import ConvNeuMF, ConvNeuMFModel  # noqa: F401

@@ -975,6 +975,53 @@ int eb_random_draws(uint32_t *state, uint32_t *words, int64_t capacity, int64_t 
 int eb_complement_select(const int32_t *r_in, const int64_t *indptr, const int32_t *train, const int32_t *users,
                          int32_t user_begin, int64_t n_sel, int k, int32_t *out, void *stream);
 
+/* ------------------------------------------------------------------------
+ * ConvNeuMF (neural/ConvNeuMF/convolutional_neural_matrix_factorization_model.py), fp32 tables, kernels and strides 2.
+ * Geometry: f factors, L conv layers, H_L = floor(f / 2^L) >= 1 final positions per axis, f <= 256; level-1 rows per
+ * pair R_1 = H_L^2 4^(L-1), stored in the Z-order of elliot_b200/csrc/convneumf.cu (the four level-(l-1) rows of a
+ * level-l position are consecutive, so level l >= 2 is a GEMM [rows_l][4 c_(l-1)] x [4 c_(l-1)][c_l], K = (da, db, c)).
+ * W1 is Keras's [2][2][1][c1] kernel flattened; channel widths are multiples of 8 in [8, 64].  A pair p is the user row
+ * pu[p] of U and the item row pi[p] of I (row stride ld).
+ * eb_convneumf_l1_fwd: out [n_pairs R_1][c1] = relu'd level-1 values, bf16 (out_bf16) or fp32.
+ * eb_convneumf_l1_bwd: from dx1 [n_pairs R_1][c1] (the gradient at the level-1 outputs) adds dW1, db1 and each pair's
+ *   dU / dI rows (vector reductions), recomputing the ReLU mask; also adds l_w u to pairs below n_user_reg and l_w i to
+ *   every pair (the gradient of l_w l2_loss, once per occurrence).
+ * eb_convneumf_head: triples t < n of a batch of n_total, pairs (tu, ti) at hL rows [t R_L, ...) and (tu, tj) at
+ *   [(n + t) R_L, ...), hL [2 n R_L][cL] the last level's relu'd outputs.  Per pair s = the rows' sum (fixed order),
+ *   y = wd2 . drop(Wd1^T drop(s) + bd1) + bd2 (Wd1 [cL][cL] Keras [in][out]; inverted dropout at rate p_drop, Philox key
+ *   seed, counter first + t for the positive pair and n_total + first + t for the negative); loss (double) +=
+ *   softplus(-clip(y+ - y-, -80, 1e8)) + l_w (|u|^2 + |i|^2 + |j|^2) / 2 (fp64); adds dWd1, dbd1, dwd2, dbd2 and writes
+ *   dpre [2 n R_L][cL], the gradient at the last level's pre-activations.  y_out [2 n_total] and mask_out
+ *   [n_total][2 pairs][2 layers][cL] (the dropout scale of each unit) are optional.
+ * eb_convneumf_score: scores [n_ub][lds] of users u0 .. u0 + n_ub - 1 against every item, dropout off, one fused kernel
+ *   (level 1 on the CUDA cores, levels 2..L on wgmma, nothing but the score leaves the chip; bit-identical reruns).
+ *   widths: byte l - 1 = c_l.  Wp: bf16 W_l [c_l][4 c_(l-1)] for l = 2..L back to back, bp: fp32 b_l back to back.
+ *   eb_convneumf_score_smem_bytes gives its shared memory (0 for a bad geometry; more than 227 KB is refused).
+ * eb_dense_rank_f32: the (n_pos, sum_c) of eb_score_rank_f32 for rows of a dense score block (row q is user rows[q], or
+ *   row_begin + q), with its list and tie rule: items outside the train mask whose score is neither -inf nor NaN, by
+ *   (score desc, item asc).
+ * ------------------------------------------------------------------------ */
+int eb_convneumf_l1_fwd(const float *U, const float *I, int64_t ld, int f, const int32_t *pu, const int32_t *pi,
+                        int64_t n_pairs, int L, int HL, int c1, const float *W1, const float *b1, void *out, int out_bf16,
+                        void *stream);
+int eb_convneumf_l1_bwd(const float *U, const float *I, int64_t ld, int f, const int32_t *pu, const int32_t *pi,
+                        int64_t n_pairs, int64_t n_user_reg, int L, int HL, int c1, const float *W1, const float *b1,
+                        const float *dx1, float l_w, float *dU, float *dI, float *dW1, float *db1, void *stream);
+int eb_convneumf_head(const float *hL, int64_t RL, int cL, const float *Wd1, const float *bd1, const float *wd2,
+                      const float *bd2, const float *U, const float *I, int64_t ld, int f, const int32_t *tu,
+                      const int32_t *ti, const int32_t *tj, int64_t n, int64_t first, int64_t n_total, float p_drop,
+                      uint64_t seed, float l_w, double *loss, float *dWd1, float *dbd1, float *dwd2, float *dbd2,
+                      float *dpre, float *y_out, float *mask_out, void *stream);
+size_t eb_convneumf_score_smem_bytes(int f, int L, int HL, uint64_t widths);
+int eb_convneumf_score(const float *U, const float *I, int64_t ld, int f, int L, int HL, uint64_t widths,
+                       const float *W1, const float *b1, const void *Wp, const float *bp, const float *Wd1,
+                       const float *bd1, const float *wd2, const float *bd2, int u0, int n_ub, int n_items,
+                       float *scores, int64_t lds, void *stream);
+int eb_dense_rank_f32(const float *scores, int64_t lds, int n_rows, int n_items, const int32_t *rows,
+                      int32_t row_begin, const int64_t *mask_indptr, const int32_t *mask_indices,
+                      const int64_t *rel_indptr, const int32_t *rel_items, int64_t *out_n_pos, int64_t *out_sum_c,
+                      void *stream);
+
 #ifdef __cplusplus
 }
 #endif
